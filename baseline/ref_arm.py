@@ -3,7 +3,7 @@
 `Qwen3TTSTalkerForConditionalGeneration` (talker + code predictor, core/models/modeling_qwen3_tts.py) and
 `Qwen3TTSTokenizerV2Decoder` (tokenizer_12hz/modeling_qwen3_tts_tokenizer_v2.py) are imported from the unmodified
 package installed in baseline/_ref (baseline/install_reference.sh) through the three probe-only shims of
-oracle/ref_shims.py, loaded with the SAME seeded synthetic weights as the B200 arm, and driven by the restated
+oracle/ref_shims.py, loaded with the SAME seeded synthetic weights as the GPU arm, and driven by the restated
 generation loop (:1665-1744, :1250-1312 — the reference's HF `generate()` cannot execute under the installed
 transformers 5.5.0, SURVEY §8c): prefill, then per frame 15 code-predictor forwards + sampling + one talker step,
 then `chunked_decode` of the generated frames.  fp32, eager attention, all usable host threads.
@@ -114,7 +114,7 @@ class ReferenceArm:
         toks = []
         for b in range(self.B):
             s = OS.process_logits(logits[b], generated_ids=self.gen[b], **self.lp)
-            s[self.ocfg.codec_eos_token_id] = -np.inf  # fixed horizon (suppress_eos), like the B200 arm
+            s[self.ocfg.codec_eos_token_id] = -np.inf  # fixed horizon (suppress_eos), like the GPU arm
             tok, _ = OS.sample_from_scores(s, do_sample=self.sp.do_sample, u=philox.uniform(self.seed, b, frame, 0))
             self.gen[b].append(int(tok))
             toks.append(tok)

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — hot-path benchmark of the B200-native Qwen3-TTS engine (contract: see the task statement).
+"""bench.py — hot-path benchmark of the H100-native Qwen3-TTS engine.
 
 One "step" = one pass of the hot path over one batch of synthetic utterances of the configuration BASELINE.json
 quotes the metric on (config[2]: Qwen3-TTS-12Hz-1.7B CustomVoice, batch 8, non-streaming):
@@ -8,7 +8,9 @@ quotes the metric on (config[2]: Qwen3-TTS-12Hz-1.7B CustomVoice, batch 8, non-s
     codec decode of the 8 x 125 frames to 24 kHz waveform.
 metric = speech tokens (12.5 Hz frames; x16 for individual codebook tokens) per second, whole job.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
+`--dump-outputs DIR` writes what the last timed GPU step computed (its codes and waveforms) as DIR/<name>.npy, so two
+builds can be compared output for output: the inputs, weights and sampling seeds are fixed.
 N > 1 is launched by torchrun (one rank per GPU, full replica each; the request list is sharded and the waveforms
 gathered by qwen3_tts_b200.parallel.run_data_parallel; `value` is the weak view — B utterances per GPU — and
 `strong_scaling` the fixed-global-batch-32 view).  `--impl reference` times the reference's own modules
@@ -81,7 +83,11 @@ def parse():
     ap.add_argument("--cpu-frames", type=int, default=0, help="frame-steps per CPU sample (0 = sized from the time budget)")
     ap.add_argument("--no-extras", action="store_true", help="skip the side measurements (other batch sizes, 0.6B, encoders)")
     ap.add_argument("--no-parity-check", action="store_true")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's codes and waveforms as DIR/<name>.npy")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    return args
 
 
 def _pin(t):
@@ -112,7 +118,7 @@ def model_cfg(name):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, index):
         self.index = index
@@ -294,7 +300,7 @@ def parity_self_check(eng, cfg, W, embs, trail, pad, dev, frames=4):
             worst, worst_mean = max(worst, float(d.max())), max(worst_mean, float(d.mean()))
     ok = bool(prog[0] == frames and (codes == forced).all() and worst < 0.4 and worst_mean < 0.075)
     return {"ok": ok, "frames": frames, "rows": int(len(embs)), "max_abs_err_over_std": worst, "max_mean_err_over_std": worst_mean,
-            "tolerance": "max < 0.4 std, mean < 0.075 std = 1.5x PyTorch bf16's own gap to the fp32 oracle at these shapes (profiles/r02_tolerance_calibration.txt)", "oracle_s": time.perf_counter() - t0}
+            "tolerance": "max < 0.4 std, mean < 0.075 std = 1.5x PyTorch bf16's own gap to the fp32 oracle at these shapes (tools/calibrate_tolerance.py)", "oracle_s": time.perf_counter() - t0}
 
 
 def decode_probe(eng, q, cfg, args, spk, B, N, dev, greedy=False):
@@ -417,7 +423,7 @@ def hbm_peak():
     peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(peaks_path):
         return float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet 3.35 TB/s (not a measurement)"
 
 
 def main():
@@ -483,9 +489,9 @@ def main():
         emit(out)
         return
 
-    # ------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------ GPU arm
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device (the B200 path has no CPU fallback)")
+        raise SystemExit("bench.py: no CUDA device (the GPU path has no CPU fallback)")
     dev = f"cuda:{local}"
     torch.cuda.set_device(local)
     dist = None
@@ -539,7 +545,7 @@ def main():
         if timed:
             torch.cuda.synchronize()
             t_pre += e0.elapsed_time(e1); t_dec += e1.elapsed_time(e2); t_cod += e2.elapsed_time(e3)
-        return wav
+        return codes, wav
 
     for _ in range(args.warmup):
         step_resident(False)
@@ -549,7 +555,7 @@ def main():
     s0, s1 = ev(), ev()
     s0.record(stream)
     for _ in range(args.steps):
-        wav = step_resident(True)
+        codes, wav = step_resident(True)
     s1.record(stream)
     barrier()
     ms_total = s0.elapsed_time(s1)
@@ -557,6 +563,11 @@ def main():
     fd, n_valid, _ = eng.ar.progress()
     assert fd == N and all(v == N for v in n_valid), (fd, n_valid)
     assert torch.isfinite(wav).all()
+    if args.dump_outputs and rank == 0:
+        # codes [B][N][16] (exact in float32) and waveforms [B][1][N * 1920]: 7.7 MB at the default B=8, N=125
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in (("codes", codes), ("waveform", wav)):
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), t.float().cpu().numpy())
 
     # ---- end-to-end through the public calls: pinned host inputs, H2D + D2H inside the timed region.  The global
     # request list (B per GPU) goes through parallel.run_data_parallel: shard -> synthesize -> gather of waveforms
@@ -646,18 +657,8 @@ def main():
     t_step = (t_dec / args.steps) / N / 1000.0  # s per frame-step (this rank)
     peak, peak_src = hbm_peak()
     achieved = a_bytes / t_step / 1e9
-    # measured DRAM traffic of this kernel from the committed `ncu --set full` capture (profiles/): bytes per
-    # frame-step of the B=8 capture scaled to this launch's frame count; null when no capture of this round exists
-    traffic, traffic_src = None, None
-    try:
-        if args.batch == 8 and args.model == "1.7b":
-            meta = json.load(open(os.path.join(ROOT, "profiles", "r02_decode_kernel_traffic.json")))
-            traffic = float(meta["dram_bytes_per_frame_step"]) * N
-            traffic_src = meta["source"]
-    except Exception:
-        traffic = None
     roof = {"bound": "hbm", "kernel": "q3_step_kernel (fused frame-step)", "achieved": achieved, "peak": peak, "unit": "GB/s",
-            "frac": achieved / peak, "peak_source": peak_src, "traffic": traffic, "traffic_source": traffic_src,
+            "frac": achieved / peak, "peak_source": peak_src,
             "algorithmic_bytes_per_launch": a_bytes * N, "algorithmic_bytes_per_frame_step": a_bytes,
             "no_residency_bytes_per_frame_step": a_stream, "ms_per_frame_step": t_step * 1e3, "mean_context": S_mean}
 

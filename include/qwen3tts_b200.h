@@ -1,5 +1,5 @@
 /*
- * qwen3tts_b200.h — C ABI of the B200-native Qwen3-TTS hot-path library (libqwen3tts_b200.so).
+ * qwen3tts_b200.h — C ABI of the H100-native Qwen3-TTS hot-path library (libqwen3tts_b200.so).
  *
  * The reference (QwenLM/Qwen3-TTS) is pure Python with no FFI/plugin interface (SURVEY.md §8b), so the
  * boundary below is defined at the two narrowest seams of the reference and each entry point cites the

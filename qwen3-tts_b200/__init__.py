@@ -1,4 +1,4 @@
-"""qwen3-tts_b200 — B200-native (sm_100a) hot paths of Qwen3-TTS behind the reference's Python API.
+"""qwen3-tts_b200 — H100-native (sm_90a) hot paths of Qwen3-TTS behind the reference's Python API.
 
 Importable as `qwen3_tts_b200` (see the shim module at the repo root; the directory name carries a hyphen).
 """

@@ -1,4 +1,4 @@
-"""Build libqwen3tts_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Build libqwen3tts_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 import hashlib
 import os
 import subprocess
@@ -8,8 +8,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libqwen3tts_b200.so")
-SOURCES = ["ar_engine.cu", "codec_engine.cu", "codec_encoder.cu", "speaker_encoder.cu", "gemm_sm100.cu"]
-NVCC_FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+SOURCES = ["ar_engine.cu", "codec_engine.cu", "codec_encoder.cu", "speaker_encoder.cu", "gemm_sm90.cu"]
+NVCC_FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-cudart", "shared", "--expt-relaxed-constexpr"]
 
 
@@ -49,7 +49,7 @@ def build(force=False, verbose=False):
         if r.returncode != 0:
             raise RuntimeError(f"nvcc failed for {s}:\n{r.stdout}\n{r.stderr}")
         objs.append(obj)
-    cmd = [_nvcc(), "-shared", "-cudart", "shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB_PATH] + objs
+    cmd = [_nvcc(), "-shared", "-cudart", "shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB_PATH] + objs
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

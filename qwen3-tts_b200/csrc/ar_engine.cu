@@ -1,4 +1,4 @@
-// AR hot path of Qwen3-TTS on B200 (sm_100a): talker + 15-pass code predictor + logits processing + sampling
+// AR hot path of Qwen3-TTS on H100 (sm_90a): talker + 15-pass code predictor + logits processing + sampling
 // + next-embed as ONE persistent cooperative kernel per group of frame-steps.
 //
 // Replaces (reference, paths relative to /root/reference/qwen_tts/core/models/modeling_qwen3_tts.py):
@@ -18,7 +18,7 @@
 //   * rounding points mirror the PyTorch bf16 path (linear outputs, RMSNorm, RoPE, residual adds are
 //     rounded to bf16 exactly where the reference rounds).
 #include "common.cuh"
-#include "gemm_sm100.cuh"
+#include "gemm_sm90.cuh"
 #include "../../include/qwen3tts_b200.h"
 
 #include <cooperative_groups.h>
@@ -98,9 +98,8 @@ __global__ void __launch_bounds__(CTA_THREADS, 1) q3_step_kernel(const __grid_co
 
   // L2 eviction priorities of the weight stream (createpolicy): the talker and the 15 heads are read once per
   // frame-step -> evict_first; the code predictor's layer weights (157 MB) are re-read on each of its 15 passes -> a
-  // fixed, address-hashed fraction of their lines is evict_last, i.e. stays in the 126 MB L2 between passes and is not
-  // re-fetched from HBM.  No effect on time (the kernel is latency-bound); the effect is on DRAM traffic
-  // (profiles/r02_l2_residency.txt).
+  // fixed, address-hashed fraction of their lines is evict_last, i.e. stays in L2 between passes and is not
+  // re-fetched from HBM.  The kernel is latency-bound, so the effect is on DRAM traffic rather than on time.
   uint64_t pol_stream, pol_keep;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol_stream));
   asm volatile("createpolicy.fractional.L2::evict_last.L2::evict_first.b64 %0, %1;" : "=l"(pol_keep) : "f"(P.keep_fraction));
@@ -205,9 +204,10 @@ struct PieceTable {
 struct q3_engine {
   q3_engine_cfg cfg;
   int sm_count = 0;
+  size_t l2_bytes = 0;
   cudaStream_t copy_stream = nullptr;
   std::map<std::string, PackedW> packed;   // GEMV weights
-  std::map<std::string, bf16*> gemm_w;      // plain [N][K] copies of the talker layer weights for the tcgen05 prefill GEMMs
+  std::map<std::string, bf16*> gemm_w;      // plain [N][K] copies of the talker layer weights for the wgmma prefill GEMMs
   bf16 *pf_x = nullptr, *pf_xn = nullptr, *pf_qkv = nullptr, *pf_attn = nullptr, *pf_act = nullptr;
   int *pf_seq = nullptr, *pf_pos = nullptr;
   int pf_cap = 0;
@@ -315,10 +315,11 @@ extern "C" int q3_engine_create(const q3_engine_cfg* cfg, q3_engine** out) {
   Q3_CUDA(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   Q3_CUDA(cudaGetDeviceProperties(&prop, cfg->device));
-  Q3_REQUIRE(prop.major == 10, "this library is built for sm_100a (B200); device is sm_%d%d", prop.major, prop.minor);
+  Q3_REQUIRE(prop.major == 9 && prop.minor == 0, "this library is built for sm_90a (H100); device is sm_%d%d", prop.major, prop.minor);
   q3_engine* e = new q3_engine();
   e->cfg = *cfg;
   e->sm_count = prop.multiProcessorCount;
+  e->l2_bytes = (size_t)prop.l2CacheSize;
   if (const char* g = getenv("Q3_GRID")) {  // experiment knob: persistent grid smaller than the SM count
     const int v = atoi(g);
     if (v >= 8 && v <= e->sm_count) e->sm_count = v;
@@ -376,7 +377,7 @@ extern "C" int q3_engine_load_tensor(q3_engine* e, const char* name, const void*
     Q3_CUDA(cudaGetLastError());
     Q3_CUDA(cudaStreamSynchronize(e->copy_stream));
     e->packed[n] = pw;
-    if (n.rfind("talker.layers.", 0) == 0 || (n == "cp.proj" && cols % 64 == 0)) {  // tcgen05 GEMM operand: [N][K] is already K-major
+    if (n.rfind("talker.layers.", 0) == 0 || (n == "cp.proj" && cols % 64 == 0)) {  // wgmma GEMM operand: [N][K] is already K-major
       Q3_REQUIRE(cols % 64 == 0, "%s: K must be a multiple of 64 for the prefill GEMM", name);
       bf16* g = nullptr;
       if (e->alloc(&g, (size_t)rows * cols)) return 1;
@@ -559,7 +560,7 @@ static int build_programs(q3_engine* e, int B) {
     if (need_packed(e, "cp.proj", Hc, H, &wproj) || need_plain(e, "cp.proj_bias", Hc, &bproj)) return 1;
   }
   // ---- prefill-chunk program: talker layers over the chunk's columns
-  e->prog_layers.clear();  // (prefill runs on the tcgen05 GEMM path, see q3_prefill)
+  e->prog_layers.clear();  // (prefill runs on the wgmma GEMM path, see q3_prefill)
   // ---- prefill-head program: final norm + codec_head on the last token of each row, sample frame-0 codebook-0
   e->prog_head.clear();
   {
@@ -664,7 +665,7 @@ extern "C" int q3_engine_finalize(q3_engine* e) {
                  (int64_t)(c.num_code_groups - 1) * c.cp.vocab_size * c.talker.hidden_size, &p))
     return 1;
   // projection table: passes >= 1 of the code predictor feed small_to_mtp_projection(codec_embedding[j-1](c_j)) (:1281-1283),
-  // a function of the sampled id only -> one tcgen05 GEMM over all (G-1)*Vc embedding rows here, no GEMV phase per pass
+  // a function of the sampled id only -> one wgmma GEMM over all (G-1)*Vc embedding rows here, no GEMV phase per pass
   if (c.has_cp_projection && e->use_proj_tab && e->gemm_w.count("cp.proj") && !e->proj_tab) {
     const int H = c.talker.hidden_size, Hc = c.cp.hidden_size;
     const int rows = (c.num_code_groups - 1) * c.cp.vocab_size;
@@ -721,9 +722,10 @@ extern "C" int q3_engine_finalize(q3_engine* e) {
   e->w_talker_bytes = 2.0 * wt;
   e->w_cp_unique_bytes = 2.0 * (cpl + proj + heads);
   e->w_cp_stream_bytes = 2.0 * ((c.num_code_groups - 1) * (cpl + proj) + heads);
-  // L2 residency of the code predictor's layer weights (re-read on each of its passes): keep ~80 MB of them at
-  // evict_last priority beside the talker's evict_first stream (126 MB L2)
-  if (!getenv("Q3_KEEP_FRACTION")) e->keep_fraction = (float)std::min(1.0, 68e6 / (2.0 * cpl));  // measured: more than ~75 MB of evict_last lines thrash (profiles/r02_l2_residency.txt)
+  // L2 residency of the code predictor's layer weights (re-read on each of its passes): keep a bit over half of the
+  // L2 (27 MB of H100's 50 MB) of them at evict_last priority beside the talker's evict_first stream; much more than
+  // that and the evict_last lines evict each other
+  if (!getenv("Q3_KEEP_FRACTION")) e->keep_fraction = (float)std::min(1.0, 0.54 * (double)e->l2_bytes / (2.0 * cpl));
   e->finalized = true;
   return 0;
 }
@@ -762,7 +764,7 @@ static int launch_program(q3_engine* e, int off, int n, int mode, int max_iters,
   return 0;
 }
 
-// Prefill of `n` prompts (packed back to back in embeds_dev) into the engine slots slots[0..n): tcgen05 GEMMs over all
+// Prefill of `n` prompts (packed back to back in embeds_dev) into the engine slots slots[0..n): wgmma GEMMs over all
 // their tokens at once, K/V into the slots' cache rows, then the head GEMV + the first codebook-0 sample of exactly
 // those rows (admit_mask).  Shared by the static batch (q3_prefill) and by continuous batching (q3_admit).
 static int prefill_rows(q3_engine* e, int n, const int* slots, const void* embeds_dev, const int32_t* lens_host, cudaStream_t stream) {

@@ -12,10 +12,10 @@ using q3ring::RunGeom;
 
 // ------------------------------------------------------------------------------------------------
 // grid barrier.  Two interchangeable implementations (KParams.flags bit 0):
-//   counter (default): release-red on one counter + relaxed poll by thread 0 (arrive -> release ~1.0 us measured).
+//   counter (default): release-red on one counter + relaxed poll by thread 0.
 //   flags            : every CTA owns one epoch word; arrive = st.release of the new epoch, wait = warp 0 polls all
-//                      gridDim words.  Measured SLOWER on B200 (arrive -> release 3-4 us: 148 pollers x 5 lines), kept
-//                      as an A/B knob only (profiles/r02_barrier_ab.txt).
+//                      gridDim words.  Every CTA polls every word, so the release costs grow with the grid;
+//                      kept as an A/B knob only.
 // Polls are RELAXED on purpose: ld.acquire.gpu compiles to LDG.STRONG + CCTL.IVALL (a full L1 invalidation per
 // poll iteration).  Correctness does not need it: every cross-CTA read in this kernel is an L2 access
 // (ld.global.cg / cp.async.cg / cp.async.bulk), the writers released at gpu scope before their arrival became
@@ -147,8 +147,8 @@ __device__ __forceinline__ uint4 lds128(uint32_t addr) {
 // (build_run_table): per CTA and warp the (address, length) of every contiguous run of one program pass; pieces are
 // the <= SB-block chunks of a run.  A refill costs one expect_tx and one cp.async.bulk; the next run's descriptor is
 // loaded a whole run ahead, so nothing is computed and no load latency is exposed on the device.
-// (Measured alternatives, profiles/r02_phase_breakdown.txt: a device-side iterator inside the consumer loop cost
-// ~0.3 us per piece, a dedicated producer warp ~0.7 us per piece of serialised iterator work.)
+// (The alternatives, a device-side iterator inside the consumer loop or a dedicated producer warp, put serialised
+// iterator work in front of every piece.)
 // ------------------------------------------------------------------------------------------------
 struct Ring {
   uint32_t slots;          // shared address of the warp's first slot
@@ -191,7 +191,7 @@ __device__ __forceinline__ void ring_issue(Ring& rg, const KParams& P, int lane,
     const char* src = P.wbase + ((size_t)rg.cur_off << 4);
     // L2 priority of the line fill: pol_stream = evict_first (read once per frame-step), pol_keep = a fixed,
     // address-hashed fraction evict_last (the code predictor's layer weights are re-read on each of its 15 passes:
-    // what stays in L2 is not re-fetched from HBM; measured traffic: profiles/r02_l2_residency.txt)
+    // what stays in L2 is not re-fetched from HBM)
     const uint64_t pol = rg.cur_keep ? pol_keep : pol_stream;
     if (DEV && (P.flags & 4)) bulk_g2s_plain(rg.slots + (uint32_t)(rg.p_slot * rg.SB) * 1024u, src, bytes, bar);
     else bulk_g2s(rg.slots + (uint32_t)(rg.p_slot * rg.SB) * 1024u, src, bytes, bar, pol);
@@ -374,7 +374,7 @@ __device__ __forceinline__ void flush_acc(float (&acc)[NACC][NT][4], float* pp, 
 // The phase body.  `m` is this CTA's meta of the phase (tiles owned, K blocks); the weights arrive through the ring.
 // HID: the kernel instantiation that also captures the per-step hidden states (generate(return_hidden=True)); the
 // default instantiation does not carry that code — the phase loop's instruction footprint is a first-order term
-// (measured: 4.22 -> 4.14 ms per frame-step at B=8 without it).  DEV: the development instantiation with the
+// (it exceeds the instruction cache, so every line it carries costs).  DEV: the development instantiation with the
 // device-timestamp marks and the ablation / A-B knobs of KParams::flags; production kernels carry none of it.
 template <int NT, bool HID, bool DEV>
 __device__ __forceinline__ uint32_t gemv_phase(const Phase& ph, const PMeta m, const KParams& P, Ring& rg, unsigned char* smem,
@@ -455,7 +455,7 @@ __device__ __forceinline__ uint32_t gemv_phase(const Phase& ph, const PMeta m, c
 
     // ---- main loop: this warp's run, piece by piece, out of its ring.  All fragment loads of a piece are issued
     // before its MMAs, and consecutive MMAs go to independent accumulators (NACC sets), so neither the LDS latency
-    // nor the MMA latency serialises (measured before: ~280 cycles per 1 KB block with the naive order)
+    // nor the MMA latency serialises
     {
       constexpr int NACC = NT <= 2 ? 4 : 2;
       float acc[NACC][NT][4];

@@ -1,4 +1,4 @@
-// Row-wise kernels around the tcgen05 prefill GEMMs, and the weight re-packing kernels.
+// Row-wise kernels around the wgmma prefill GEMMs, and the weight re-packing kernels.
 // Part of the ar_engine.cu translation unit (include order: ar_program, ar_gemv, ar_attention, ar_sampler,
 // the persistent kernel in ar_engine.cu, ar_prefill).
 #pragma once
@@ -6,7 +6,7 @@
 namespace {
 
 // ------------------------------------------------------------------------------------------------
-// PREFILL on tensor cores: talker linears are tcgen05 tap-GEMMs (gemm_sm100.cu) over all prompt tokens at once
+// PREFILL on tensor cores: talker linears are wgmma tap-GEMMs (gemm_sm90.cu) over all prompt tokens at once
 // (M = sum of prompt lengths); the row-wise pieces around them are the small kernels below.
 // ------------------------------------------------------------------------------------------------
 __global__ void pf_rmsnorm_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, bf16* __restrict__ y, int rows, int C,

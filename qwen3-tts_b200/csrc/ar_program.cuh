@@ -20,7 +20,7 @@ constexpr int PCOL = 20;         // padded row count of a partial column (bank-c
 // part   : split-K partial sums [warp][seg][col][PCOL] fp32
 // nw     : RMSNorm weights of the current GEMV phase (<= 2048 bf16)
 // rings  : per warp R slots of SB KB, filled by cp.async.bulk (TMA) ahead of the consumer, across phases
-constexpr int SMEM_OPTIN = 232448;             // 227 KB per CTA on sm_100
+constexpr int SMEM_OPTIN = 232448;             // 227 KB per CTA on sm_90
 constexpr int MAX_PHASES = 640;                // phases per program (meta table)
 constexpr int ATT_SMEM = (2 * 2 * 128 + 32 * 2 * 130) * 4 + 2 * 60 * 128 * 2;  // attention: fp32 queries + half-warp partials + 60-row K and V windows
 constexpr int SAMPLER_SMEM = (2 * 4096 + 64 + 256) * 4;
@@ -30,7 +30,7 @@ constexpr int MAX_SLOTS = 8;
 // x-area budget: 16 columns x K <= 2048 for batch classes 1-2 (8 x 4160 B ... 16 x 4160 B), 32 x 4160 B for class 4.  Inputs
 // with a larger K (the down projections) are read un-staged.  Keeping the whole plan of classes 1-2 under 195 KB
 // leaves the SM a 32 KB L1, which is what absorbs the stack traffic of the phase functions (with a 227 KB request
-// every local-memory access is an L2 round trip: measured +0.5 us per phase).
+// every local-memory access is an L2 round trip).
 __host__ __device__ constexpr int x_budget_nt(int nt) { return (nt <= 2 ? 16 : 32) * (2 * 2048 + 64); }
 __host__ __device__ constexpr int part_bytes_nt(int nt) { return NWARPS * 2 * nt * 8 * PCOL * 4; }
 

@@ -1,4 +1,4 @@
-// Qwen3-TTS-Tokenizer-12Hz codec ENCODER on B200 (sm_100a): 24 kHz waveform -> 16 x 12.5 Hz codes.
+// Qwen3-TTS-Tokenizer-12Hz codec ENCODER on H100 (sm_90a): 24 kHz waveform -> 16 x 12.5 Hz codes.
 // Replaces Qwen3TTSTokenizerV2Model.encode (qwen_tts/core/tokenizer_12hz/modeling_qwen3_tts_tokenizer_v2.py:961-991),
 // i.e. transformers' MimiModel._encode_frame (modeling_mimi.py:1455-1488): SEANet encoder (:454-496) -> 8-layer
 // sliding-window transformer (:926-993, :1015-1140) -> stride-2 downsample (:1420-1430) -> split RVQ encode (:1311-1338).
@@ -8,7 +8,7 @@
 // flip cascades down the residual chain.  Activations are [B][C][T] fp32 (time contiguous, the reference's own
 // layout); every Conv1d / Linear is one launch of a register-tiled direct convolution with the preceding ELU, the
 // bias, GELU, LayerScale and the residual add fused in.  It is a first correct version: ~12 GFLOP per 3 s of
-// audio on CUDA cores; moving the strided convolutions onto tcgen05 (tf32) is the follow-up once parity is pinned.
+// audio on CUDA cores; moving the strided convolutions onto wgmma (tf32) is the follow-up once parity is pinned.
 #include "common.cuh"
 #include "../../include/qwen3tts_b200.h"
 
@@ -317,7 +317,7 @@ extern "C" int q3_codec_enc_create(const q3_codec_enc_cfg* cfg, q3_codec_enc** o
   Q3_CUDA(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   Q3_CUDA(cudaGetDeviceProperties(&prop, cfg->device));
-  Q3_REQUIRE(prop.major == 10, "this library is built for sm_100a (B200); device is sm_%d%d", prop.major, prop.minor);
+  Q3_REQUIRE(prop.major == 9 && prop.minor == 0, "this library is built for sm_90a (H100); device is sm_%d%d", prop.major, prop.minor);
   Q3_REQUIRE(cfg->n_ratios >= 1 && cfg->n_ratios <= 8, "1..8 downsampling ratios");
   Q3_REQUIRE(cfg->head_dim % 2 == 0 && cfg->head_dim <= 64, "encoder head_dim must be even and <= 64");
   Q3_REQUIRE(cfg->num_heads * cfg->head_dim == cfg->hidden_size, "num_heads * head_dim must equal hidden_size");

@@ -1,13 +1,13 @@
-// Qwen3-TTS-Tokenizer-12Hz codec DECODER on B200 (sm_100a): codes -> 24 kHz waveform.
+// Qwen3-TTS-Tokenizer-12Hz codec DECODER on H100 (sm_90a): codes -> 24 kHz waveform.
 // Replaces Qwen3TTSTokenizerV2Decoder.forward (qwen_tts/core/tokenizer_12hz/modeling_qwen3_tts_tokenizer_v2.py:869-884).
 //
 // Layout: every activation is channels-last bf16 [B][T][C]; every Conv1d / ConvTranspose1d / Linear is ONE
-// tcgen05 tap-GEMM launch (gemm_sm100.cu) whose A tiles are TMA-loaded with a per-tap row shift — no im2col
+// wgmma tap-GEMM launch (gemm_sm90.cu) whose A tiles are TMA-loaded with a per-tap row shift — no im2col
 // buffer — with bias, LayerScale, residual add and the *next* layer's SnakeBeta fused into the epilogue.
 // Small row-wise ops (RVQ gather, RMSNorm, RoPE, 72-frame sliding-window attention, depthwise conv + LayerNorm,
 // the final 96->1 conv + clamp) are plain CUDA kernels: they are <2 % of the FLOPs and HBM-trivial.
 #include "common.cuh"
-#include "gemm_sm100.cuh"
+#include "gemm_sm90.cuh"
 #include "../../include/qwen3tts_b200.h"
 
 #include <algorithm>
@@ -317,7 +317,7 @@ extern "C" int q3_codec_create(const q3_codec_cfg* cfg, q3_codec** out) {
   Q3_CUDA(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   Q3_CUDA(cudaGetDeviceProperties(&prop, cfg->device));
-  Q3_REQUIRE(prop.major == 10, "this library is built for sm_100a (B200); device is sm_%d%d", prop.major, prop.minor);
+  Q3_REQUIRE(prop.major == 9 && prop.minor == 0, "this library is built for sm_90a (H100); device is sm_%d%d", prop.major, prop.minor);
   Q3_REQUIRE(cfg->head_dim % 2 == 0 && cfg->head_dim <= 64, "codec head_dim must be even and <= 64");
   Q3_REQUIRE(cfg->sliding_window <= 96, "sliding_window > 96 unsupported");
   Q3_REQUIRE(cfg->num_heads == cfg->num_kv_heads, "codec transformer is MHA in the reference config");
@@ -747,7 +747,7 @@ extern "C" int q3_codec_stream_step(q3_codec_stream* s, const int32_t* codes_dev
     rmsnorm_rows_kernel<<<(rows + 7) / 8, 256, 0, stream>>>(xres, R.b16(p + ".ln1", Hh), X, rows, Hh, g.rms_eps);
     { GemmEpilogue e = none; e.out_raw = Z; R.gemm(X, n, Hh, (p + ".qkv.w").c_str(), 3 * nh * hd, 1, &zero, e); }
     const HistBuf& kv = s->kv[l];
-    rope_append_kernel<<<148, 256, 0, stream>>>(Z, R.b16("rope.cos", (int64_t)g.max_frames * (hd / 2)),
+    rope_append_kernel<<<132, 256, 0, stream>>>(Z, R.b16("rope.cos", (int64_t)g.max_frames * (hd / 2)),
                                                 R.b16("rope.sin", (int64_t)g.max_frames * (hd / 2)), kv.p, B, n, nh, hd, s->pos, kv.hist,
                                                 kv.bs_rows());
     swa_stream_kernel<<<(rows * nh + 7) / 8, 256, 0, stream>>>(Z, kv.p, X, B, n, nh, hd, g.sliding_window, s->pos, kv.bs_rows());

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the B200 (sm_100a) Qwen3-TTS hot-path kernels.
+// Shared device/host helpers for the H100 (sm_90a) Qwen3-TTS hot-path kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>

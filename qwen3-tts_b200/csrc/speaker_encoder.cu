@@ -1,9 +1,9 @@
-// Speaker x-vector path of voice cloning on B200 (sm_100a): 24 kHz waveform -> log-mel -> ECAPA-TDNN -> (enc_dim,) embedding.
+// Speaker x-vector path of voice cloning on H100 (sm_90a): 24 kHz waveform -> log-mel -> ECAPA-TDNN -> (enc_dim,) embedding.
 // Replaces Qwen3TTSForConditionalGeneration.extract_speaker_embedding (qwen_tts/core/models/modeling_qwen3_tts.py:1941-1954):
 // mel_spectrogram (:396-448) + Qwen3TTSSpeakerEncoder.forward (:371-393) with TimeDelayNetBlock :229-250, Res2NetBlock
 // :95-126, SqueezeExcitationBlock :129-157, SqueezeExcitationRes2NetBlock :253-297, AttentiveStatisticsPooling :160-226.
 //
-// Validated on a B200 against the CPU oracle (tests/test_gpu_speaker_encoder.py: log-mel, ECAPA embedding and the
+// Checked against the CPU oracle by tests/test_gpu_speaker_encoder.py (log-mel, ECAPA embedding and the
 // waveform-to-embedding path at tiny and default shapes, golden vectors).
 //
 // fp32 throughout, activations [B][C][T] (time contiguous).  One generalised direct-convolution kernel serves every
@@ -253,7 +253,7 @@ extern "C" int q3_spk_create(const q3_spk_cfg* cfg, q3_spk** out) {
   Q3_CUDA(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   Q3_CUDA(cudaGetDeviceProperties(&prop, cfg->device));
-  Q3_REQUIRE(prop.major == 10, "this library is built for sm_100a (B200); device is sm_%d%d", prop.major, prop.minor);
+  Q3_REQUIRE(prop.major == 9 && prop.minor == 0, "this library is built for sm_90a (H100); device is sm_%d%d", prop.major, prop.minor);
   Q3_REQUIRE(cfg->n_blocks >= 3 && cfg->n_blocks <= 8, "3..8 encoder stages (enc_channels entries)");
   Q3_REQUIRE(cfg->n_fft >= 64 && (cfg->n_fft & (cfg->n_fft - 1)) == 0 && cfg->n_fft <= 4096, "n_fft must be a power of two <= 4096");
   Q3_REQUIRE(cfg->hop >= 1 && cfg->hop <= cfg->n_fft && cfg->win == cfg->n_fft, "win_size must equal n_fft; 1 <= hop <= n_fft");

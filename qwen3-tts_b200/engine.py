@@ -23,7 +23,7 @@ def _rope_tables(n_pos, head_dim, theta, device):
 
 
 class AREngine:
-    """Talker + code predictor + sampler on one B200.  `weights` maps the reference's state_dict names
+    """Talker + code predictor + sampler on one H100.  `weights` maps the reference's state_dict names
     (`talker.model.layers.0.self_attn.q_proj.weight`, …) to tensors."""
 
     def __init__(self, cfg: TTSConfig, weights, device="cuda:0", max_batch=32, max_ctx=4096):

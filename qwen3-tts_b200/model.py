@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's Python API on top of the B200 engines (drop-in boundary, SURVEY §8b).
+"""Host-side mirror of the reference's Python API on top of the H100 engines (drop-in boundary, SURVEY §8b).
 
   * `Qwen3TTSForConditionalGenerationB200.generate(...)`  == core/models/modeling_qwen3_tts.py:2022-2292 (a1): builds the
     per-sample prefill embeddings exactly as the reference does (role / think-language-speaker prefix / text / ICL,
@@ -376,7 +376,7 @@ class Qwen3TTSForConditionalGenerationB200:
 
 # ----------------------------------------------------------------------------------------------------------------
 class Qwen3TTSTokenizer:
-    """inference/qwen3_tts_tokenizer.py:44 — decode path on the B200 codec engine."""
+    """inference/qwen3_tts_tokenizer.py:44 — decode path on the H100 codec engine."""
 
     def __init__(self, cfg: CodecConfig, weights, device="cuda:0", max_frames=1024, encoder_cfg=None,
                  encoder_weights=None):
@@ -402,7 +402,7 @@ class Qwen3TTSTokenizer:
         if want is not None and str(want).replace("torch.", "") in ("float32", "float", "float64", "double"):
             # not silent: the reference's standalone tokenizer (examples/test_tokenizer_12hz.py) runs in fp32
             import warnings
-            warnings.warn(f"Qwen3TTSTokenizer: dtype={want} requested, but the B200 codec DECODER always computes in bf16 on the "
+            warnings.warn(f"Qwen3TTSTokenizer: dtype={want} requested, but the H100 codec DECODER always computes in bf16 on the "
                           "tensor cores (fp32 accumulation; ~30 dB SNR against an fp32 forward, DESIGN.md section 5); the "
                           "ENCODER runs in fp32 and returns the same codes as the fp32 reference.", RuntimeWarning, stacklevel=2)
         d = checkpoint.resolve_dir(pretrained_model_name_or_path)

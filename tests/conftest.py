@@ -1,8 +1,6 @@
 import os
 import sys
 
-import pytest
-
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
@@ -10,14 +8,5 @@ os.environ.setdefault("PYTHONDONTWRITEBYTECODE", "1")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
-    config.addinivalue_line("markers", "reference: needs /root/reference (build container only)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
-
-def pytest_collection_modifyitems(config, items):
-    from oracle import ref_shims
-    have_ref = ref_shims.reference_available()
-    skip_ref = pytest.mark.skip(reason="/root/reference not present (GPU box)")
-    for item in items:
-        if "reference" in item.keywords and not have_ref:
-            item.add_marker(skip_ref)

@@ -144,15 +144,14 @@ def write_tiny_checkpoint(directory, device="cpu", sharded=False, seed=0, model_
 
 def report_parity(name, record):
     """Parity figures the GPU tests measure (free-running exact-match rates, worst logit errors): printed, and
-    collected into gpurun_out/parity_report.json so a GPU run leaves them behind as an artifact."""
+    collected into the JSON file named by $Q3_PARITY_REPORT when that is set."""
     import json, os
     record = {k: (float(v) if isinstance(v, (np.floating, float)) else int(v) if isinstance(v, (np.integer,)) else v) for k, v in record.items()}
     print(f"[parity] {name}: {json.dumps(record)}")
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    out = os.path.join(root, "gpurun_out")
+    path = os.environ.get("Q3_PARITY_REPORT")
+    if not path:
+        return
     try:
-        os.makedirs(out, exist_ok=True)
-        path = os.path.join(out, "parity_report.json")
         data = json.load(open(path)) if os.path.exists(path) else {}
         data[name] = record
         json.dump(data, open(path, "w"), indent=1, sort_keys=True)

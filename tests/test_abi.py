@@ -1,4 +1,4 @@
-"""CPU-side checks of the drop-in boundary: the C-ABI library builds for sm_100a, loads, and exports every
+"""CPU-side checks of the drop-in boundary: the C-ABI library builds for sm_90a, loads, and exports every
 symbol include/qwen3tts_b200.h declares (no compute calls without a GPU)."""
 import ctypes
 import os
@@ -55,16 +55,15 @@ def test_engine_fails_loudly_without_gpu():
         CodecEncoder(synthetic.cfg_encoder_tiny(), {}, device="cpu")
 
 
-def test_sass_is_sm100a_with_tcgen05_tma():
-    """The shipped cubins target sm_100a; the codec/prefill GEMM carries tcgen05 (UTCHMMA), TMEM loads (LDTM) and
-    TMA tile loads (UTMALDG); the frame-step kernel stages its weights with bulk TMA copies into shared memory
-    (UBLKCP.S.G) completed on mbarriers (SYNCS...TRYWAIT), prefetches KV rows with cp.async (LDGSTS) and runs the
+def test_sass_is_sm90a_with_wgmma_tma():
+    """The shipped cubins target sm_90a; the codec/prefill GEMM carries wgmma (HGMMA) fed by TMA tile loads
+    (UTMALDG); the frame-step kernel stages its weights with bulk TMA copies into shared memory (UBLKCP.S.G) completed on mbarriers (SYNCS...TRYWAIT), prefetches KV rows with cp.async (LDGSTS) and runs the
     batch-in-N mma.sync (HMMA)."""
     import subprocess
     from qwen3_tts_b200 import build
     path = build.build()
     out = subprocess.run(["cuobjdump", "-lelf", path], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
     sass = subprocess.run(["cuobjdump", "-sass", path], capture_output=True, text=True).stdout
-    for mnemonic in ("UTCHMMA", "LDTM", "UTMALDG", "UBLKCP.S.G", "SYNCS.PHASECHK.TRANS64.TRYWAIT", "LDGSTS", "HMMA"):
+    for mnemonic in ("HGMMA", "UTMALDG", "UBLKCP.S.G", "SYNCS.PHASECHK.TRANS64.TRYWAIT", "LDGSTS", "HMMA"):
         assert mnemonic in sass, f"{mnemonic} missing from SASS"

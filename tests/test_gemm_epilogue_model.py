@@ -1,10 +1,11 @@
-"""CPU model of the tap-GEMM epilogue's shared-memory staging (csrc/gemm_sm100.cu): the index math that has to be right
-for the coalesced stores to be correct and bank-conflict free, and the shared-memory budget of every tile width.  The
-constants are read from the CUDA source so the model follows the kernel."""
+"""CPU model of the tap-GEMM kernel's tiling (csrc/gemm_sm90.cu): the accumulator-fragment index math the epilogue uses
+to find each output element, and the shared-memory budget of every tile width.  The constants are read from the CUDA
+source so the model follows the kernel."""
 import os
 import re
 
-SRC = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "qwen3-tts_b200", "csrc", "gemm_sm100.cu")).read()
+SRC = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "qwen3-tts_b200", "csrc", "gemm_sm90.cu")).read()
+TILE_WIDTHS = (64, 128)   # what gemm_make_plan_v accepts
 
 
 def const(name):
@@ -14,60 +15,52 @@ def const(name):
     return int(eval(expr, {}, {k: const(k) for k in re.findall(r"[A-Z_]{2,}", expr) if k != name}))
 
 
-def slot(row, chunk):
-    """byte offset of 16-byte chunk `chunk` of row `row` inside a 32 x 128 B staging buffer (XOR swizzle by the row)"""
-    return row * 128 + ((chunk ^ (row & 7)) << 4)
+def fragment(warp, lane, i):
+    """(row, column) inside a warpgroup's 64 x bn accumulator of accumulator register i (m64nNk16, f32)"""
+    j, h, e = i // 4, (i // 2) % 2, i % 2
+    return 16 * (warp % 4) + lane // 4 + 8 * h, 8 * j + 2 * (lane % 4) + e
 
 
-def test_own_slots_and_cooperative_items_cover_the_block_exactly_once():
-    own = {}
-    for j in range(4):             # the four warps of a TMEM lane quadrant
-        for lane in range(32):     # thread = output row
-            for c in (2 * j, 2 * j + 1):
-                own[slot(lane, c)] = (lane, c)
-    assert len(own) == 256 and sorted(own) == [16 * i for i in range(256)]
-    coop = {}
-    for tq in range(128):
-        for i in range(2):
-            item = tq + 128 * i
-            row, chunk = item >> 3, item & 7
-            assert row == (tq >> 3) + 16 * i and chunk == tq & 7   # what the kernel computes
-            coop[slot(row, chunk)] = (row, chunk)
-    assert coop == own   # every (row, chunk) written by its owner is moved by exactly one cooperative item
+def test_fragments_cover_each_warpgroup_tile_exactly_once():
+    for bn in TILE_WIDTHS:
+        seen = {}
+        for warp in range(4):
+            for lane in range(32):
+                for i in range(bn // 2):
+                    rc = fragment(warp, lane, i)
+                    assert rc not in seen, (bn, rc)
+                    seen[rc] = (warp, lane, i)
+        assert sorted(seen) == [(r, c) for r in range(64) for c in range(bn)]
 
 
-def test_staging_accesses_are_bank_conflict_free():
-    # a 16-byte access is served per quarter-warp (8 lanes): the 8 lanes must hit 8 different 16-byte bank groups
-    for j in range(4):
-        for c in (2 * j, 2 * j + 1):
-            for q0 in range(0, 32, 8):
-                groups = {(slot(lane, c) >> 4) & 7 for lane in range(q0, q0 + 8)}
-                assert len(groups) == 8
-    for tq0 in range(0, 128, 8):   # cooperative side: 8 consecutive threads = one row, 8 chunks
-        for i in range(2):
-            rows = {(tq + 128 * i) >> 3 for tq in range(tq0, tq0 + 8)}
-            groups = {(slot((tq + 128 * i) >> 3, tq & 7) >> 4) & 7 for tq in range(tq0, tq0 + 8)}
-            assert len(rows) == 1 and len(groups) == 8
-
-
-def test_a_warp_store_covers_whole_128_byte_row_segments():
-    # lanes 8k..8k+7 of a cooperative store write the 8 chunks of ONE row: 4 full lines per instruction, not 32
-    for w in range(4):
-        for i in range(2):
-            lines = {((32 * w + l + 128 * i) >> 3) for l in range(32)}
-            assert len(lines) == 4
+def test_pair_and_gated_epilogues_read_matching_columns():
+    for bn in TILE_WIDTHS:
+        for warp in range(4):
+            for lane in range(32):
+                for j in range(bn // 8):
+                    for h in range(2):
+                        r0, c0 = fragment(warp, lane, 4 * j + 2 * h)
+                        r1, c1 = fragment(warp, lane, 4 * j + 2 * h + 1)
+                        assert r0 == r1 and c0 % 2 == 0 and c1 == c0 + 1   # one 4-byte bf16 pair per store
+                for j in range(bn // 16):   # ACT_SWIGLU_BLK8: gate in columns 16j..16j+7, up 8 columns later, same row
+                    for h in range(2):
+                        for e in range(2):
+                            rg, cg = fragment(warp, lane, 8 * j + 2 * h + e)
+                            ru, cu = fragment(warp, lane, 8 * j + 4 + 2 * h + e)
+                            assert rg == ru and cu == cg + 8 and cg // 16 == j and cg % 16 < 8
 
 
 def test_shared_memory_budget_for_every_tile_width():
     BM, BK = const("BM"), const("BK")
     a_bytes = BM * BK * 2
-    optin, epi, bar, max_stages = const("SMEM_OPTIN"), 4 * 3 * 32 * 128, const("BAR_BYTES"), const("MAX_STAGES")
-    assert const("EPI_BYTES") == epi and const("A_BYTES") == a_bytes
-    for bn in range(16, 257, 16):
+    optin, bar, max_stages = const("SMEM_OPTIN"), const("BAR_BYTES"), const("MAX_STAGES")
+    assert const("A_BYTES") == a_bytes and 2 * 8 * max_stages <= bar
+    for bn in TILE_WIDTHS:
         stage = a_bytes + ((bn * BK * 2 + 1023) & ~1023)
-        nst = min(max_stages, (optin - 1024 - bar - epi) // stage)
-        assert nst >= 3, (bn, nst)                      # the TMA ring never gets shallower than 3 stages
-        assert 1024 + nst * stage + bar + epi <= optin  # what gemm_launch asks for fits the 227 KB opt-in
+        nst = min(max_stages, (optin - 1024 - bar) // stage)
+        assert nst >= 4, (bn, nst)                      # the TMA ring never gets shallower than 4 stages
+        assert 1024 + nst * stage + bar <= optin        # what gemm_launch asks for fits the 227 KB opt-in
         assert stage % 1024 == 0                        # SWIZZLE_128B operand tiles stay 1024-byte aligned
     threads = const("GEMM_THREADS")
-    assert threads == 64 + 32 * const("EPI_WARPS") and const("EPI_WARPS") % 4 == 0 and threads <= 1024
+    assert threads == 128 * const("CONSUMER_WGS") + 32 and const("PRODUCER_WARP") == 4 * const("CONSUMER_WGS")
+    assert BM == 64 * const("CONSUMER_WGS")

@@ -224,7 +224,7 @@ def _full_shape_case(model, lens, N, seed):
         r = ref.record["talker_logits"][f]
         scale = float(np.std(r))
         d = np.abs(tl[f] - r)
-        # calibration (tools/calibrate_tolerance.py -> profiles/r02_tolerance_calibration.txt): PyTorch's OWN bf16 run of
+        # calibration (tools/calibrate_tolerance.py): PyTorch's OWN bf16 run of
         # these shapes (ctx 200-230, 8 frames, two seeds) deviates from the fp32 oracle by up to max 0.18*std / mean
         # 0.037*std on the talker logits and max 0.27*std / mean 0.051*std on the code-predictor logits; the engine is
         # held to 1.5x those figures (MAX_TOL, MEAN_TOL)

@@ -1,7 +1,5 @@
 """GPU parity of the speaker x-vector path (csrc/speaker_encoder.cu through the C ABI) against the CPU oracle
-(oracle/speaker_encoder.py, itself bit-identical to the reference's Qwen3TTSSpeakerEncoder / mel_spectrogram).
-
-Validated on a B200 at the very end of round 1 (all tests green on the first hardware run)."""
+(oracle/speaker_encoder.py, itself bit-identical to the reference's Qwen3TTSSpeakerEncoder / mel_spectrogram)."""
 import os
 
 import numpy as np

@@ -1,5 +1,4 @@
-"""Checkpoint loading and voice cloning from raw audio, end to end on the GPU (BASELINE config 5 in miniature): both green
-on a B200 (last GPU call of round 1)."""
+"""Checkpoint loading and voice cloning from raw audio, end to end on the GPU (BASELINE config 5 in miniature)."""
 import numpy as np
 import pytest
 import torch

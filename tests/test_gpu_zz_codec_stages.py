@@ -1,9 +1,6 @@
 """Per-stage parity of the codec DECODER against the CPU oracle (through q3_codec_debug_capture), so an error in one
-small kernel cannot hide behind the waveform SNR, and the full default config at 64 frames.
-
-These tests and the capture hook were written after the round's GPU budget had been spent: their first execution on a
-B200 is the driver's round-end run.  They are therefore marked xfail(strict=False) — an XPASS is the validation, a
-failure here must not mask the rest of the (validated) suite.  The file sorts last on purpose."""
+small kernel cannot hide behind the waveform SNR, and the full default config at 64 frames.  The file sorts last on
+purpose: the full-config captures are the largest allocations of the suite."""
 import pytest
 import torch
 
@@ -11,8 +8,7 @@ from oracle import codec as OC
 from tests.helpers import report_parity
 from tests.test_gpu_codec import DEV, _bf16_round, _pkg_cfg, _small_cfg, _snr_db
 
-pytestmark = [pytest.mark.gpu,
-              pytest.mark.xfail(strict=False, reason="added after the round's GPU budget was spent; first hardware run is the driver's")]
+pytestmark = pytest.mark.gpu
 
 
 def _reference_stages(Wf, cfg, codes):
