@@ -138,15 +138,14 @@ int q3_set_hidden_capture(q3_engine* e, void* hid_dev, int32_t stride);
 int q3_set_debug(q3_engine* e, const int32_t* forced_dev, int32_t n_frames, float* talker_logits_dev,
                  float* cp_logits_dev);
 
-/* Profiling hooks (tools/critical_path.py, tools/profile_frame.py): prof_dev = uint64 [n_phases][grid][8] %globaltimer
- * ns written by thread 0 of EVERY CTA during the first frame of each q3_decode: [0] phase body end, [1] barrier passed,
- * [2..5] inner marks of the phase body, [6] phase start, [7] staging mark; q3_describe_frame_program returns -n_phases
- * and fills kinds[i] = type*100 + stack*10 + epilogue. */
+/* Profiling hooks (tools/profile_frame.py): prof_dev = uint64 [n_phases][grid][16], written by thread 0 of EVERY CTA
+ * during the first frame of each q3_decode while it is set (the decode then runs the profiled kernel instantiation).
+ * %globaltimer ns: [0] phase body end, [1] barrier passed, [2..4] inner marks of the phase body (GEMV: activations
+ * staged, main loop done, epilogue done; attention: K/V window loaded, partials done, combine done), [6] phase start, [8] / [7] start / end of
+ * warp 0's GEMV main loop; [5] clock cycles warp 0 waited for ring data in a GEMV phase; slots 9..15 are not written.
+ * q3_describe_frame_program returns -n_phases and fills kinds[i] = type*100 + stack*10 + epilogue. */
 int q3_set_profile(q3_engine* e, unsigned long long* prof_dev);
 int q3_describe_frame_program(q3_engine* e, int32_t* kinds, int32_t capacity);
-/* time `count` repetitions of frame-program phases [first, first+span) as one launch (instruction-cache probe) */
-int q3_debug_set_skip(q3_engine* e, int32_t mask); /* ablation bits for tools/ablate_phase.py; 0 = normal */
-int q3_debug_time_phases(q3_engine* e, int32_t first, int32_t span, int32_t count, float* ms_out, void* stream);
 
 /* Bytes the fused frame-step kernel must stream per step for batch B at mean context S
  * (SURVEY §8d: W_talker + W_cp_unique + B*(S+1)*KV_tok), and the no-residency figure. */

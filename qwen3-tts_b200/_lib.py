@@ -60,7 +60,7 @@ class SpkCfg(C.Structure):
 # every symbol include/qwen3tts_b200.h declares (tests/test_abi.py checks the header against this list)
 AR_SYMBOLS = ["q3_abi_version", "q3_last_error", "q3_engine_create", "q3_engine_destroy", "q3_engine_load_tensor",
               "q3_engine_finalize", "q3_prefill", "q3_decode", "q3_get_progress", "q3_set_debug",
-              "q3_algorithmic_bytes", "q3_set_profile", "q3_describe_frame_program", "q3_debug_time_phases", "q3_debug_set_skip",
+              "q3_algorithmic_bytes", "q3_set_profile", "q3_describe_frame_program",
               "q3_session_begin", "q3_admit", "q3_release_slots", "q3_append_trailing", "q3_set_hidden_capture"]
 CODEC_SYMBOLS = ["q3_codec_create", "q3_codec_destroy", "q3_codec_load_tensor", "q3_codec_finalize",
                  "q3_codec_forward", "q3_codec_total_upsample", "q3_codec_last_launch_count", "q3_codec_debug_capture",
@@ -116,8 +116,6 @@ def load():
     lib.q3_set_debug.argtypes = [vp, vp, i32, vp, vp]
     lib.q3_set_profile.argtypes = [vp, vp]
     lib.q3_describe_frame_program.argtypes = [vp, C.POINTER(i32), i32]
-    lib.q3_debug_set_skip.argtypes = [vp, i32]
-    lib.q3_debug_time_phases.argtypes = [vp, i32, i32, i32, C.POINTER(C.c_float), vp]
     lib.q3_algorithmic_bytes.argtypes = [vp, i32, i32, C.POINTER(C.c_double), C.POINTER(C.c_double)]
     if hasattr(lib, "q3_codec_create"):
         lib.q3_codec_create.argtypes = [C.POINTER(CodecCfg), C.POINTER(vp)]

@@ -23,7 +23,6 @@
 
 #include <cooperative_groups.h>
 #include <stdarg.h>
-#include <stdlib.h>
 #include <algorithm>
 #include <map>
 #include <vector>
@@ -50,8 +49,8 @@ namespace {
 // ------------------------------------------------------------------------------------------------
 // the persistent kernel
 // ------------------------------------------------------------------------------------------------
-// VAR: 0 = production, 1 = production + per-step hidden-state capture, 2 = development (hidden capture + device-timestamp
-// marks + the ablation / A-B knobs of KParams::flags).  See gemv_phase for why these are separate instantiations.
+// VAR: 0 = production, 1 = production + per-step hidden-state capture, 2 = profiled (hidden capture + device-timestamp
+// marks).  See gemv_phase for why these are separate instantiations.
 template <int NT, int VAR>
 __global__ void __launch_bounds__(CTA_THREADS, 1) q3_step_kernel(const __grid_constant__ KParams P) {
   extern __shared__ __align__(1024) unsigned char smem[];
@@ -60,8 +59,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 1) q3_step_kernel(const __grid_co
   DevState* st = P.st;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   constexpr bool HID = VAR >= 1, DEV = VAR == 2;
-  const bool use_counter = !DEV || (P.flags & 1) == 0;
-  unsigned int epoch = 0;  // host resets bar_count / bar_flags to 0 before every launch
+  unsigned int epoch = 0;  // host resets bar_count to 0 before every launch
   PMeta* meta = reinterpret_cast<PMeta*>(smem + P.plan.meta_off);
   const int R = P.plan.nslots, SB = P.plan.slot_blocks;
   const uint32_t full0 = smem_addr(smem + P.plan.bar_off);      // [NWARPS][R] full barriers, then the x barrier
@@ -94,7 +92,6 @@ __global__ void __launch_bounds__(CTA_THREADS, 1) q3_step_kernel(const __grid_co
   __syncthreads();
   if (s_ph[0].type == PH_GEMV && s_ph[0].norm_w != nullptr && tid < s_ph[0].kb * 4)
     reinterpret_cast<uint4*>(smem + P.plan.nw_off)[tid] = reinterpret_cast<const uint4*>(s_ph[0].norm_w)[tid];
-  if (s_ph[0].type == PH_ATTN) attn_prefetch(s_ph[0], P, smem + P.plan.x_off, st->step);  // (synthetic profiling programs only)
 
   // L2 eviction priorities of the weight stream (createpolicy): the talker and the 15 heads are read once per
   // frame-step -> evict_first; the code predictor's layer weights (157 MB) are re-read on each of its 15 passes -> a
@@ -115,7 +112,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 1) q3_step_kernel(const __grid_co
     ring_init(rg, P.runs + o0, (int)(o1 - o0), (long long)(o1 - o0) * niter);
   }
 #pragma unroll 1
-  for (int i = 0; i < R; ++i) ring_issue<DEV>(rg, P, lane, pol_stream, pol_keep);
+  for (int i = 0; i < R; ++i) ring_issue(rg, P, lane, pol_stream, pol_keep);
   __syncthreads();
 
   const int step_base = st->step;
@@ -150,7 +147,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 1) q3_step_kernel(const __grid_co
       if (dhave) reinterpret_cast<uint32_t*>(&s_ph[slot ^ 1])[tid] = dreg;
       cta_sync();  // body done (global writes of every thread precede thread 0's release), next descriptor visible
       PROF_MARK(0);
-      grid_arrive(st, epoch, use_counter);
+      grid_arrive(st, epoch);
       // work that does not depend on the other CTAs, between arrive and wait: the next GEMV's RMSNorm weights
       // (load now, store after the wait) and the KV rows the next attention phase will need
       uint4 nwv = make_uint4(0, 0, 0, 0);
@@ -164,7 +161,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 1) q3_step_kernel(const __grid_co
           attn_prefetch(nph, P, smem + P.plan.x_off, pi + 1 >= P.n_phases ? frame + 1 : frame);
         }
       }
-      grid_wait(st, epoch, use_counter);
+      grid_wait(st, epoch);
       slot ^= 1;
       if (nw_have) reinterpret_cast<uint4*>(smem + P.plan.nw_off)[tid] = nwv;
       cta_sync();
@@ -234,17 +231,15 @@ struct q3_engine {
   int prog_cap = 0;
   // programs (host copies) for the current batch size
   int prog_B = -1;
-  int flags = 0;              // Q3_FLAGS / q3_debug_set_skip: A/B knobs of the frame-step kernel (see KParams.flags)
   const char* wbase = nullptr;  // lowest packed-weight address (PMeta offsets)
   float keep_fraction = 0.5f;
   int cp_phases = 0;
   int nt_frame = 1, nt_head = 1, max_dyn_smem = 0;
   SmemPlan plan_frame{}, plan_head{};
   PieceTable pt_frame{}, pt_head{};
-  bool use_proj_tab = true;   // Q3_CP_PROJ_TAB=0 keeps the projection GEMV in passes >= 1 (A/B knob)
   bf16* proj_tab = nullptr;   // small_to_mtp_projection(cp.codec_embedding) [(G-1)*Vc][Hc], built once at finalize
-  std::vector<Phase> prog_layers, prog_head, prog_frame;
-  int off_layers = 0, off_head = 0, off_frame = 0;
+  std::vector<Phase> prog_head, prog_frame;
+  int off_head = 0, off_frame = 0;
   q3_sampling sp{};
   bool finalized = false;
   int B = 0;
@@ -320,11 +315,6 @@ extern "C" int q3_engine_create(const q3_engine_cfg* cfg, q3_engine** out) {
   e->cfg = *cfg;
   e->sm_count = prop.multiProcessorCount;
   e->l2_bytes = (size_t)prop.l2CacheSize;
-  if (const char* g = getenv("Q3_GRID")) {  // experiment knob: persistent grid smaller than the SM count
-    const int v = atoi(g);
-    if (v >= 8 && v <= e->sm_count) e->sm_count = v;
-  }
-  if (const char* f = getenv("Q3_CP_PROJ_TAB")) e->use_proj_tab = atoi(f) != 0;
   Q3_CUDA(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
   if (gemm_init()) return 1;
   if (e->alloc(&e->st, 1)) return 1;
@@ -339,8 +329,6 @@ extern "C" int q3_engine_create(const q3_engine_cfg* cfg, q3_engine** out) {
   if (e->alloc(&e->split_buf, (size_t)MAXB * cfg->talker.num_kv_heads * MAXSPLIT * RMAX * 130)) return 1;
   static_assert(SAMPLER_SMEM <= X_MIN_BYTES && ATT_SMEM <= X_MIN_BYTES, "attention / sampler scratch must fit the x area");
   Q3_REQUIRE((size_t)SMEM_OPTIN <= (size_t)prop.sharedMemPerBlockOptin, "not enough shared memory per block");
-  if (const char* f = getenv("Q3_FLAGS")) e->flags = atoi(f);
-  if (const char* f = getenv("Q3_KEEP_FRACTION")) e->keep_fraction = (float)atof(f);
   *out = e;
   return 0;
 }
@@ -452,9 +440,8 @@ static int add_layers(q3_engine* e, std::vector<Phase>& prog, const char* pfx, S
 // Run table of a program: for every (CTA, warp) the sequence of contiguous weight runs (offset from the weight arena
 // base in 16-byte units, number of 1 KB blocks) of ONE pass over the program, enumerated with the same iterator the
 // model check in tests/test_ring_model.py exercises.  The kernel's consumer loop derives the same runs from run_geom().
-static int build_piece_table(q3_engine* e, const std::vector<Phase>& prog, int SB, PieceTable* out, int keep_phases = 0) {
+static int build_piece_table(q3_engine* e, const std::vector<Phase>& prog, PieceTable* out, int keep_phases = 0) {
   const int grid = e->sm_count, n = (int)prog.size();
-  (void)SB;
   std::vector<uint2> pieces;
   std::vector<uint32_t> off;
   off.reserve((size_t)grid * NWARPS + 1);
@@ -522,18 +509,15 @@ static int make_smem_plan(q3_engine* e, std::vector<Phase>& prog, int B, int nt,
   const int meta_bytes = up((int)prog.size() * (int)sizeof(q3ring::PMeta), 16);
   const int bar_bytes = 8 * (NWARPS * MAX_SLOTS + 1) + 8;  // one full barrier per ring slot, the x barrier
   // batch classes 1-2 stay under the 196 KB carve-out (195 KB per CTA) so that 32 KB of the SM remain L1: the phase
-  // functions' stack traffic then hits L1 instead of making an L2 round trip each (Q3_SMEM_FULL=1 lifts the cap: A/B)
+  // functions' stack traffic then hits L1 instead of making an L2 round trip each
   int limit = e->max_dyn_smem;
-  if (nt <= 2 && !getenv("Q3_SMEM_FULL")) limit = std::min(limit, 195 * 1024 - (SMEM_OPTIN - e->max_dyn_smem) - 256);
+  if (nt <= 2) limit = std::min(limit, 195 * 1024 - (SMEM_OPTIN - e->max_dyn_smem) - 256);
   const int avail = limit - pl.ring_off - meta_bytes - bar_bytes;
-  int slot_cap = MAX_SLOTS;
-  if (const char* f = getenv("Q3_RING_SLOTS")) slot_cap = std::max(2, std::min(MAX_SLOTS, atoi(f)));
   pl.slot_blocks = 0;
-  int sb_first = nt == 4 ? 2 : 4;  // the largest batch class keeps its B fragments of a piece in registers: 2-block pieces
-  if (const char* f = getenv("Q3_SLOT_BLOCKS")) sb_first = std::max(1, std::min(sb_first, atoi(f)));
+  const int sb_first = nt == 4 ? 2 : 4;  // the largest batch class keeps its B fragments of a piece in registers: 2-block pieces
   for (int sb : {sb_first, 2, 1}) {
     const int r = avail / (NWARPS * sb * 1024);
-    if (r >= 2) { pl.slot_blocks = sb; pl.nslots = std::min(r, slot_cap); break; }
+    if (r >= 2) { pl.slot_blocks = sb; pl.nslots = std::min(r, MAX_SLOTS); break; }
   }
   Q3_REQUIRE(pl.slot_blocks > 0, "no shared memory left for the weight rings (x area %d B, batch class %d)", pl.x_bytes, nt);
   pl.meta_off = pl.ring_off + NWARPS * pl.nslots * pl.slot_blocks * 1024;
@@ -559,8 +543,6 @@ static int build_programs(q3_engine* e, int B) {
   if (c.has_cp_projection) {
     if (need_packed(e, "cp.proj", Hc, H, &wproj) || need_plain(e, "cp.proj_bias", Hc, &bproj)) return 1;
   }
-  // ---- prefill-chunk program: talker layers over the chunk's columns
-  e->prog_layers.clear();  // (prefill runs on the wgmma GEMM path, see q3_prefill)
   // ---- prefill-head program: final norm + codec_head on the last token of each row, sample frame-0 codebook-0
   e->prog_head.clear();
   {
@@ -616,7 +598,7 @@ static int build_programs(q3_engine* e, int B) {
     Phase s{}; s.type = PH_SAMPLE; s.group = 0;
     F.push_back(s);
   }
-  for (std::vector<Phase>* pv : {&e->prog_layers, &e->prog_head, &e->prog_frame})
+  for (std::vector<Phase>* pv : {&e->prog_head, &e->prog_frame})
     for (Phase& p : *pv)
       if (p.type == PH_GEMV) { p.tq = p.n_tiles / e->sm_count; p.tr = p.n_tiles % e->sm_count; }
   // shared-memory plans: which phases stage their activations, how large the x area is, what is left for the rings
@@ -625,22 +607,19 @@ static int build_programs(q3_engine* e, int B) {
   if (make_smem_plan(e, e->prog_head, B, e->nt_head, &e->plan_head) || make_smem_plan(e, e->prog_frame, B, e->nt_frame, &e->plan_frame))
     return 1;
   Q3_REQUIRE((int)F.size() <= MAX_PHASES, "frame program has %d phases (max %d)", (int)F.size(), MAX_PHASES);
-  if (build_piece_table(e, e->prog_head, e->plan_head.slot_blocks, &e->pt_head) ||
-      build_piece_table(e, e->prog_frame, e->plan_frame.slot_blocks, &e->pt_frame, e->cp_phases))
+  if (build_piece_table(e, e->prog_head, &e->pt_head) || build_piece_table(e, e->prog_frame, &e->pt_frame, e->cp_phases))
     return 1;
   // upload (a batch-size change is rare: wait for launches that may still walk the old program)
   Q3_CUDA(cudaDeviceSynchronize());
-  const size_t total = e->prog_layers.size() + e->prog_head.size() + F.size();
+  const size_t total = e->prog_head.size() + F.size();
   if ((int)total > e->prog_cap) {
     e->release(e->prog_dev);
     e->prog_dev = nullptr;
     if (e->alloc(&e->prog_dev, total + 64)) return 1;
     e->prog_cap = (int)total + 64;
   }
-  e->off_layers = 0;
-  e->off_head = (int)e->prog_layers.size();
-  e->off_frame = e->off_head + (int)e->prog_head.size();
-  Q3_CUDA(cudaMemcpy(e->prog_dev + e->off_layers, e->prog_layers.data(), e->prog_layers.size() * sizeof(Phase), cudaMemcpyHostToDevice));
+  e->off_head = 0;
+  e->off_frame = (int)e->prog_head.size();
   Q3_CUDA(cudaMemcpy(e->prog_dev + e->off_head, e->prog_head.data(), e->prog_head.size() * sizeof(Phase), cudaMemcpyHostToDevice));
   Q3_CUDA(cudaMemcpy(e->prog_dev + e->off_frame, F.data(), F.size() * sizeof(Phase), cudaMemcpyHostToDevice));
   e->prog_B = B;
@@ -666,7 +645,8 @@ extern "C" int q3_engine_finalize(q3_engine* e) {
     return 1;
   // projection table: passes >= 1 of the code predictor feed small_to_mtp_projection(codec_embedding[j-1](c_j)) (:1281-1283),
   // a function of the sampled id only -> one wgmma GEMM over all (G-1)*Vc embedding rows here, no GEMV phase per pass
-  if (c.has_cp_projection && e->use_proj_tab && e->gemm_w.count("cp.proj") && !e->proj_tab) {
+  // (without a GEMM copy of cp.proj, i.e. a talker hidden size that is not a multiple of 64, each pass keeps its projection GEMV)
+  if (c.has_cp_projection && e->gemm_w.count("cp.proj") && !e->proj_tab) {
     const int H = c.talker.hidden_size, Hc = c.cp.hidden_size;
     const int rows = (c.num_code_groups - 1) * c.cp.vocab_size;
     const bf16* bproj;
@@ -725,7 +705,7 @@ extern "C" int q3_engine_finalize(q3_engine* e) {
   // L2 residency of the code predictor's layer weights (re-read on each of its passes): keep a bit over half of the
   // L2 (27 MB of H100's 50 MB) of them at evict_last priority beside the talker's evict_first stream; much more than
   // that and the evict_last lines evict each other
-  if (!getenv("Q3_KEEP_FRACTION")) e->keep_fraction = (float)std::min(1.0, 0.54 * (double)e->l2_bytes / (2.0 * cpl));
+  e->keep_fraction = (float)std::min(1.0, 0.54 * (double)e->l2_bytes / (2.0 * cpl));
   e->finalized = true;
   return 0;
 }
@@ -747,14 +727,14 @@ static int launch_program(q3_engine* e, int off, int n, int mode, int max_iters,
   else { P.cp_next = P.emb_cp; P.cp_next_dst = P.x_cp; P.cp_next_w = e->cfg.talker.hidden_size; }
   P.tts_pad = e->tts_pad; P.seen = e->seen; P.codes_out = codes_dev; P.codes_stride = e->codes_stride;
   P.split_buf = e->split_buf; P.forced = e->forced; P.n_forced = e->n_forced; P.dbg_tlogits = e->dbg_t; P.dbg_clogits = e->dbg_c; P.prof = (mode == 1) ? e->prof : nullptr;
-  P.flags = e->flags; P.wbase = e->wbase; P.keep_fraction = e->keep_fraction;
+  P.wbase = e->wbase; P.keep_fraction = e->keep_fraction;
   P.hid_out = e->hid_out; P.hid_stride = e->hid_stride;
   P.runs = pt.runs; P.run_off = pt.off;
-  P.plan = plan; P.cp_phases = (off == e->off_frame && n == (int)e->prog_frame.size()) ? e->cp_phases : 0;
+  P.plan = plan;
   Q3_REQUIRE(n <= MAX_PHASES, "program of %d phases exceeds %d", n, MAX_PHASES);
-  Q3_CUDA(cudaMemsetAsync(&e->st->bar_count, 0, sizeof(unsigned int) * (1 + 256), stream));  // counter + per-CTA flags
+  Q3_CUDA(cudaMemsetAsync(&e->st->bar_count, 0, sizeof(unsigned int), stream));
   void* args[] = {&P};
-  const int var = (P.flags != 0 || P.prof) ? 2 : P.hid_out ? 1 : 0;
+  const int var = P.prof ? 2 : P.hid_out ? 1 : 0;
   static const void* const kfn[3][3] = {
       {(const void*)q3_step_kernel<1, 0>, (const void*)q3_step_kernel<2, 0>, (const void*)q3_step_kernel<4, 0>},
       {(const void*)q3_step_kernel<1, 1>, (const void*)q3_step_kernel<2, 1>, (const void*)q3_step_kernel<4, 1>},
@@ -1046,52 +1026,6 @@ extern "C" int q3_describe_frame_program(q3_engine* e, int32_t* kinds, int32_t c
     }
   }
   return -n;  // negative = count (0 is reserved for success elsewhere); callers use abs()
-}
-
-// Debug/profiling: run a synthetic program made of `count` repetitions of the frame-program phases
-// [first, first+span) (mode 0, one pass) and return the elapsed device time.  Used by tools/icache_probe.py.
-// A/B knobs of the frame-step kernel (KParams.flags): 1 = counter barrier, 2 = LDG staging of un-normed inputs
-extern "C" int q3_debug_set_skip(q3_engine* e, int32_t mask) { if (e) e->flags = mask; return 0; }
-
-extern "C" int q3_debug_time_phases(q3_engine* e, int32_t first, int32_t span, int32_t count, float* ms_out, void* stream_) {
-  Q3_REQUIRE(e && e->prog_B > 0 && e->B > 0, "prefill first");
-  Q3_REQUIRE(first >= 0 && span >= 1 && first + span <= (int)e->prog_frame.size() && count >= 1, "bad phase range");
-  Q3_REQUIRE(count * span <= MAX_PHASES, "count*span must be <= %d", MAX_PHASES);
-  cudaStream_t stream = (cudaStream_t)stream_;
-  std::vector<Phase> prog;
-  for (int i = 0; i < count; ++i)
-    for (int j = 0; j < span; ++j) {
-      Phase p = e->prog_frame[first + j];
-      if (p.type == PH_SAMPLE) continue;
-      prog.push_back(p);
-    }
-  const int n = (int)prog.size();
-  Phase* dev = nullptr;
-  Q3_CUDA(cudaMalloc(&dev, (size_t)n * sizeof(Phase)));
-  Q3_CUDA(cudaMemcpy(dev, prog.data(), (size_t)n * sizeof(Phase), cudaMemcpyHostToDevice));
-  Phase* saved = e->prog_dev;
-  e->prog_dev = dev;
-  const int nt = e->nt_frame;
-  SmemPlan plan;
-  PieceTable pt;
-  int rc = make_smem_plan(e, prog, e->B, nt, &plan);
-  if (!rc) rc = build_piece_table(e, prog, plan.slot_blocks, &pt);
-  cudaEvent_t e0, e1;
-  cudaEventCreate(&e0); cudaEventCreate(&e1);
-  if (!rc) rc = launch_program(e, 0, n, 0, 1, nt, plan, pt, nullptr, stream);  // warm
-  cudaEventRecord(e0, stream);
-  if (!rc) rc = launch_program(e, 0, n, 0, 1, nt, plan, pt, nullptr, stream);
-  cudaEventRecord(e1, stream);
-  cudaStreamSynchronize(stream);
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, e0, e1);
-  if (ms_out) *ms_out = ms;
-  e->prog_dev = saved;
-  e->release(pt.runs);
-  e->release(pt.off);
-  cudaFree(dev);
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
-  return rc;
 }
 
 extern "C" int q3_algorithmic_bytes(q3_engine* e, int32_t B, int32_t S, double* a_bytes, double* a_stream_bytes) {

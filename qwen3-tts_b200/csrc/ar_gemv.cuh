@@ -11,11 +11,7 @@ using q3ring::ProdIter;
 using q3ring::RunGeom;
 
 // ------------------------------------------------------------------------------------------------
-// grid barrier.  Two interchangeable implementations (KParams.flags bit 0):
-//   counter (default): release-red on one counter + relaxed poll by thread 0.
-//   flags            : every CTA owns one epoch word; arrive = st.release of the new epoch, wait = warp 0 polls all
-//                      gridDim words.  Every CTA polls every word, so the release costs grow with the grid;
-//                      kept as an A/B knob only.
+// grid barrier: release-red on one counter + relaxed poll by thread 0.
 // Polls are RELAXED on purpose: ld.acquire.gpu compiles to LDG.STRONG + CCTL.IVALL (a full L1 invalidation per
 // poll iteration).  Correctness does not need it: every cross-CTA read in this kernel is an L2 access
 // (ld.global.cg / cp.async.cg / cp.async.bulk), the writers released at gpu scope before their arrival became
@@ -27,45 +23,22 @@ __device__ __forceinline__ void barrier_timeout(DevState* st) {
   __trap();
 }
 
-__device__ __forceinline__ void grid_arrive(DevState* st, unsigned int& epoch, bool use_counter) {
+__device__ __forceinline__ void grid_arrive(DevState* st, unsigned int& epoch) {
   // caller: cta_sync() already executed (every thread's global writes happen-before thread 0's release)
   if (threadIdx.x == 0) {
-    if (use_counter) {
-      epoch += gridDim.x;
-      asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(&st->bar_count) : "memory");
-    } else {
-      epoch += 1;
-      asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(&st->bar_flags[blockIdx.x]), "r"(epoch) : "memory");
-    }
+    epoch += gridDim.x;
+    asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(&st->bar_count) : "memory");
   }
 }
 
-__device__ __forceinline__ void grid_wait(DevState* st, unsigned int epoch, bool use_counter) {
-  if (use_counter) {
-    if (threadIdx.x == 0) {
-      const long long t0 = clock64();
-      unsigned int v;
-      while (true) {
-        asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(&st->bar_count) : "memory");
-        if ((int)(v - epoch) >= 0) break;
-        if (clock64() - t0 > 8000000000LL) barrier_timeout(st);  // ~4 s: never hang the box
-      }
-    }
-  } else if (threadIdx.x < 32) {
+__device__ __forceinline__ void grid_wait(DevState* st, unsigned int epoch) {
+  if (threadIdx.x == 0) {
     const long long t0 = clock64();
-    const int n = (int)gridDim.x;
-    // thread 0 carries the epoch; broadcast it inside warp 0
-    const unsigned int ep = __shfl_sync(0xffffffffu, epoch, 0);
+    unsigned int v;
     while (true) {
-      bool ok = true;
-#pragma unroll 1
-      for (int i = threadIdx.x; i < n; i += 32) {
-        unsigned int v;
-        asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(&st->bar_flags[i]) : "memory");
-        ok = ok && ((int)(v - ep) >= 0);
-      }
-      if (__all_sync(0xffffffffu, ok)) break;
-      if (clock64() - t0 > 8000000000LL) barrier_timeout(st);
+      asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(&st->bar_count) : "memory");
+      if ((int)(v - epoch) >= 0) break;
+      if (clock64() - t0 > 8000000000LL) barrier_timeout(st);  // ~4 s: never hang the box
     }
   }
 }
@@ -75,7 +48,7 @@ __device__ __forceinline__ void cta_sync() { __syncthreads(); }
 
 // fine-grained profiling marks (thread 0 only, first frame of a profiled launch)
 __shared__ unsigned long long* g_prof_row;
-// (compiled only into the development instantiation: a constexpr bool DEV must be in scope)
+// (compiled only into the profiled instantiation: a constexpr bool DEV must be in scope)
 #define PROF_MARK(k)                                                                   \
   do {                                                                                 \
     if constexpr (DEV) if (threadIdx.x == 0 && g_prof_row) {                           \
@@ -174,7 +147,6 @@ __device__ __forceinline__ void ring_init(Ring& rg, const uint2* list, int len, 
 }
 
 // request the next piece (<= SB blocks of the current run) into slot p_slot; lane 0 issues, every lane keeps the books
-template <bool DEV>
 __device__ __forceinline__ void ring_issue(Ring& rg, const KParams& P, int lane, uint64_t pol_stream, uint64_t pol_keep) {
   if (rg.cur_left == 0) {
     if (rg.runs_left <= 0) return;
@@ -193,8 +165,7 @@ __device__ __forceinline__ void ring_issue(Ring& rg, const KParams& P, int lane,
     // address-hashed fraction evict_last (the code predictor's layer weights are re-read on each of its 15 passes:
     // what stays in L2 is not re-fetched from HBM)
     const uint64_t pol = rg.cur_keep ? pol_keep : pol_stream;
-    if (DEV && (P.flags & 4)) bulk_g2s_plain(rg.slots + (uint32_t)(rg.p_slot * rg.SB) * 1024u, src, bytes, bar);
-    else bulk_g2s(rg.slots + (uint32_t)(rg.p_slot * rg.SB) * 1024u, src, bytes, bar, pol);
+    bulk_g2s(rg.slots + (uint32_t)(rg.p_slot * rg.SB) * 1024u, src, bytes, bar, pol);
   }
   rg.cur_off += (uint32_t)nb << 6;
   rg.cur_left -= nb;
@@ -202,12 +173,11 @@ __device__ __forceinline__ void ring_issue(Ring& rg, const KParams& P, int lane,
   ++rg.outstanding;
 }
 
-template <bool DEV>
 __device__ __forceinline__ void ring_release(Ring& rg, const KParams& P, int lane, uint64_t pol_stream, uint64_t pol_keep) {
   __syncwarp();  // every lane's reads of the slot are done before the async proxy overwrites it
   if (++rg.c_slot == rg.R) { rg.c_slot = 0; rg.c_par ^= 1; }
   --rg.outstanding;
-  ring_issue<DEV>(rg, P, lane, pol_stream, pol_keep);
+  ring_issue(rg, P, lane, pol_stream, pol_keep);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -374,8 +344,8 @@ __device__ __forceinline__ void flush_acc(float (&acc)[NACC][NT][4], float* pp, 
 // The phase body.  `m` is this CTA's meta of the phase (tiles owned, K blocks); the weights arrive through the ring.
 // HID: the kernel instantiation that also captures the per-step hidden states (generate(return_hidden=True)); the
 // default instantiation does not carry that code — the phase loop's instruction footprint is a first-order term
-// (it exceeds the instruction cache, so every line it carries costs).  DEV: the development instantiation with the
-// device-timestamp marks and the ablation / A-B knobs of KParams::flags; production kernels carry none of it.
+// (it exceeds the instruction cache, so every line it carries costs).  DEV: the profiled instantiation with the
+// device-timestamp marks and ring-wait clocks; production kernels carry none of it.
 template <int NT, bool HID, bool DEV>
 __device__ __forceinline__ uint32_t gemv_phase(const Phase& ph, const PMeta m, const KParams& P, Ring& rg, unsigned char* smem,
                                                RoundTab* tab, uint32_t xbar, uint32_t xpar, uint64_t pol_stream, uint64_t pol_keep, int frame) {
@@ -400,7 +370,7 @@ __device__ __forceinline__ uint32_t gemv_phase(const Phase& ph, const PMeta m, c
   const uint32_t xs_sh = smem_addr(xs);
 
   // ---- activations -> shared memory
-  if (staged && (ntc > 0 || save) && !(DEV && (P.flags & 32))) {
+  if (staged && (ntc > 0 || save)) {
     if (normed) {
       stage_columns(src, src_ld, ph.eps, save, P.mode == 0 ? P.admit_mask : 0xffffffffu, K, nc, xs, xstride, nw_s,
                     (HID && save) ? P.hid_out : nullptr, P.hid_stride, P.mode == 0 ? 0 : frame + 1, P.frame0);
@@ -492,10 +462,7 @@ __device__ __forceinline__ uint32_t gemv_phase(const Phase& ph, const PMeta m, c
         mbar_wait(rg.full + 8u * rg.c_slot, (uint32_t)rg.c_par, P.st);
         if (DEV && g_prof_row && tid == 0) wait_cycles += clock64() - w0;
         const uint32_t sp = rg.slots + (uint32_t)(rg.c_slot * rg.SB) * 1024u + (uint32_t)lane * 16u;
-        if (DEV && (P.flags & 64)) {
-          kbi += nb;  // (experiment: consume the ring without touching the data)
-          if (kbi > KB) kbi -= KB;
-        } else if (full) {
+        if (full) {
           // a full piece inside one tile: all fragment loads are issued back to back, then 8 MMAs per n-tile on
           // independent accumulators
           if (staged) {
@@ -506,10 +473,8 @@ __device__ __forceinline__ uint32_t gemv_phase(const Phase& ph, const PMeta m, c
               for (int n = 0; n < NT; ++n)
                 if (i < nb && n < nct) bq[i][n] = lds128(xb + (uint32_t)(i * 64 + n * 8 * xstride));
           }
-          if (!(DEV && (P.flags & 16))) {  // (flag 16: experiment, skip the tensor work)
-            if (PB == 4 && nb == 4) piece_full<NT, NACC, PB>(acc, sp, bq, nct);
-            else piece_full<NT, NACC, 2>(acc, sp, bq, nct);
-          }
+          if (PB == 4 && nb == 4) piece_full<NT, NACC, PB>(acc, sp, bq, nct);
+          else piece_full<NT, NACC, 2>(acc, sp, bq, nct);
           kbi += nb;
         } else {
           // general path (tiny test shapes, a tile boundary inside the piece): one block at a time, rolled
@@ -538,7 +503,7 @@ __device__ __forceinline__ uint32_t gemv_phase(const Phase& ph, const PMeta m, c
           kbi = 0;
           ++seg;
         }
-        ring_release<DEV>(rg, P, lane, pol_stream, pol_keep);
+        ring_release(rg, P, lane, pol_stream, pol_keep);
         if (!staged) {
 #pragma unroll
           for (int i = 0; i < PB; ++i)
@@ -557,7 +522,7 @@ __device__ __forceinline__ uint32_t gemv_phase(const Phase& ph, const PMeta m, c
     PROF_MARK(3);
     // ---- cross-warp reduce + epilogue, one output element per thread-iteration
 #pragma unroll 1
-    for (int e = tid, it = 0; e < ((DEV && (P.flags & 128)) ? 0 : nelem); e += NTHREADS, ++it) {
+    for (int e = tid, it = 0; e < nelem; e += NTHREADS, ++it) {
       const int r = e & ((1 << rsh) - 1);
       const int tl = (e >> rsh) & ((1 << tbl) - 1);
       const int col = e >> (rsh + tbl);

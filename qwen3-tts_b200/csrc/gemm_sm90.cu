@@ -7,8 +7,6 @@
 //   warp 8    : TMA producer (A tile via a 3-D map with a per-tap row shift, W tile via a 2-D map)
 #include "gemm_sm90.cuh"
 #include <algorithm>
-#include <cstdio>
-#include <cstdlib>
 #include <cstring>
 
 namespace {
@@ -382,10 +380,6 @@ int gemm_pick_bn(int N, int mtiles, int B) {
 int gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
   const long long total = (long long)((plan.T + BM - 1) / BM) * ((plan.N + plan.bn - 1) / plan.bn) * plan.B;
   const int grid = (int)std::min<long long>(total, g_sm_count);  // persistent: one CTA per SM walks the tiles
-  static const bool trace = getenv("Q3_GEMM_TRACE") != nullptr;  // shape of every launch, for per-layer timing breakdowns
-  if (trace)
-    fprintf(stderr, "[tap_gemm] B=%d T=%d N=%d Kp=%d taps=%d bn=%d tiles=%lld act=%d resid=%d\n", plan.B, plan.T, plan.N, plan.Kp,
-            plan.ntaps, plan.bn, total, plan.ep.act, plan.ep.resid ? 1 : 0);
   const int smem_bytes = 1024 + plan.nst * stage_bytes_for(plan.bn) + BAR_BYTES;
   if (plan.bn == 128) {
     if (launch_bn<128>(plan, grid, smem_bytes, stream)) return 1;

@@ -295,6 +295,38 @@ def test_long_context_cross_cta_split_attention():
         eng.close()
 
 
+def test_profiled_decode_matches_production_decode():
+    """The profiled kernel instantiation (selected while a profile buffer is registered) samples the same codes as the
+    production one from the same prefill and seed, and writes ordered device timestamps for every phase and CTA."""
+    cfg = _tiny()
+    Wb, _ = Hh.bf16_weights(OT.random_weights(cfg, seed=15))
+    lens = [6, 10, 4]
+    B, N, G = len(lens), 5, cfg.num_code_groups
+    embs, trail, pad = Hh.make_inputs(cfg, lens, [1, 0, 2], seed=16)
+    sp = Hh.to_pkg_sampling(OT.SamplingCfg(do_sample=True, subtalker_dosample=True, max_new_tokens=N + 1,
+                                           suppress_eos=True, seed=5))
+    eng = _engine(cfg, Wb)
+    runs = []
+    for profiled in (False, True):
+        eng.prefill(embs, trail, pad, sp)
+        codes = torch.zeros(B, N + 1, G, dtype=torch.int32, device=DEV)
+        if profiled:
+            kinds, t_end, t_bar, _ = eng.profile_frame(N, codes)
+        else:
+            eng.decode(N, codes)
+            torch.cuda.synchronize()
+        assert eng.progress()[0] == N
+        runs.append(codes.cpu().numpy())
+    assert (runs[0] == runs[1]).all()
+    t = eng.last_profile_all  # [phase][cta][16]
+    assert t.shape[0] == len(kinds) > 0
+    end, passed = t[:, :, 0], t[:, :, 1]
+    assert (end > 0).all() and (passed > 0).all()
+    assert (end <= passed).all()
+    assert (passed[:-1] <= end[1:]).all()  # a CTA starts phase i + 1 only after passing barrier i
+    eng.close()
+
+
 def test_per_step_hidden_states_second_return_value():
     """generate()'s second return (modeling_qwen3_tts.py:2281,2290): the final-norm hidden state of the newest position
     of every step.  Check: codec_head(hidden[s]) reproduces the step's own raw logits, for every row and step."""

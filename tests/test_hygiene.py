@@ -34,6 +34,12 @@ def test_gpu_tests_bench_and_smoke_do_not_read_the_reference_tree():
             assert "ref_shims" not in src and "ref_driver" not in src and "/root/reference" not in src, f
 
 
+def test_native_library_reads_no_environment_variables():
+    csrc = os.path.join(ROOT, "qwen3-tts_b200", "csrc")
+    bad = [f for f in _py_files(csrc) if re.search(r"\bgetenv\s*\(", open(f, encoding="utf-8").read())]
+    assert not bad, f"native sources read environment variables: {bad}"
+
+
 def test_no_cpu_fallback_in_product_entry_points():
     eng = open(os.path.join(ROOT, "qwen3-tts_b200", "engine.py")).read()
     cod = open(os.path.join(ROOT, "qwen3-tts_b200", "codec.py")).read()
