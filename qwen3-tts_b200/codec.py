@@ -93,6 +93,11 @@ class CodecDecoder:
         out[:, :k] = w
         return out
 
+    @staticmethod
+    def _gate_up_pair(gate, up):
+        """gate, up [I][K] -> [2I][K] with rows (gate_i, up_i) adjacent (ACT_SWIGLU_PAIR)."""
+        return torch.stack([gate, up], 1).reshape(2 * gate.shape[0], gate.shape[1])
+
     def _snake(self, name, alpha, beta):
         self._f(name + "_ea", torch.exp(alpha.float()))
         self._f(name + "_ib", 1.0 / (torch.exp(beta.float()) + 1e-9))
@@ -123,8 +128,7 @@ class CodecDecoder:
             qkv = torch.cat([g(f"{lp}.self_attn.q_proj.weight"), g(f"{lp}.self_attn.k_proj.weight"), g(f"{lp}.self_attn.v_proj.weight")], 0)
             self._w(f"{q}.qkv.w", self._lin_w(qkv))
             self._w(f"{q}.o.w", self._lin_w(g(f"{lp}.self_attn.o_proj.weight")))
-            gate, up = g(f"{lp}.mlp.gate_proj.weight"), g(f"{lp}.mlp.up_proj.weight")
-            gu = torch.stack([gate, up], 1).reshape(2 * gate.shape[0], gate.shape[1])  # rows (gate_i, up_i) adjacent
+            gu = self._gate_up_pair(g(f"{lp}.mlp.gate_proj.weight"), g(f"{lp}.mlp.up_proj.weight"))
             self._w(f"{q}.gate_up.w", self._lin_w(gu))
             self._w(f"{q}.down.w", self._lin_w(g(f"{lp}.mlp.down_proj.weight")))
             self._w(f"{q}.ln1", g(f"{lp}.input_layernorm.weight"))

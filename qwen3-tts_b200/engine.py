@@ -60,6 +60,12 @@ class AREngine:
             x = x[None]
         _lib.check(self.lib.q3_engine_load_tensor(self.h, name.encode(), x.data_ptr(), x.shape[0], x.shape[1]))
 
+    @staticmethod
+    def _gate_up_blk8(gate, up):
+        """gate, up [I][K] -> [2I][K] in blocks of 16 rows: gate rows 8i..8i+7, then up rows 8i..8i+7 (ACT_SWIGLU_BLK8)."""
+        I, K = gate.shape
+        return torch.stack([gate.view(I // 8, 8, K), up.view(I // 8, 8, K)], 1).reshape(2 * I, K)
+
     def _load(self, W):
         cfg = self.cfg
 
@@ -69,10 +75,7 @@ class AREngine:
                 g = lambda n: W[f"{p}.{n}.weight"].to(self.device, torch.bfloat16)  # noqa: E731
                 self._put(f"{q}.qkv", torch.cat([g("self_attn.q_proj"), g("self_attn.k_proj"), g("self_attn.v_proj")], 0))
                 self._put(f"{q}.o", g("self_attn.o_proj"))
-                gate, up = g("mlp.gate_proj"), g("mlp.up_proj")
-                I, K = gate.shape
-                gu = torch.stack([gate.view(I // 8, 8, K), up.view(I // 8, 8, K)], 1).reshape(2 * I, K)
-                self._put(f"{q}.gate_up", gu)
+                self._put(f"{q}.gate_up", self._gate_up_blk8(g("mlp.gate_proj"), g("mlp.up_proj")))
                 self._put(f"{q}.down", g("mlp.down_proj"))
                 self._put(f"{q}.ln1", g("input_layernorm"))
                 self._put(f"{q}.ln2", g("post_attention_layernorm"))

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 tap-GEMM codec decoder against the CPU oracle (through the C ABI)."""
+"""GPU parity of the wgmma tap-GEMM codec decoder against the CPU oracle (through the C ABI)."""
 import numpy as np
 import pytest
 import torch
