@@ -193,7 +193,7 @@ int q3_codec_stream_reset(q3_codec_stream* s, void* stream);
 int q3_codec_stream_position(q3_codec_stream* s);
 void q3_codec_stream_close(q3_codec_stream* s);
 int q3_codec_total_upsample(q3_codec* c);
-/* kernels launched by the last q3_codec_forward (bench.py's gpu_launches bookkeeping) */
+/* kernels launched by the last q3_codec_forward or q3_codec_stream_step (bench.py's gpu_launches bookkeeping) */
 int q3_codec_last_launch_count(q3_codec* c);
 /* Test hook (tests/ only): per-stage capture of the DECODER, so that an error in one small kernel cannot hide behind the
  * waveform SNR.  The following q3_codec_forward calls copy the bf16 [B][T_stage][C_stage] tensor of `stage` into dst_dev

@@ -1,5 +1,7 @@
 """Stateful streaming codec decoder (q3_codec_stream_*, SURVEY §8b / §8f-2) against the engine's own one-shot causal
 forward and against the CPU oracle's streaming spec (oracle/codec.py::StreamingDecoder)."""
+import dataclasses
+
 import numpy as np
 import pytest
 import torch
@@ -65,4 +67,21 @@ def test_full_config_stream_packets_of_4():
     ref = OC.decoder_forward(Wf, cfg, codes)
     assert _snr_db(ref, got) > 22.0
     st.close()
+    dec.close()
+
+
+@pytest.mark.parametrize("layers,ok", [(27, True), (28, False)])
+def test_open_bounds_history_buffers_by_the_roll_table(layers, ok):
+    """One launch after every packet rolls all history buffers (pre, in, out, one K/V window per layer, one per
+    upsampling stage, four per decoder block) from a table of 48 entries. Open accepts 3 + 27 + 2 + 16 = 48 buffers
+    and refuses 49 with an error instead of overrunning the table. Open only: nothing is stepped."""
+    from qwen3_tts_b200.codec import CodecDecoder
+    cfg = dataclasses.replace(_small_cfg(), num_layers=layers)
+    Wb, _ = _bf16_round(OC.random_weights(cfg, seed=3))
+    dec = CodecDecoder(_pkg_cfg(cfg), Wb, device=DEV, max_frames=64)
+    if ok:
+        dec.open_stream(2, max_packet_frames=4).close()
+    else:
+        with pytest.raises(RuntimeError, match="49 history buffers"):
+            dec.open_stream(2, max_packet_frames=4)
     dec.close()

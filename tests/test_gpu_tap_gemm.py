@@ -548,6 +548,7 @@ def codec_sites(Cd=64, Cl=96, Hh=128, I=160, C=192, T=150):
         "dec.in": Case(T=T, K=Cl, N=C, shifts=tuple(range(-6, 1)), act=ACT_SNAKE, raw=False),
         "dec.c1": Case(T=T, K=Co, N=Co, shifts=tuple(-(6 - j) * 9 for j in range(7)), act=ACT_SNAKE, raw=False, big=128),
         "dec.c2": Case(T=T, K=Co, N=Co, resid="sep", act=ACT_SNAKE, big=128),
+        "dec.c2.inplace": Case(T=T, K=Co, N=Co, resid="inplace", act=ACT_SNAKE, big=128),   # the residual stream in place
         # streaming: history-prefixed inputs and outputs inside larger per-row buffers
         "s.rvq.proj": Case(T=T, K=Cd, N=Cd, bias=False, pad=7),
         "s.pre_conv": Case(T=T, K=Cd, N=Cl, shifts=(-2, -1, 0), hist=2, pad=3),
@@ -557,6 +558,7 @@ def codec_sites(Cd=64, Cl=96, Hh=128, I=160, C=192, T=150):
         "s.dec.c1": Case(T=T, K=Co, N=Co, shifts=tuple(-(6 - j) * 9 for j in range(7)), act=ACT_SNAKE, raw=False,
                          hist=54, pad=54, big=128),
         "s.dec.c2": Case(T=T, K=Co, N=Co, resid="sep", act=ACT_SNAKE, pad=9),
+        "s.dec.c2.inplace": Case(T=T, K=Co, N=Co, resid="inplace", act=ACT_SNAKE, pad=9),
         # SwiGLU gates out to +-100 (exp overflow must give 0, not NaN), with a gate/up bias
         "gate_up.pair.big": Case(T=T, K=Hh, N=2 * I, act=ACT_SWIGLU_PAIR, raw=False, big=64),
         "gate_up.blk8.big": Case(T=T, K=Hh, N=2 * I, act=ACT_SWIGLU_BLK8, raw=False, big=64),
