@@ -56,7 +56,12 @@ typedef struct {
   int32_t device;            /* CUDA ordinal */
 } q3_engine_cfg;
 
-/* Generation kwargs of seam B (modeling_qwen3_tts.py:2044-2066; defaults inference/qwen3_tts_model.py:287-352). */
+/* Generation kwargs of seam B (modeling_qwen3_tts.py:2044-2066; defaults inference/qwen3_tts_model.py:287-352).
+ * Accepted ranges (HF's processors, plus finiteness where the sampler needs it); q3_prefill and q3_session_begin reject
+ * anything else with an error naming the field, before any device work:
+ *   temperature / subtalker_temperature: finite and > 0 when do_sample / subtalker_dosample is set (ignored otherwise);
+ *   top_k, subtalker_top_k >= 0 (0 = off); 0 <= top_p, subtalker_top_p <= 1 (1 = off);
+ *   repetition_penalty finite and > 0 (1 = off); min_new_tokens >= 0. */
 typedef struct {
   int32_t do_sample, top_k;
   float top_p, temperature, repetition_penalty;

@@ -24,6 +24,7 @@
 #include <cooperative_groups.h>
 #include <stdarg.h>
 #include <algorithm>
+#include <cmath>
 #include <map>
 #include <vector>
 
@@ -817,10 +818,31 @@ static int ensure_trailing(q3_engine* e, int stride, cudaStream_t stream) {
   return 0;
 }
 
+// The ranges HF's processors accept, plus finiteness where the sample phase needs it: a temperature of 0, a negative or
+// non-finite one, or a repetition penalty of 0 turns scores into NaN, and the phase would then find no token at all.
+static int check_sampling(const q3_sampling& s) {
+  Q3_REQUIRE(!s.do_sample || (std::isfinite(s.temperature) && s.temperature > 0.f),
+             "sampling: temperature %g must be finite and > 0 when do_sample is set", (double)s.temperature);
+  Q3_REQUIRE(!s.subtalker_dosample || (std::isfinite(s.subtalker_temperature) && s.subtalker_temperature > 0.f),
+             "sampling: subtalker_temperature %g must be finite and > 0 when subtalker_dosample is set",
+             (double)s.subtalker_temperature);
+  Q3_REQUIRE(s.top_k >= 0, "sampling: top_k %d must be >= 0", s.top_k);
+  Q3_REQUIRE(s.subtalker_top_k >= 0, "sampling: subtalker_top_k %d must be >= 0", s.subtalker_top_k);
+  Q3_REQUIRE(s.top_p >= 0.f && s.top_p <= 1.f, "sampling: top_p %g must be in [0, 1]", (double)s.top_p);
+  Q3_REQUIRE(s.subtalker_top_p >= 0.f && s.subtalker_top_p <= 1.f, "sampling: subtalker_top_p %g must be in [0, 1]",
+             (double)s.subtalker_top_p);
+  Q3_REQUIRE(std::isfinite(s.repetition_penalty) && s.repetition_penalty > 0.f,
+             "sampling: repetition_penalty %g must be finite and > 0", (double)s.repetition_penalty);
+  Q3_REQUIRE(s.min_new_tokens >= 0, "sampling: min_new_tokens %d must be >= 0", s.min_new_tokens);
+  return 0;
+}
+
 extern "C" int q3_prefill(q3_engine* e, int32_t B, const void* embeds_dev, const int32_t* lens_host,
                           const void* trailing_dev, const int32_t* trailing_lens_host, int32_t trailing_stride,
                           const void* tts_pad_dev, const q3_sampling* sp, void* stream_) {
   Q3_REQUIRE(e && e->finalized, "engine not finalized");
+  Q3_REQUIRE(sp, "null argument");
+  if (check_sampling(*sp)) return 1;
   Q3_REQUIRE(B >= 1 && B <= e->cfg.max_batch, "batch %d out of range", B);
   Q3_REQUIRE(embeds_dev && lens_host && tts_pad_dev && sp, "null argument");
   Q3_CUDA(cudaSetDevice(e->cfg.device));
@@ -861,6 +883,8 @@ extern "C" int q3_prefill(q3_engine* e, int32_t B, const void* embeds_dev, const
 extern "C" int q3_session_begin(q3_engine* e, int32_t n_slots, int32_t max_trailing, const void* tts_pad_dev, const q3_sampling* sp,
                                 void* stream_) {
   Q3_REQUIRE(e && e->finalized, "engine not finalized");
+  Q3_REQUIRE(sp, "bad argument");
+  if (check_sampling(*sp)) return 1;
   Q3_REQUIRE(n_slots >= 1 && n_slots <= e->cfg.max_batch, "n_slots %d out of range", n_slots);
   Q3_REQUIRE(tts_pad_dev && sp && max_trailing >= 0, "bad argument");
   Q3_CUDA(cudaSetDevice(e->cfg.device));

@@ -112,58 +112,82 @@ def test_free_running_greedy_matches_oracle():
     eng.close()
 
 
+# Configurations that route q3_step_kernel's sample phase through each of its paths on the engine's own logits: the
+# fast top-k path, its bin-0 fallback (T = 0.02 spreads the scores far beyond max - 32), the radix select (k > 128), the
+# full-vocabulary generic path, top-p with and without top-k, the repetition penalty, min_new_tokens without
+# suppress_eos, and greedy.
+ENGINE_SAMPLING = {
+    "k50_T0.9": dict(top_k=50, temperature=0.9),
+    "k50_T0.02": dict(top_k=50, temperature=0.02),
+    "k200": dict(top_k=200, temperature=0.9),
+    "k0_T3": dict(top_k=0, temperature=3.0),
+    "p0.8_k0": dict(top_k=0, top_p=0.8, temperature=0.9),
+    "p0.8_k50": dict(top_k=50, top_p=0.8, temperature=0.9),
+    "penalty1.3": dict(top_k=50, temperature=0.9, repetition_penalty=1.3),
+    "min_new5": dict(top_k=50, temperature=0.9, min_new_tokens=5),
+    "greedy": dict(do_sample=False),
+}
+
+
 def test_sampler_against_oracle_on_engine_logits():
     """Sampling (rep-penalty, min-new-tokens, suppress, temperature, top-k, top-p, inverse CDF with Philox
-    uniforms): feed the ENGINE's own captured logits to the oracle's sampler and require the same tokens."""
+    uniforms) inside the production kernel, in every configuration of ENGINE_SAMPLING: feed the ENGINE's own captured
+    logits to the oracle's sampler.  Tokens are held to the rule of tests/test_gpu_sampler.py: greedy exact; a sampled
+    token in the oracle's kept set and equal to the inverse-CDF token unless u * total lies within the stated fp32 bound
+    of the boundary between the two."""
     cfg = _tiny()
     Wb, _ = Hh.bf16_weights(OT.random_weights(cfg, seed=6))
+    eng = _engine(cfg, Wb)
+    for name in sorted(ENGINE_SAMPLING):
+        _sample_on_engine_logits(eng, cfg, name)
+    eng.close()
+
+
+def _sample_on_engine_logits(eng, cfg, name):
+    from tests.test_gpu_sampler import sampled_token_error
     lens = [5, 8, 13]
     B, N, G = len(lens), 12, cfg.num_code_groups
     embs, trail, pad = Hh.make_inputs(cfg, lens, [1, 2, 0], seed=9)
-    for top_p, seed in ((1.0, 11), (0.8, 12)):
-        sp = OT.SamplingCfg(do_sample=True, subtalker_dosample=True, top_k=50, top_p=top_p, temperature=0.9,
-                            subtalker_top_k=50, subtalker_top_p=top_p, subtalker_temperature=0.9,
-                            repetition_penalty=1.05, max_new_tokens=N + 1, seed=seed)
-        eng = _engine(cfg, Wb)
-        V, Vc = cfg.talker.vocab_size, cfg.cp.vocab_size
-        tl = torch.zeros(N + 1, B, V, dtype=torch.float32, device=DEV)
-        cl = torch.zeros(N, G - 1, B, Vc, dtype=torch.float32, device=DEV)
-        eng.set_debug(None, 0, tl, cl)
-        eng.prefill(embs, trail, pad, Hh.to_pkg_sampling(sp))
-        codes = torch.zeros(B, N + 1, G, dtype=torch.int32, device=DEV)
-        eng.decode(N, codes)
-        torch.cuda.synchronize()
-        fd, n_valid, fin = eng.progress()
-        codes, tl, cl = codes.cpu().numpy(), tl.cpu().numpy(), cl.cpu().numpy()
-        lp = OT.talker_logits_processors(cfg, sp)
-        mism = 0
-        for b in range(B):
-            gen = []
-            for f in range(min(fd, N)):
-                s = OS.process_logits(tl[f, b], generated_ids=gen, **lp)
-                u = philox.uniform(sp.seed, b, f, 0)
-                tok, cdf = OS.sample_from_scores(s, do_sample=True, u=u)
-                got = int(codes[b, f, 0])
-                if tok != got:
-                    # only tolerated on a CDF boundary (fp32 scan order vs fp64 cumsum)
-                    lo = cdf[got - 1] if got > 0 else 0.0
-                    assert min(abs(u - lo), abs(u - cdf[got])) < 1e-4, (b, f, tok, got, u)
-                    mism += 1
-                gen.append(got)
-                if got == cfg.codec_eos_token_id:
-                    break
-                for j in range(G - 1):
-                    s = OS.process_logits(cl[f, j, b], do_sample=True, temperature=sp.subtalker_temperature,
-                                          top_k=sp.subtalker_top_k, top_p=sp.subtalker_top_p)
-                    u = philox.uniform(sp.seed, b, f, j + 1)
-                    tok, cdf = OS.sample_from_scores(s, do_sample=True, u=u)
-                    got = int(codes[b, f, j + 1])
-                    if tok != got:
-                        lo = cdf[got - 1] if got > 0 else 0.0
-                        assert min(abs(u - lo), abs(u - cdf[got])) < 1e-4, (b, f, j, tok, got, u)
-                        mism += 1
-        assert mism <= 3
-        eng.close()
+    kw = ENGINE_SAMPLING[name]
+    do_sample = kw.get("do_sample", True)
+    top_k, top_p, T = kw.get("top_k", 50), kw.get("top_p", 1.0), kw.get("temperature", 0.9)
+    sp = OT.SamplingCfg(do_sample=do_sample, subtalker_dosample=do_sample, top_k=top_k, top_p=top_p, temperature=T,
+                        subtalker_top_k=top_k, subtalker_top_p=top_p, subtalker_temperature=T,
+                        repetition_penalty=kw.get("repetition_penalty", 1.05), min_new_tokens=kw.get("min_new_tokens", 2),
+                        max_new_tokens=N + 1, seed=11 + len(name))
+    V, Vc = cfg.talker.vocab_size, cfg.cp.vocab_size
+    tl = torch.zeros(N + 1, B, V, dtype=torch.float32, device=DEV)
+    cl = torch.zeros(N, G - 1, B, Vc, dtype=torch.float32, device=DEV)
+    eng.set_debug(None, 0, tl, cl)
+    eng.prefill(embs, trail, pad, Hh.to_pkg_sampling(sp))
+    codes = torch.zeros(B, N + 1, G, dtype=torch.int32, device=DEV)
+    eng.decode(N, codes)
+    torch.cuda.synchronize()
+    fd, n_valid, fin = eng.progress()
+    codes, tl, cl = codes.cpu().numpy(), tl.cpu().numpy(), cl.cpu().numpy()
+    lp = OT.talker_logits_processors(cfg, sp)
+
+    def check(raw, proc, u, got, what):
+        s = proc(raw, top_p)
+        if not do_sample:
+            assert got == int(np.argmax(s)), (what, got, int(np.argmax(s)))
+            return
+        err = sampled_token_error(s, proc(raw, 1.0) if top_p < 1.0 else None, top_p, u, got)
+        assert err is None, (what, err)
+
+    for b in range(B):
+        gen = []
+        for f in range(min(fd, N)):
+            got = int(codes[b, f, 0])
+            check(tl[f, b], lambda x, p: OS.process_logits(x, generated_ids=gen, **dict(lp, top_p=p)),
+                  philox.uniform(sp.seed, b, f, 0), got, (name, b, f, 0))
+            gen.append(got)
+            if got == cfg.codec_eos_token_id:
+                break
+            for j in range(G - 1):
+                check(cl[f, j, b], lambda x, p: OS.process_logits(x, do_sample=do_sample, temperature=T, top_k=top_k, top_p=p),
+                      philox.uniform(sp.seed, b, f, j + 1), int(codes[b, f, j + 1]), (name, b, f, j + 1))
+    eng.set_debug(None, 0, None, None)
 
 
 def test_full_shape_1p7b_two_frames():
