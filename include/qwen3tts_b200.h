@@ -190,12 +190,27 @@ int q3_codec_forward(q3_codec* c, const int32_t* codes_dev, int32_t B, int32_t T
  * (…v2.py:869-884) over everything pushed, with only the NEW frames' work per packet.
  * open: B rows, packets of <= max_packet_frames frames.  step: codes_dev int32 [B][num_quantizers][n] (the next n
  * frames of every row) -> wav_dev fp32 [B][n * total_upsample]; asynchronous on `stream`.  reset: start new
- * utterances in all rows.  The position (frames pushed) must stay below the engine's max_frames (RoPE table). */
+ * utterances in all rows.  A row's position (frames pushed since its reset) may not pass the engine's max_frames (RoPE
+ * table).
+ * Per row (continuous batching: rows start and end at different frames, slots are reused):
+ * step_rows: row b takes only the first counts_host[b] (0 <= counts_host[b] <= n, host int32 [B]) of the n frames in
+ *   codes_dev; its audio is wav_dev[b][0, counts_host[b] * total_upsample) and the rest of its row is zeros.  Codes past
+ *   a row's count are never read (any value, -1 included).  A row with count 0 keeps its state and position.
+ *   q3_codec_stream_step(s, codes, n, wav, stream) is step_rows with every count n.
+ * reset_rows: the n rows in rows_host (host int32, each in [0, B), no repeats) start new utterances at position 0;
+ *   the other rows are untouched.
+ * position: the common position of all rows, or -1 (q3_last_error says why) when rows differ; row_position: one row's.
+ * Bad arguments (a count outside [0, n], position + count > max_frames, a reset row out of range or listed twice, null
+ * pointers) are rejected with an error naming the row before any device work, and leave every position unchanged. */
 typedef struct q3_codec_stream q3_codec_stream;
 int q3_codec_stream_open(q3_codec* c, int32_t B, int32_t max_packet_frames, q3_codec_stream** out);
 int q3_codec_stream_step(q3_codec_stream* s, const int32_t* codes_dev, int32_t n, float* wav_dev, void* stream);
+int q3_codec_stream_step_rows(q3_codec_stream* s, const int32_t* codes_dev, int32_t n, const int32_t* counts_host,
+                              float* wav_dev, void* stream);
 int q3_codec_stream_reset(q3_codec_stream* s, void* stream);
+int q3_codec_stream_reset_rows(q3_codec_stream* s, int32_t n, const int32_t* rows_host, void* stream);
 int q3_codec_stream_position(q3_codec_stream* s);
+int q3_codec_stream_row_position(q3_codec_stream* s, int32_t row);
 void q3_codec_stream_close(q3_codec_stream* s);
 int q3_codec_total_upsample(q3_codec* c);
 /* kernels launched by the last q3_codec_forward or q3_codec_stream_step (bench.py's gpu_launches bookkeeping) */

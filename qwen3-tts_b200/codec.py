@@ -10,7 +10,7 @@ on libqwen3tts_b200.so.  The reference state_dict is re-laid-out here into the e
 """
 import ctypes as C
 import math
-from typing import List
+from typing import List, Optional, Sequence
 
 import torch
 
@@ -263,7 +263,8 @@ class CodecDecoder:
 
 class CodecStream:
     """Handle on a q3_codec_stream (conv tails, ConvTranspose overlap rows and 71 frames of rotated K/V per transformer
-    layer live on the device).  `push(codes (B,K,n))` -> wav (B,1,n*upsample) of those n frames."""
+    layer live on the device).  `push(codes (B,K,n))` -> wav (B,1,n*upsample) of those n frames.  Every row has its
+    own position: `push(codes, counts)` advances row b by counts[b] frames only, and `reset(rows)` restarts some rows."""
 
     def __init__(self, dec: CodecDecoder, batch: int, max_packet_frames: int = 8):
         self.dec, self.B, self.nmax = dec, int(batch), int(max_packet_frames)
@@ -273,28 +274,53 @@ class CodecStream:
 
     @property
     def position(self) -> int:
+        """Frames pushed since the last reset, common to all rows (-1 when rows differ: see `positions`)."""
         return int(self.dec.lib.q3_codec_stream_position(self.h))
 
+    @property
+    def positions(self) -> List[int]:
+        """Frames pushed to each row since its last reset."""
+        return [int(self.dec.lib.q3_codec_stream_row_position(self.h, b)) for b in range(self.B)]
+
     @torch.no_grad()
-    def push(self, codes: torch.Tensor) -> torch.Tensor:
+    def push(self, codes: torch.Tensor, counts: Optional[Sequence[int]] = None) -> torch.Tensor:
+        """codes (B,K,n) -> wav (B,1,n*upsample).  With `counts`, row b takes only its first counts[b] frames
+        (0 <= counts[b] <= n; the codes past them are never read): its audio is wav[b, 0, :counts[b]*upsample] and
+        the rest of its row is zeros."""
         dec = self.dec
         if codes.dim() != 3 or codes.shape[0] != self.B or codes.shape[1] != dec.cfg.num_quantizers:
             raise ValueError(f"expected codes of shape ({self.B}, {dec.cfg.num_quantizers}, n), got {tuple(codes.shape)}")
         n = int(codes.shape[2])
+        if counts is not None:
+            counts = [int(k) for k in counts]
+            if len(counts) != self.B:
+                raise ValueError(f"expected {self.B} counts, got {len(counts)}")
+            for b, k in enumerate(counts):
+                if not 0 <= k <= n:
+                    raise ValueError(f"row {b}: count {k} outside [0, {n}]")
         out = []
         for s0 in range(0, n, self.nmax):  # longer pushes are cut into packets of the stream's capacity
             c = codes[:, :, s0:s0 + self.nmax].to(dec.device, torch.int32).contiguous()
             m = int(c.shape[2])
             wav = torch.empty(self.B, m * dec.total_upsample, dtype=torch.float32, device=dec.device)
-            stream = torch.cuda.current_stream(dec.device).cuda_stream
-            _lib.check(dec.lib.q3_codec_stream_step(self.h, c.data_ptr(), m, wav.data_ptr(), C.c_void_p(stream)))
+            stream = C.c_void_p(torch.cuda.current_stream(dec.device).cuda_stream)
+            if counts is None:
+                _lib.check(dec.lib.q3_codec_stream_step(self.h, c.data_ptr(), m, wav.data_ptr(), stream))
+            else:  # a row's frames fill the packets in order: this packet holds frames s0 .. s0+m of the push
+                k = (C.c_int32 * self.B)(*[min(max(kb - s0, 0), m) for kb in counts])
+                _lib.check(dec.lib.q3_codec_stream_step_rows(self.h, c.data_ptr(), m, k, wav.data_ptr(), stream))
             self._keep = c
             out.append(wav)
         return torch.cat(out, 1)[:, None, :] if out else torch.zeros(self.B, 1, 0, device=dec.device)
 
-    def reset(self):
-        stream = torch.cuda.current_stream(self.dec.device).cuda_stream
-        _lib.check(self.dec.lib.q3_codec_stream_reset(self.h, C.c_void_p(stream)))
+    def reset(self, rows: Optional[Sequence[int]] = None):
+        """Start new utterances in `rows` (all rows when None); the other rows keep their state."""
+        stream = C.c_void_p(torch.cuda.current_stream(self.dec.device).cuda_stream)
+        if rows is None:
+            _lib.check(self.dec.lib.q3_codec_stream_reset(self.h, stream))
+        else:
+            rows = [int(r) for r in rows]
+            _lib.check(self.dec.lib.q3_codec_stream_reset_rows(self.h, len(rows), (C.c_int32 * max(len(rows), 1))(*rows), stream))
 
     def close(self):
         if getattr(self, "h", None):

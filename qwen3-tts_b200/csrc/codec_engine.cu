@@ -24,11 +24,22 @@ struct DevTensor {
 };
 
 // ---------------------------------------------------------------------------------------------- small kernels
-// RVQ decode (…v2.py:815-821, :721-727, :676-679): e[b][t][0:D] = table[0][c0]; e[b][t][D:2D] = sum_{k>=1} table[k][c_k]
+// Per-row frame window of a decode of n frames per row: rp[b] is row b's position (of its frame 0) and rp[B + b] its
+// count, the frames [0, count) that are its own; frames past the count are computed but are not part of the row's
+// stream.  rp == nullptr: every row at position 0 with all n frames (the one-shot forward).
+__device__ __forceinline__ int row_pos(const int* rp, int b) { return rp ? rp[b] : 0; }
+__device__ __forceinline__ int row_count(const int* rp, int B, int b, int n) { return rp ? rp[B + b] : n; }
+
+// RVQ decode (…v2.py:815-821, :721-727, :676-679): e[b][t][0:D] = table[0][c0]; e[b][t][D:2D] = sum_{k>=1} table[k][c_k].
+// A frame past its row's count reads no code and gets a zero embedding.
 __global__ void rvq_gather_kernel(const int* __restrict__ codes, const bf16* __restrict__ table, bf16* __restrict__ e,
-                                  int B, int K, int T, int D, int bins) {
+                                  int B, int K, int T, int D, int bins, const int* __restrict__ rp) {
   const int bt = blockIdx.x;  // b*T + t
   const int b = bt / T, t = bt % T;
+  if (t >= row_count(rp, B, b, T)) {
+    for (int d = threadIdx.x; d < 2 * D; d += blockDim.x) e[(size_t)bt * 2 * D + d] = f2bf(0.f);
+    return;
+  }
   for (int d = threadIdx.x; d < D; d += blockDim.x) {
     const int c0 = codes[((size_t)b * K + 0) * T + t];
     e[(size_t)bt * 2 * D + d] = table[((size_t)0 * bins + c0) * D + d];
@@ -90,11 +101,13 @@ __global__ void dwconv_ln_kernel(const bf16* __restrict__ x, const float* __rest
   for (int c = threadIdx.x; c < C; c += blockDim.x) y[(size_t)bt * C + c] = f2bf((sh[c] - mean) * inv * lnw[c] + lnb[c]);
 }
 
-// RoPE in place on q,k of qkv [B][n][3*nh*hd] at positions pos0 + t (…v2.py:329, apply_rotary_pos_emb).  With a K/V
+// RoPE in place on q,k of qkv [B][n][3*nh*hd] at positions rp[b] + t (…v2.py:329, apply_rotary_pos_emb).  With a K/V
 // window buffer kv [B][hist + n_cap][2*nh*hd] (the streaming decoder's) the rotated k and the v heads are also appended
-// at rows [hist, hist+n); kv == nullptr rotates only and does not visit the v heads.
+// at rows [hist, hist+n); kv == nullptr rotates only and does not visit the v heads.  Frames past the row's count are
+// skipped, so a row parked at the end of the RoPE table never indexes past it.
 __global__ void rope_append_kernel(bf16* __restrict__ qkv, const bf16* __restrict__ cosT, const bf16* __restrict__ sinT,
-                                   bf16* __restrict__ kv, int B, int n, int nh, int hd, int pos0, int hist, int kv_bs_rows) {
+                                   bf16* __restrict__ kv, int B, int n, int nh, int hd, const int* __restrict__ rp, int hist,
+                                   int kv_bs_rows) {
   const int half = hd / 2;
   const int heads = kv ? 3 * nh : 2 * nh;  // q heads, k heads[, v heads]
   const size_t total = (size_t)B * n * heads * half;
@@ -103,10 +116,12 @@ __global__ void rope_append_kernel(bf16* __restrict__ qkv, const bf16* __restric
     const int h = (int)((i / half) % heads);
     const size_t bt = i / ((size_t)half * heads);
     const int t = (int)(bt % n), b = (int)(bt / n);
+    if (t >= row_count(rp, B, b, n)) continue;
+    const int pos = row_pos(rp, b) + t;
     bf16* v = qkv + bt * (size_t)(3 * nh * hd) + (size_t)h * hd;
     float y1 = bf2f(v[f]), y2 = bf2f(v[f + half]);
     if (h < 2 * nh) {
-      const float c = bf2f(cosT[(size_t)(pos0 + t) * half + f]), sn = bf2f(sinT[(size_t)(pos0 + t) * half + f]);
+      const float c = bf2f(cosT[(size_t)pos * half + f]), sn = bf2f(sinT[(size_t)pos * half + f]);
       const float x1 = y1, x2 = y2;
       y1 = rbf(x1 * c) + rbf(-x2 * sn);
       y2 = rbf(x2 * c) + rbf(x1 * sn);
@@ -124,15 +139,18 @@ __global__ void rope_append_kernel(bf16* __restrict__ qkv, const bf16* __restric
 
 // causal sliding-window attention of the n queries of qkv [B][n][3*nh*hd], one warp per (b, head, t) (…v2.py:321-354;
 // key k visible iff 0 <= t-k < window).  Keys and values come from a K/V view: row r of batch row b starts at
-// kv + (b*kv_bs_rows + r)*ld with the K heads, then (nh*hd further) the V heads, of absolute position pos0 - hist + r
+// kv + (b*kv_bs_rows + r)*ld with the K heads, then (nh*hd further) the V heads, of absolute position rp[b] - hist + r
 // (rows of negative position are not valid yet); query t is row hist + t.  The one-shot forward passes qkv itself
-// (kv = qkv + nh*hd, ld = 3*nh*hd, kv_bs_rows = n, hist = pos0 = 0), the stream its layer's window buffer.
+// (kv = qkv + nh*hd, ld = 3*nh*hd, kv_bs_rows = n, hist = 0, rp = nullptr), the stream its layer's window buffer.
+// Queries past the row's count are skipped (their output rows are left as they are).
 __global__ void swa_stream_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ kv, int ld, int kv_bs_rows, int hist,
-                                  bf16* __restrict__ out, int B, int n, int nh, int hd, int window, int pos0) {
+                                  bf16* __restrict__ out, int B, int n, int nh, int hd, int window, const int* __restrict__ rp) {
   const int wid = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (wid >= B * n * nh) return;
   const int lane = threadIdx.x & 31;
   const int h = wid % nh, t = (wid / nh) % n, b = wid / (nh * n);
+  if (t >= row_count(rp, B, b, n)) return;
+  const int pos0 = row_pos(rp, b);
   const bf16* q = qkv + ((size_t)b * n + t) * (size_t)(3 * nh * hd) + (size_t)h * hd;
   const int r1 = hist + t;                              // the query's own row
   const int r0 = max(max(r1 - window + 1, hist - pos0), 0);  // oldest visible row
@@ -178,31 +196,49 @@ __global__ void swa_stream_kernel(const bf16* __restrict__ qkv, const bf16* __re
     *reinterpret_cast<uint32_t*>(out + ((size_t)b * n + t) * (size_t)(nh * hd) + (size_t)h * hd + lane * 2) = pack_bf16(o0, o1);
 }
 
-// after a packet: every history buffer keeps its last `hist` rows ([hist + T] rows were valid) at the front.
-// One launch for all buffers; block = (entry, batch row); rows ascend so an overlapping move (T < hist) is safe.
-struct RollEntry { bf16* p; int hist, T, C, bs_rows; };
+// after a packet: every history buffer keeps, per batch row b, its last `hist` rows ([hist + T] rows were valid, T =
+// factor * rp[B + b]: the row's count times the buffer's rows per frame) at the front.  One launch for all buffers;
+// block = (entry, batch row); rows ascend so an overlapping move (T < hist) is safe.  A row with count 0 stays.
+struct RollEntry { bf16* p; int hist, factor, C, bs_rows; };
 constexpr int kRollMax = 48;
 struct RollTable { int n; RollEntry e[kRollMax]; };
-__global__ void roll_history_kernel(RollTable tb, int B) {
+__global__ void roll_history_kernel(RollTable tb, const int* __restrict__ rp, int B) {
   const RollEntry E = tb.e[blockIdx.x / B];
   const int b = blockIdx.x % B;
+  const int T = E.factor * rp[B + b];
+  if (T == 0) return;
   bf16* base = E.p + (size_t)b * E.bs_rows * E.C;
   const int cv = E.C / 8;  // C % 16 == 0
   for (int r = 0; r < E.hist; ++r) {
-    const uint4* src = reinterpret_cast<const uint4*>(base + (size_t)(E.T + r) * E.C);
+    const uint4* src = reinterpret_cast<const uint4*>(base + (size_t)(T + r) * E.C);
     uint4* dst = reinterpret_cast<uint4*>(base + (size_t)r * E.C);
     for (int c = threadIdx.x; c < cv; c += blockDim.x) dst[c] = src[c];
     __syncthreads();  // row r complete before row r+1 may overwrite what a later source row aliases
   }
 }
 
-// final causal conv k=7, C -> 1, + clamp(-1,1) (…v2.py:863,884); one thread per output sample
+// zero the history rows of every buffer of the table for the batch rows b with rp[B + b] != 0 (a fresh utterance:
+// zero history is the causal left padding); block = (entry, batch row)
+__global__ void reset_history_kernel(RollTable tb, const int* __restrict__ rp, int B) {
+  const RollEntry E = tb.e[blockIdx.x / B];
+  const int b = blockIdx.x % B;
+  if (rp[B + b] == 0) return;
+  uint4* base = reinterpret_cast<uint4*>(E.p + (size_t)b * E.bs_rows * E.C);
+  const int nv = E.hist * E.C / 8;
+  for (int i = threadIdx.x; i < nv; i += blockDim.x) base[i] = make_uint4(0u, 0u, 0u, 0u);
+}
+
+// final causal conv k=7, C -> 1, + clamp(-1,1) (…v2.py:863,884); one thread per output sample.  The T samples of a row
+// are `up` per frame; the samples of frames past the row's count are written as zeros.
 __global__ void final_conv_kernel(const bf16* __restrict__ x, const float* __restrict__ w /*[7][C]*/, const float* __restrict__ bias_p,
-                                  float* __restrict__ wav, int B, int T, int C, int x_bs_rows, int hist) {
+                                  float* __restrict__ wav, int B, int T, int C, int x_bs_rows, int hist, const int* __restrict__ rp,
+                                  int up) {
   const size_t total = (size_t)B * T;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const int t = (int)(i % T);
-    const size_t xrow = (i / T) * (size_t)x_bs_rows + hist + t;
+    const int b = (int)(i / T);
+    if (rp && t >= rp[B + b] * up) { wav[i] = 0.f; continue; }
+    const size_t xrow = (size_t)b * x_bs_rows + hist + t;
     float acc = __ldg(bias_p);
     for (int j = 0; j < 7; ++j) {
       const int tt = t - 6 + j;
@@ -435,11 +471,16 @@ struct HistBuf {
 // convolution with taps, the last input row of every k=2r ConvTranspose, and per transformer layer the rotated K and V
 // of the last window-1 frames.  Every such tensor lives in a history-prefixed buffer [B][hist + T_cap][C]: its producer
 // GEMM writes the new rows behind the history, its consumer GEMM reads through a TMA map whose taps reach back into the
-// history (GemmViews), and one roll kernel per packet moves the last `hist` rows to the front.
+// history (GemmViews), and one roll kernel per packet moves the last `hist` rows to the front.  Every row has its own
+// position and may take fewer frames than the packet (its count) or be reset alone, so rows that start and end at
+// different frames share one stream (a continuous-batching session).
 // =================================================================================================
 struct q3_codec_stream {
   q3_codec* c = nullptr;
-  int B = 0, nmax = 0, pos = 0;
+  int B = 0, nmax = 0;
+  std::vector<int> pos;       // frames pushed per row since its last reset
+  std::vector<int32_t> rp_h;  // host image of rp: [0, B) positions, [B, 2B) counts of the next step (reset mask of a reset)
+  int32_t* rp = nullptr;      // device int32 [2][B], uploaded with one copy per step or reset
   std::vector<void*> allocs;
   HistBuf pre, in, out;
   std::vector<HistBuf> dw, ct, kv;
@@ -457,13 +498,15 @@ static void for_each_hist(const q3_codec_stream* s, F f) {
   for (const auto& v : s->c1) for (const HistBuf& h : v) f(h);
 }
 
-// The decoder's layer sequence for n new frames of every row, frame t at position pos0 + t: codes int32 [B][K][n] ->
-// wav fp32 [B][n * total_upsample].  The tensors that a layer reads back in time (pre, kv, dw, in, ct, c1, out) are
-// HistBuf views: with a stream state `s` its history-prefixed buffers; without one (the one-shot forward, pos0 = 0)
+// The decoder's layer sequence for n new frames of every row, frame t of row b at position rp[b] + t, of which the first
+// rp[B + b] are the row's (see row_pos; rp == nullptr: position 0, all n): codes int32 [B][K][n] -> wav fp32
+// [B][n * total_upsample], zero past each row's count.  The tensors that a layer reads back in time (pre, kv, dw, in, ct, c1, out) are
+// HistBuf views: with a stream state `s` its history-prefixed buffers; without one (the one-shot forward, rp = nullptr)
 // plain views of the scratch buffers, where the TMA zero fill of negative rows is the causal left padding.  Scratch
 // X, Y, Z, W (`scratch`, per_frame * B * n elements each) hold everything else.  One-shot mapping: pre, dw -> Y;
-// in -> Z; ct, out -> X; c1 -> W.  No GEMM's A operand aliases one of its outputs.
-static int decode_frames(q3_codec* c, const q3_codec_stream* s, const int32_t* codes, int B, int n, int pos0,
+// in -> Z; ct, out -> X; c1 -> W.  No GEMM's A operand aliases one of its outputs.  Every layer is causal and row-local, so
+// the frames past a row's count change nothing before them; they only never reach the history, the RoPE table or the codes.
+static int decode_frames(q3_codec* c, const q3_codec_stream* s, const int32_t* codes, int B, int n, const int* rp,
                          bf16* const scratch[4], float* wav, cudaStream_t stream) {
   const q3_codec_cfg& g = c->cfg;
   const int Cl = g.latent_dim, Hh = g.hidden_size, nh = g.num_heads, hd = g.head_dim, I = g.intermediate_size;
@@ -483,7 +526,7 @@ static int decode_frames(q3_codec* c, const q3_codec_stream* s, const int32_t* c
   // ---- RVQ decode -> X [B][n][codebook_dim]; projection -> pre_conv's input
   const int D = g.codebook_dim / 2;
   rvq_gather_kernel<<<B * n, 128, 0, stream>>>(codes, R.b16("rvq.table", (int64_t)g.num_quantizers * g.codebook_size * D), X, B,
-                                               g.num_quantizers, n, D, g.codebook_size);
+                                               g.num_quantizers, n, D, g.codebook_size, rp);
   c->launches++;
   if (R.err) return 1;
   const HistBuf pre = s ? s->pre : HistBuf{Y, 0, g.codebook_dim, n};
@@ -505,9 +548,9 @@ static int decode_frames(q3_codec* c, const q3_codec_stream* s, const int32_t* c
     { GemmEpilogue e = none; e.out_raw = Z; R.gemm(X, n, Hh, (int64_t)n * Hh, (p + ".qkv.w").c_str(), 3 * nh * hd, 1, &zero, e, {}); }
     // keys and values: the stream appends them to the layer's window buffer, the one-shot attends over qkv itself
     const HistBuf kv = s ? s->kv[l] : HistBuf{Z + nh * hd, 0, 3 * nh * hd, n};
-    rope_append_kernel<<<296, 256, 0, stream>>>(Z, cosT, sinT, s ? kv.p : nullptr, B, n, nh, hd, pos0, kv.hist, kv.bs_rows());
+    rope_append_kernel<<<296, 256, 0, stream>>>(Z, cosT, sinT, s ? kv.p : nullptr, B, n, nh, hd, rp, kv.hist, kv.bs_rows());
     swa_stream_kernel<<<(rows * nh + 7) / 8, 256, 0, stream>>>(Z, kv.p, kv.C, kv.bs_rows(), kv.hist, X, B, n, nh, hd,
-                                                                g.sliding_window, pos0);
+                                                                g.sliding_window, rp);
     { GemmEpilogue e = none; e.scale = R.f32(p + ".ls1", Hh); e.resid = xres; e.out_raw = W;
       R.gemm(X, n, nh * hd, (int64_t)n * nh * hd, (p + ".o.w").c_str(), Hh, 1, &zero, e, {}); }
     rmsnorm_rows_kernel<<<(rows + 7) / 8, 256, 0, stream>>>(W, R.b16(p + ".ln2", Hh), X, rows, Hh, g.rms_eps);
@@ -605,7 +648,7 @@ static int decode_frames(q3_codec* c, const q3_codec_stream* s, const int32_t* c
     const float* w = R.f32("dec.out.w", (int64_t)7 * C);
     const float* bsrc = R.f32("dec.out.b", 1);
     if (R.err) return 1;
-    final_conv_kernel<<<1184, 256, 0, stream>>>(a.p, w, bsrc, wav, B, Tc, C, a.bs_rows(), a.hist);  // bias read on the device: no host round trip
+    final_conv_kernel<<<1184, 256, 0, stream>>>(a.p, w, bsrc, wav, B, Tc, C, a.bs_rows(), a.hist, rp, c->total_up);  // bias read on the device
     c->launches++;
   }
   Q3_CUDA(cudaGetLastError());
@@ -622,7 +665,7 @@ extern "C" int q3_codec_forward(q3_codec* c, const int32_t* codes_dev, int32_t B
     if (alloc_scratch(c->allocs, c->buf, need)) return 1;
     c->buf_elems = need;
   }
-  return decode_frames(c, nullptr, codes_dev, B, T, 0, c->buf, wav_dev, (cudaStream_t)stream_);
+  return decode_frames(c, nullptr, codes_dev, B, T, nullptr, c->buf, wav_dev, (cudaStream_t)stream_);
 }
 
 static int hist_alloc(q3_codec_stream* s, HistBuf* h, int hist, int C, int cap) {
@@ -665,6 +708,11 @@ extern "C" int q3_codec_stream_open(q3_codec* c, int32_t B, int32_t max_packet_f
   }
   if (!rc) rc = hist_alloc(s, &s->out, 6, C, Tc);
   if (!rc) rc = alloc_scratch(s->allocs, s->buf, scratch_per_frame(g) * (size_t)B * n);
+  void* rp = nullptr;
+  if (!rc) rc = dev_alloc(s->allocs, &rp, (size_t)2 * B * sizeof(int32_t), true);
+  s->rp = reinterpret_cast<int32_t*>(rp);
+  s->pos.assign(B, 0);
+  s->rp_h.assign(2 * B, 0);
   if (rc) { for (void* p : s->allocs) cudaFree(p); delete s; return 1; }
   Q3_CUDA(cudaDeviceSynchronize());
   *out = s;
@@ -677,39 +725,91 @@ extern "C" void q3_codec_stream_close(q3_codec_stream* s) {
   delete s;
 }
 
-extern "C" int q3_codec_stream_position(q3_codec_stream* s) { return s ? s->pos : -1; }
+// the history buffers of a stream as a table for the roll and reset kernels.  A buffer's capacity is max_packet_frames
+// times its stage's rows per frame, so its factor is cap / nmax.  q3_codec_stream_open bounds the number of buffers.
+static RollTable hist_table(const q3_codec_stream* s) {
+  RollTable tb{};
+  for_each_hist(s, [&](const HistBuf& h) {
+    if (h.hist > 0) tb.e[tb.n++] = RollEntry{h.p, h.hist, h.cap / s->nmax, h.C, h.bs_rows()};
+  });
+  return tb;
+}
 
-// next n frames of every row: codes_dev int32 [B][K][n] -> wav_dev fp32 [B][n * total_upsample]
-extern "C" int q3_codec_stream_step(q3_codec_stream* s, const int32_t* codes_dev, int32_t n, float* wav_dev, void* stream_) {
-  Q3_REQUIRE(s && codes_dev && wav_dev, "null argument");
-  Q3_REQUIRE(n >= 1 && n <= s->nmax, "packet of %d frames (max %d)", n, s->nmax);
+// the common position of all rows; -1 (q3_last_error says why) when rows differ
+extern "C" int q3_codec_stream_position(q3_codec_stream* s) {
+  if (!s) { q3_set_err("null stream"); return -1; }
+  for (int b = 1; b < s->B; ++b)
+    if (s->pos[b] != s->pos[0]) {
+      q3_set_err("rows are at different positions (row 0 at %d, row %d at %d): use q3_codec_stream_row_position", s->pos[0], b,
+                 s->pos[b]);
+      return -1;
+    }
+  return s->pos[0];
+}
+
+// frames pushed to `row` since its last reset; -1 for a bad row
+extern "C" int q3_codec_stream_row_position(q3_codec_stream* s, int32_t row) {
+  if (!s || row < 0 || row >= s->B) { q3_set_err("row %d out of range [0, %d)", row, s ? s->B : 0); return -1; }
+  return s->pos[row];
+}
+
+// next frames of every row: codes_dev int32 [B][K][n]; row b takes the first counts_host[b] of them -> wav_dev fp32
+// [B][n * total_upsample], zero past each row's count.  Every argument is checked before any device work.
+extern "C" int q3_codec_stream_step_rows(q3_codec_stream* s, const int32_t* codes_dev, int32_t n, const int32_t* counts_host,
+                                         float* wav_dev, void* stream_) {
+  Q3_REQUIRE(s && codes_dev && counts_host && wav_dev, "null argument");
   const q3_codec_cfg& g = s->c->cfg;
-  Q3_REQUIRE(s->pos + n <= g.max_frames, "stream position %d + %d exceeds the RoPE table (max_frames %d)", s->pos, n, g.max_frames);
+  for (int b = 0; b < s->B; ++b) {
+    Q3_REQUIRE((int64_t)s->pos[b] + counts_host[b] <= g.max_frames,
+               "row %d: position %d + %d frames exceeds the RoPE table (max_frames %d)", b, s->pos[b], counts_host[b], g.max_frames);
+    Q3_REQUIRE(counts_host[b] >= 0 && counts_host[b] <= n, "row %d: count %d outside [0, %d]", b, counts_host[b], n);
+  }
+  Q3_REQUIRE(n >= 1 && n <= s->nmax, "packet of %d frames (max %d)", n, s->nmax);
   Q3_CUDA(cudaSetDevice(g.device));
   cudaStream_t stream = (cudaStream_t)stream_;
-  if (decode_frames(s->c, s, codes_dev, s->B, n, s->pos, s->buf, wav_dev, stream)) return 1;
-  // a buffer's capacity is max_packet_frames times its stage's upsampling factor: the packet filled cap / nmax * n rows.
-  // q3_codec_stream_open bounds the number of buffers by the table size.
-  RollTable roll{};
-  for_each_hist(s, [&](const HistBuf& h) {
-    if (h.hist > 0) roll.e[roll.n++] = RollEntry{h.p, h.hist, h.cap / s->nmax * n, h.C, h.bs_rows()};
-  });
-  roll_history_kernel<<<roll.n * s->B, 128, 0, stream>>>(roll, s->B);
+  for (int b = 0; b < s->B; ++b) { s->rp_h[b] = s->pos[b]; s->rp_h[s->B + b] = counts_host[b]; }
+  Q3_CUDA(cudaMemcpyAsync(s->rp, s->rp_h.data(), (size_t)2 * s->B * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+  if (decode_frames(s->c, s, codes_dev, s->B, n, s->rp, s->buf, wav_dev, stream)) return 1;
+  const RollTable roll = hist_table(s);
+  roll_history_kernel<<<roll.n * s->B, 128, 0, stream>>>(roll, s->rp, s->B);
   s->c->launches++;
   Q3_CUDA(cudaGetLastError());
-  s->pos += n;
+  for (int b = 0; b < s->B; ++b) s->pos[b] += counts_host[b];
   return 0;
 }
 
-// forget everything: the next packet starts a new utterance
+// next n frames of every row: codes_dev int32 [B][K][n] -> wav_dev fp32 [B][n * total_upsample]
+extern "C" int q3_codec_stream_step(q3_codec_stream* s, const int32_t* codes_dev, int32_t n, float* wav_dev, void* stream_) {
+  Q3_REQUIRE(s, "null argument");
+  const std::vector<int32_t> counts(s->B, n);
+  return q3_codec_stream_step_rows(s, codes_dev, n, counts.data(), wav_dev, stream_);
+}
+
+// forget the listed rows: their next packet starts a new utterance at position 0; the other rows are untouched
+extern "C" int q3_codec_stream_reset_rows(q3_codec_stream* s, int32_t n, const int32_t* rows_host, void* stream_) {
+  Q3_REQUIRE(s && rows_host, "null argument");
+  for (int i = 0; i < n; ++i) Q3_REQUIRE(rows_host[i] >= 0 && rows_host[i] < s->B, "reset row %d out of range [0, %d)", rows_host[i], s->B);
+  for (int i = 0; i < n; ++i)
+    for (int j = 0; j < i; ++j) Q3_REQUIRE(rows_host[i] != rows_host[j], "reset row %d listed twice", rows_host[i]);
+  Q3_REQUIRE(n >= 0 && n <= s->B, "%d rows to reset, the stream has %d", n, s->B);
+  if (n == 0) return 0;
+  std::vector<int32_t> mask(s->B, 0);
+  for (int i = 0; i < n; ++i) mask[rows_host[i]] = 1;
+  Q3_CUDA(cudaSetDevice(s->c->cfg.device));
+  cudaStream_t stream = (cudaStream_t)stream_;
+  for (int b = 0; b < s->B; ++b) { s->rp_h[b] = mask[b] ? 0 : s->pos[b]; s->rp_h[s->B + b] = mask[b]; }
+  Q3_CUDA(cudaMemcpyAsync(s->rp, s->rp_h.data(), (size_t)2 * s->B * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+  const RollTable tb = hist_table(s);
+  reset_history_kernel<<<tb.n * s->B, 128, 0, stream>>>(tb, s->rp, s->B);
+  Q3_CUDA(cudaGetLastError());
+  for (int b = 0; b < s->B; ++b) if (mask[b]) s->pos[b] = 0;
+  return 0;
+}
+
+// forget everything: the next packet starts a new utterance in every row
 extern "C" int q3_codec_stream_reset(q3_codec_stream* s, void* stream_) {
   Q3_REQUIRE(s, "null stream");
-  cudaStream_t stream = (cudaStream_t)stream_;
-  cudaError_t e = cudaSuccess;
-  for_each_hist(s, [&](const HistBuf& h) {
-    if (e == cudaSuccess) e = cudaMemsetAsync(h.p, 0, (size_t)s->B * h.bs_rows() * h.C * 2, stream);
-  });
-  Q3_CUDA(e);
-  s->pos = 0;
-  return 0;
+  std::vector<int32_t> rows(s->B);
+  for (int b = 0; b < s->B; ++b) rows[b] = b;
+  return q3_codec_stream_reset_rows(s, s->B, rows.data(), stream_);
 }

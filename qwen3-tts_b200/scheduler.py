@@ -7,13 +7,20 @@ prefilled into a free slot between two decode chunks (`packet_frames` frame-step
 K/V, positions, sampling history and Philox streams, and leaves as soon as it samples EOS.  Every per-row quantity of
 the fused kernel is keyed by the row's own frame counter and by the request's Philox key, so a request generates
 exactly what it would generate alone (tests/test_gpu_scheduler.py).
+
+With a codec the batcher also streams audio: one codec stream of `n_slots` rows follows the session, a slot's row is
+reset when a request enters it, and after every decode each running slot pushes its new frames as its own count (idle
+slots push none).  A request's concatenated chunks equal the one-shot decode of its codes alone
+(tests/test_gpu_scheduler_audio.py).
 """
 from collections import deque
 from dataclasses import dataclass, field
-from typing import Deque, Dict, List, Optional
+from typing import Deque, Dict, Iterator, List, Optional, Tuple
 
+import numpy as np
 import torch
 
+from .codec import CodecDecoder
 from .config import SamplingParams
 from .engine import AREngine
 
@@ -31,7 +38,7 @@ class _Request:
 
 class ContinuousBatcher:
     def __init__(self, engine: AREngine, tts_pad_embed: torch.Tensor, sp: SamplingParams, n_slots: int = 8, packet_frames: int = 4,
-                 max_trailing: int = 256):
+                 max_trailing: int = 256, codec: Optional[CodecDecoder] = None):
         self.eng, self.sp = engine, sp
         self.n_slots, self.packet = int(n_slots), int(packet_frames)
         self.G = engine.cfg.num_code_groups
@@ -44,6 +51,8 @@ class ContinuousBatcher:
         self.max_trailing = int(max_trailing)
         engine.session_begin(self.n_slots, tts_pad_embed, sp, max_trailing=self.max_trailing)
         self.frames_total = 0
+        self.codec = codec
+        self.cstream = codec.open_stream(self.n_slots, max_packet_frames=self.packet) if codec is not None else None
 
     # ------------------------------------------------------------------ API
     def submit(self, inputs_embeds: torch.Tensor, trailing_text: Optional[torch.Tensor] = None, key: Optional[int] = None,
@@ -59,11 +68,27 @@ class ContinuousBatcher:
         room = self.eng.max_ctx - L
         if room < 1:
             raise ValueError(f"prompt of {L} positions does not fit max_ctx={self.eng.max_ctx}")
-        self.pending.append(_Request(rid, inputs_embeds, tr, min(max_frames or self.max_frames, self.max_frames, room)))
+        horizon = min(max_frames or self.max_frames, self.max_frames, room)
+        if self.codec is not None:
+            horizon = min(horizon, self.codec.max_frames)  # a codec row's position may not pass its RoPE table
+        self.pending.append(_Request(rid, inputs_embeds, tr, horizon))
         return rid
 
     def step(self) -> List[int]:
         """Admit what fits, decode one packet, collect what finished.  Returns the ids that completed in this step."""
+        return self._advance()[1]
+
+    def stream(self) -> Iterator[Tuple[Dict[int, np.ndarray], List[int]]]:
+        """Run the session with audio out: yields per step ({request id: float32 waveform of its new frames},
+        [ids that finished in the step]) while requests are pending or running, so a request submitted between two
+        iterations is admitted at the next one."""
+        if self.cstream is None:
+            raise ValueError("stream() needs a ContinuousBatcher built with a codec")
+        while self.pending or self.running:
+            chunks, finished = self._advance()
+            yield chunks, finished
+
+    def _advance(self) -> Tuple[Dict[int, np.ndarray], List[int]]:
         free = [s for s in range(self.n_slots) if s not in self.running]
         batch = []
         while free and self.pending:
@@ -74,16 +99,20 @@ class ContinuousBatcher:
             self.eng.admit([r.slot for r in batch], [r.rid for r in batch], [r.embeds for r in batch], [r.trailing for r in batch])
             for r in batch:
                 self.running[r.slot] = r
+            if self.cstream is not None:
+                self.cstream.reset([r.slot for r in batch])
         if not self.running:
-            return []
+            return {}, []
         n = min([self.packet] + [r.max_frames - r.emitted for r in self.running.values()])
         self.eng.decode(max(n, 1), self.codes)
         torch.cuda.current_stream(self.eng.device).synchronize()
         fd, n_valid, fin = self.eng.progress()
         self.frames_total = fd
         finished, give_up = [], []
+        new = {}  # slot -> (request, first new frame, new frames)
         for slot, r in list(self.running.items()):
             have = min(n_valid[slot], r.max_frames)
+            new[slot] = (r, r.emitted, have - r.emitted)
             r.emitted = have
             if fin[slot] or have >= r.max_frames:
                 self.done[r.rid] = self.codes[slot, :have].to(torch.int64).clone()
@@ -93,7 +122,24 @@ class ContinuousBatcher:
                 del self.running[slot]
         if give_up:
             self.eng.release_slots(give_up)
-        return finished
+        return self._push_audio(new), finished
+
+    def _push_audio(self, new) -> Dict[int, np.ndarray]:
+        """One codec step over all slots: slot s takes its new frames codes[s, e0:e0+k] as its count k, idle slots 0."""
+        if self.cstream is None:
+            return {}
+        m = max([k for _, _, k in new.values()], default=0)
+        if m == 0:
+            return {}
+        start, counts = [0] * self.n_slots, [0] * self.n_slots
+        for slot, (_, e0, k) in new.items():
+            start[slot], counts[slot] = e0, k
+        idx = (torch.tensor(start)[:, None] + torch.arange(m)[None]).clamp_(max=self.max_frames - 1)
+        rows = torch.arange(self.n_slots)[:, None]
+        codes = self.codes[rows.to(self.codes.device), idx.to(self.codes.device)].transpose(1, 2)  # [S][G][m]
+        wav = self.cstream.push(codes, counts)[:, 0].cpu().numpy()
+        up = self.codec.total_upsample
+        return {r.rid: wav[slot, :k * up] for slot, (r, _, k) in new.items() if k > 0}
 
     def run(self) -> Dict[int, torch.Tensor]:
         """Drain the queue; returns {request id: (N_i, G) codes}."""
