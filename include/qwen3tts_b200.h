@@ -57,8 +57,9 @@ typedef struct {
 } q3_engine_cfg;
 
 /* Generation kwargs of seam B (modeling_qwen3_tts.py:2044-2066; defaults inference/qwen3_tts_model.py:287-352).
- * Accepted ranges (HF's processors, plus finiteness where the sampler needs it); q3_prefill and q3_session_begin reject
- * anything else with an error naming the field, before any device work:
+ * Accepted ranges (HF's processors, plus finiteness where the sampler needs it); q3_prefill, q3_session_begin and
+ * q3_admit_with_sampling reject anything else with an error naming the field, before any device work (q3_sampling_check
+ * applies the same rules on its own):
  *   temperature / subtalker_temperature: finite and > 0 when do_sample / subtalker_dosample is set (ignored otherwise);
  *   top_k, subtalker_top_k >= 0 (0 = off); 0 <= top_p, subtalker_top_p <= 1 (1 = off);
  *   repetition_penalty finite and > 0 (1 = off); min_new_tokens >= 0. */
@@ -120,6 +121,19 @@ int q3_session_begin(q3_engine* e, int32_t n_slots, int32_t max_trailing, const 
 int q3_admit(q3_engine* e, int32_t n, const int32_t* slots_host, const uint32_t* keys_host, const void* embeds_dev,
              const int32_t* lens_host, const void* trailing_dev, const int32_t* trailing_lens_host,
              int32_t trailing_stride, void* stream);
+/* q3_admit with per-request sampling parameters: request r samples (its prefill head and every frame-step) with
+ * sp_host[r] (host array [n]; NULL = the session's sp for all, which is q3_admit) and the Philox key
+ * (sp_host[r].seed, keys_host[r]), so it generates what it would generate alone in a session whose parameters are
+ * sp_host[r].  A row without a running request (never admitted, finished, released) samples with the session's sp.
+ * All n entries are checked (q3_sampling_check) before any other argument and any device work; a bad one fails the
+ * whole call with an error naming the request index and the field, and no slot, key or parameter changes. */
+int q3_admit_with_sampling(q3_engine* e, int32_t n, const int32_t* slots_host, const uint32_t* keys_host,
+                           const q3_sampling* sp_host, const void* embeds_dev, const int32_t* lens_host,
+                           const void* trailing_dev, const int32_t* trailing_lens_host, int32_t trailing_stride,
+                           void* stream);
+/* The range check q3_prefill, q3_session_begin and q3_admit_with_sampling apply (see q3_sampling): 0 if sp is
+ * accepted, else non-zero with q3_last_error() naming the field.  Host only: needs no engine and no GPU. */
+int q3_sampling_check(const q3_sampling* sp);
 /* Streaming text input: append n rows [n][H] bf16 to the trailing_text_hidden of a running row (static batch or session);
  * frame t adds trailing[t] while t < the row's trailing length and tts_pad afterwards (modeling_qwen3_tts.py:1689-1692).
  * The capacity is the trailing stride given at q3_prefill / max_trailing of q3_session_begin. */

@@ -241,7 +241,8 @@ struct q3_engine {
   bf16* proj_tab = nullptr;   // small_to_mtp_projection(cp.codec_embedding) [(G-1)*Vc][Hc], built once at finalize
   std::vector<Phase> prog_head, prog_frame;
   int off_head = 0, off_frame = 0;
-  q3_sampling sp{};
+  q3_sampling sp{};           // the batch's parameters (static path) / the session's default (continuous batching)
+  q3_sampling row_sp[MAXB]{}; // each row's own parameters (a session's admitted requests; sp everywhere else)
   bool finalized = false;
   int B = 0;
   int codes_stride = 0;
@@ -717,6 +718,11 @@ static int launch_program(q3_engine* e, int off, int n, int mode, int max_iters,
   P.prog = e->prog_dev + off; P.n_phases = n; P.mode = mode; P.max_iters = max_iters; P.st = e->st;
   P.talker = e->talker; P.cp = e->cp; P.G = e->cfg.num_code_groups; P.eos = e->cfg.codec_eos_token_id;
   P.has_proj = e->cfg.has_cp_projection; P.sp = e->sp;
+  // a session's rows sample with their own request's parameters; a row without a running request (never admitted,
+  // finished, released) with the session's, so that a request's settings stop costing the others once it has left
+  P.row_sampling = e->session ? 1 : 0;
+  if (e->session)
+    for (int b = 0; b < MAXB; ++b) P.row_sp[b] = e->active[b] ? e->row_sp[b] : e->sp;
   P.B = e->B;
   for (int b = 0; b < MAXB; ++b) { P.len0[b] = e->len0[b]; P.trailing_len[b] = e->trailing_len[b]; }
   P.max_len0 = e->max_len0;
@@ -849,6 +855,7 @@ extern "C" int q3_prefill(q3_engine* e, int32_t B, const void* embeds_dev, const
   cudaStream_t stream = (cudaStream_t)stream_;
   if (build_programs(e, B)) return 1;
   e->B = B; e->sp = *sp; e->session = false;
+  for (int b = 0; b < MAXB; ++b) e->row_sp[b] = *sp;
   const int H = e->cfg.talker.hidden_size;
   // per-request state reset
   DevState hs;
@@ -898,6 +905,7 @@ extern "C" int q3_session_begin(q3_engine* e, int32_t n_slots, int32_t max_trail
     hs.finished[b] = 1;  // an empty slot is a finished row: it keeps stepping (like HF's padded rows) and is ignored
     hs.len0[b] = 1;
     e->len0[b] = 1; e->frame0[b] = 0; e->row_key[b] = (unsigned int)b; e->trailing_len[b] = 0; e->active[b] = false;
+    e->row_sp[b] = *sp;
   }
   e->max_len0 = 1;
   Q3_CUDA(cudaMemcpyAsync(e->st, &hs, sizeof(hs), cudaMemcpyHostToDevice, stream));
@@ -910,11 +918,24 @@ extern "C" int q3_session_begin(q3_engine* e, int32_t n_slots, int32_t max_trail
   return 0;
 }
 
-extern "C" int q3_admit(q3_engine* e, int32_t n, const int32_t* slots_host, const uint32_t* keys_host, const void* embeds_dev,
-                        const int32_t* lens_host, const void* trailing_dev, const int32_t* trailing_lens_host,
-                        int32_t trailing_stride, void* stream_) {
+extern "C" int q3_sampling_check(const q3_sampling* sp) {
+  Q3_REQUIRE(sp, "null argument");
+  return check_sampling(*sp);
+}
+
+// sp_host == nullptr: every request samples with the session's parameters (q3_admit)
+extern "C" int q3_admit_with_sampling(q3_engine* e, int32_t n, const int32_t* slots_host, const uint32_t* keys_host,
+                                      const q3_sampling* sp_host, const void* embeds_dev, const int32_t* lens_host,
+                                      const void* trailing_dev, const int32_t* trailing_lens_host, int32_t trailing_stride,
+                                      void* stream_) {
   Q3_REQUIRE(e && e->finalized && e->session, "q3_session_begin first");
   Q3_REQUIRE(n >= 1 && n <= e->B && slots_host && keys_host && embeds_dev && lens_host, "bad argument");
+  // every request's parameters before anything else: one bad entry fails the whole admission and changes nothing
+  for (int r = 0; sp_host && r < n; ++r)
+    if (check_sampling(sp_host[r])) {
+      const std::string why = g_q3_err;
+      return q3_set_err("request %d: %s", r, why.c_str());
+    }
   Q3_CUDA(cudaSetDevice(e->cfg.device));
   cudaStream_t stream = (cudaStream_t)stream_;
   // the global frame at which these rows start = frames completed so far (a decode may have stopped early)
@@ -943,6 +964,7 @@ extern "C" int q3_admit(q3_engine* e, int32_t n, const int32_t* slots_host, cons
       Q3_CUDA(cudaMemcpyAsync(e->trailing + (size_t)b * e->trailing_cap * H, reinterpret_cast<const bf16*>(trailing_dev) + (size_t)r * trailing_stride * H,
                               (size_t)tl * H * 2, cudaMemcpyDeviceToDevice, stream));
   }
+  for (int r = 0; r < n; ++r) e->row_sp[slots[r]] = sp_host ? sp_host[r] : e->sp;
   for (int b = 0; b < e->B; ++b)
     if (hs.finished[b] && !std::count(slots, slots + n, b)) e->active[b] = false;
   e->max_len0 = 1;
@@ -950,6 +972,13 @@ extern "C" int q3_admit(q3_engine* e, int32_t n, const int32_t* slots_host, cons
     if (e->active[b]) e->max_len0 = std::max(e->max_len0, e->len0[b]);
   admit_state_kernel<<<n, 256, 0, stream>>>(e->st, A, e->seen, e->cfg.talker.vocab_size);
   return prefill_rows(e, n, slots, embeds_dev, lens_host, stream);
+}
+
+extern "C" int q3_admit(q3_engine* e, int32_t n, const int32_t* slots_host, const uint32_t* keys_host, const void* embeds_dev,
+                        const int32_t* lens_host, const void* trailing_dev, const int32_t* trailing_lens_host,
+                        int32_t trailing_stride, void* stream_) {
+  return q3_admit_with_sampling(e, n, slots_host, keys_host, nullptr, embeds_dev, lens_host, trailing_dev, trailing_lens_host,
+                                trailing_stride, stream_);
 }
 
 extern "C" int q3_decode(q3_engine* e, int32_t max_frames, int32_t* codes_dev, int32_t codes_stride, void* stream_) {

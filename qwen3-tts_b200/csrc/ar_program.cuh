@@ -112,7 +112,9 @@ struct KParams {
   unsigned int row_key[MAXB];  // Philox row key (the request's identity, not its slot: an admitted row samples what it would alone)
   unsigned int admit_mask;  // prefill-head program only: rows whose first token is sampled / whose hidden state is saved
   int trailing_len[MAXB];
-  q3_sampling sp;
+  q3_sampling sp;           // sampling parameters of every row, unless row_sampling is set
+  int row_sampling;         // 1: row b samples with row_sp[b] (continuous batching: per-request parameters); 0: with sp
+  q3_sampling row_sp[MAXB];
   // sampler / embed resources
   const bf16* emb_t;        // talker codec_embedding [V][H]
   const bf16* emb_cp;       // cp codec_embedding [G-1][Vc][H]
@@ -142,5 +144,7 @@ struct KParams {
   const uint32_t* run_off;  // [grid*NWARPS + 1] start of each (CTA, warp) list in `runs`
   unsigned long long* prof;  // [n_phases][grid][16]: globaltimer ns [0] phase end, [1] barrier passed, [2..4] inner marks, [6] start, [7],[8] warp-0 marks; cycles [5]
 };
+// passed by value to the kernel: stays within the classic 4 KB kernel-parameter limit
+static_assert(sizeof(KParams) <= 4096, "KParams exceeds 4 KB");
 
 }  // namespace

@@ -216,10 +216,13 @@ __device__ __forceinline__ void sample_phase(const Phase& ph, const KParams& P, 
   unsigned int* hist = reinterpret_cast<unsigned int*>(ired + 32);  // [256]
   // frame index of the token being sampled
   const int fidx = talker ? (in_prefill ? 0 : frame + 1) : frame;
-  const bool do_sample = talker ? P.sp.do_sample : P.sp.subtalker_dosample;
-  const float temperature = talker ? P.sp.temperature : P.sp.subtalker_temperature;
-  const int top_k = talker ? P.sp.top_k : P.sp.subtalker_top_k;
-  const float top_p = talker ? P.sp.top_p : P.sp.subtalker_top_p;
+  // this row's parameters: its own entry of the per-row table (each request of a session samples with its own), or the
+  // launch-wide set.  Every choice below (greedy, fast or generic path) is made per row.
+  const q3_sampling& sp = P.row_sampling ? P.row_sp[b] : P.sp;
+  const bool do_sample = talker ? sp.do_sample : sp.subtalker_dosample;
+  const float temperature = talker ? sp.temperature : sp.subtalker_temperature;
+  const int top_k = talker ? sp.top_k : sp.subtalker_top_k;
+  const float top_p = talker ? sp.top_p : sp.subtalker_top_p;
   const float* lg = S.logits + (size_t)b * V;
   const int n_gen_b = talker ? ldcgi(&st->n_gen[b]) : 0;
 
@@ -233,7 +236,7 @@ __device__ __forceinline__ void sample_phase(const Phase& ph, const KParams& P, 
   }
   float* dbg = talker ? (P.dbg_tlogits ? P.dbg_tlogits + ((size_t)fidx * B + b) * V : nullptr)
                       : (P.dbg_clogits ? P.dbg_clogits + (((size_t)frame * (P.G - 1) + (group - 1)) * B + b) * V : nullptr);
-  const float rp = P.sp.repetition_penalty;
+  const float rp = sp.repetition_penalty;
   const float inv_t = (do_sample && temperature != 1.0f) ? temperature : 1.0f;
 #pragma unroll 1
   for (int i = tid; i < V; i += NTHREADS) {
@@ -243,7 +246,7 @@ __device__ __forceinline__ void sample_phase(const Phase& ph, const KParams& P, 
       // 1. repetition penalty over generated codebook-0 tokens
       if (rp != 1.0f && __ldcg(P.seen + (size_t)b * V + i)) s = s < 0.f ? s * rp : s / rp;
       // 2. min_new_tokens (and the fixed-horizon benchmark switch)
-      if (i == P.eos && (n_gen_b < P.sp.min_new_tokens || P.sp.suppress_eos)) s = -INFINITY;
+      if (i == P.eos && (n_gen_b < sp.min_new_tokens || sp.suppress_eos)) s = -INFINITY;
       // 3. suppress [V-1024, V) \ {eos}
       if (i >= V - 1024 && i != P.eos) s = -INFINITY;
     }
@@ -264,7 +267,7 @@ __device__ __forceinline__ void sample_phase(const Phase& ph, const KParams& P, 
       if (sv[i] == mx) idx = min(idx, i);
     tok = block_min_int(idx, ired);
   } else if (top_p >= 1.0f && top_k > 0 && top_k < V && top_k <= 128 &&
-             sample_fast(sv, V, top_k, philox_uniform(P.sp.seed, P.row_key[b], (uint32_t)fidx, (uint32_t)group), pv, red, ired, &tok)) {
+             sample_fast(sv, V, top_k, philox_uniform(sp.seed, P.row_key[b], (uint32_t)fidx, (uint32_t)group), pv, red, ired, &tok)) {
     // (decided by the fast path)
   } else {
     if (top_k > 0 && top_k < V) {
@@ -333,7 +336,7 @@ __device__ __forceinline__ void sample_phase(const Phase& ph, const KParams& P, 
 #pragma unroll 1
     for (int w = 0; w < NWARPS; ++w) { if (w < wp) base += red[w]; total += red[w]; }
     const float excl = base + incl - loc;
-    const float u = philox_uniform(P.sp.seed, P.row_key[b], (uint32_t)fidx, (uint32_t)group);
+    const float u = philox_uniform(sp.seed, P.row_key[b], (uint32_t)fidx, (uint32_t)group);
     const float target = u * total;
     int cand = 0x7fffffff, lastpos = -1;
     float run = excl;

@@ -115,7 +115,8 @@ class AREngine:
             pass
 
     # ------------------------------------------------------------------ low level
-    def _sampling(self, sp: SamplingParams):
+    @staticmethod
+    def _sampling(sp: SamplingParams):
         s = _lib.Sampling()
         s.do_sample, s.top_k, s.top_p, s.temperature = int(sp.do_sample), int(sp.top_k or 0), float(sp.top_p), float(sp.temperature)
         s.repetition_penalty = float(sp.repetition_penalty)
@@ -123,6 +124,15 @@ class AREngine:
         s.subtalker_top_p, s.subtalker_temperature = float(sp.subtalker_top_p), float(sp.subtalker_temperature)
         s.min_new_tokens, s.suppress_eos, s.seed = int(sp.min_new_tokens), int(sp.suppress_eos), int(sp.seed)
         return s
+
+    @staticmethod
+    def check_sampling(sp: SamplingParams):
+        """Raise ValueError with the library's message when `sp` is outside the ranges the engine accepts
+        (q3_sampling_check: the rules q3_prefill / q3_session_begin / q3_admit_with_sampling apply).  Needs no GPU."""
+        lib = _lib.load()
+        s = AREngine._sampling(sp)
+        if lib.q3_sampling_check(C.byref(s)) != 0:
+            raise ValueError(lib.q3_last_error().decode())
 
     def prefill(self, inputs_embeds: Sequence[torch.Tensor], trailing_text: Sequence[torch.Tensor],
                 tts_pad_embed: torch.Tensor, sp: SamplingParams, trailing_capacity: int = 0):
@@ -160,12 +170,21 @@ class AREngine:
         stream = torch.cuda.current_stream(self.device).cuda_stream
         self._B = n_slots
         self._hold = (pad,)
+        self._session_sp = sp
         _lib.check(self.lib.q3_session_begin(self.h, int(n_slots), int(max_trailing), pad.data_ptr(), C.byref(s), C.c_void_p(stream)))
 
     def admit(self, slots: Sequence[int], keys: Sequence[int], inputs_embeds: Sequence[torch.Tensor],
-              trailing_text: Sequence[torch.Tensor]):
-        """Prefill new requests into free slots of the running session (q3_admit)."""
+              trailing_text: Sequence[torch.Tensor], sampling: Optional[Sequence[Optional[SamplingParams]]] = None):
+        """Prefill new requests into free slots of the running session (q3_admit_with_sampling).  `sampling`: None
+        (every request samples with the session's parameters) or one entry per request, a SamplingParams or None for
+        the session's; a bad entry fails the whole admission before anything changes.  Of each entry the fields of
+        q3_sampling are used, max_new_tokens is the caller's horizon."""
         n = len(slots)
+        sps = None
+        if sampling is not None:
+            if len(sampling) != n:
+                raise ValueError(f"sampling has {len(sampling)} entries for {n} requests")
+            sps = (_lib.Sampling * n)(*[self._sampling(self._session_sp if s is None else s) for s in sampling])
         H = self.cfg.talker.hidden_size
         dev = self.device
         emb = torch.cat([e.reshape(-1, H) for e in inputs_embeds], 0).to(dev, torch.bfloat16).contiguous()
@@ -182,8 +201,9 @@ class AREngine:
             tr, trp = None, None
         stream = torch.cuda.current_stream(dev).cuda_stream
         self._hold = self._hold + (emb, tr)
-        _lib.check(self.lib.q3_admit(self.h, n, (C.c_int32 * n)(*[int(x) for x in slots]), (C.c_uint32 * n)(*[int(k) & 0xffffffff for k in keys]),
-                                     emb.data_ptr(), lens, trp, (C.c_int32 * n)(*tl), Tt, C.c_void_p(stream)))
+        _lib.check(self.lib.q3_admit_with_sampling(self.h, n, (C.c_int32 * n)(*[int(x) for x in slots]),
+                                                   (C.c_uint32 * n)(*[int(k) & 0xffffffff for k in keys]), sps,
+                                                   emb.data_ptr(), lens, trp, (C.c_int32 * n)(*tl), Tt, C.c_void_p(stream)))
 
     def append_trailing(self, slot: int, rows: torch.Tensor):
         """Streaming text input: more trailing_text_hidden rows (n, H) for a row that is already generating."""

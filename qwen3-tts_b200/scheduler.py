@@ -8,6 +8,12 @@ K/V, positions, sampling history and Philox streams, and leaves as soon as it sa
 the fused kernel is keyed by the row's own frame counter and by the request's Philox key, so a request generates
 exactly what it would generate alone (tests/test_gpu_scheduler.py).
 
+Each request may carry its own SamplingParams (greedy or sampled, temperature, top-k / top-p, repetition penalty,
+min_new_tokens, the subtalker's settings, the Philox seed): the kernel reads every sampling field from the row's own
+entry, so requests with different parameters share one session, and each still generates what it would alone in a
+session whose default is its parameters (tests/test_gpu_scheduler_sampling.py).  Slots without a running request
+sample with the session's parameters.
+
 With a codec the batcher also streams audio: one codec stream of `n_slots` rows follows the session, a slot's row is
 reset when a request enters it, and after every decode each running slot pushes its new frames as its own count (idle
 slots push none).  A request's concatenated chunks equal the one-shot decode of its codes alone
@@ -31,6 +37,7 @@ class _Request:
     embeds: torch.Tensor
     trailing: torch.Tensor
     max_frames: int
+    sampling: Optional[SamplingParams] = None
     slot: int = -1
     emitted: int = 0
     chunks: List[torch.Tensor] = field(default_factory=list)
@@ -56,9 +63,19 @@ class ContinuousBatcher:
 
     # ------------------------------------------------------------------ API
     def submit(self, inputs_embeds: torch.Tensor, trailing_text: Optional[torch.Tensor] = None, key: Optional[int] = None,
-               max_frames: Optional[int] = None) -> int:
-        """Queue one request; returns its id (also its Philox row key unless `key` is given)."""
+               max_frames: Optional[int] = None, sampling: Optional[SamplingParams] = None) -> int:
+        """Queue one request; returns its id (also its Philox row key unless `key` is given).  `sampling`: the
+        request's own generation parameters (default: the session's); its max_new_tokens bounds the request's horizon
+        and may not exceed the session's.  Bad parameters raise ValueError here, never in a later step()."""
         H = self.eng.cfg.talker.hidden_size
+        limit = self.max_frames   # frames the request may generate: HF emits max_new_tokens - 1 complete frames
+        if sampling is not None:
+            self.eng.check_sampling(sampling)
+            want = int(sampling.max_new_tokens) - 1
+            if want > self.max_frames:
+                raise ValueError(f"max_new_tokens={sampling.max_new_tokens} exceeds the session's "
+                                 f"max_new_tokens={self.sp.max_new_tokens} (its codes buffer holds {self.max_frames} frames)")
+            limit = max(want, 0)
         rid = self._next_id if key is None else int(key)
         self._next_id = max(self._next_id, rid) + 1
         tr = trailing_text if trailing_text is not None else torch.zeros(0, H)
@@ -68,10 +85,10 @@ class ContinuousBatcher:
         room = self.eng.max_ctx - L
         if room < 1:
             raise ValueError(f"prompt of {L} positions does not fit max_ctx={self.eng.max_ctx}")
-        horizon = min(max_frames or self.max_frames, self.max_frames, room)
+        horizon = min(max_frames or limit, limit, room)
         if self.codec is not None:
             horizon = min(horizon, self.codec.max_frames)  # a codec row's position may not pass its RoPE table
-        self.pending.append(_Request(rid, inputs_embeds, tr, horizon))
+        self.pending.append(_Request(rid, inputs_embeds, tr, horizon, sampling))
         return rid
 
     def step(self) -> List[int]:
@@ -96,7 +113,11 @@ class ContinuousBatcher:
             r.slot = free.pop(0)
             batch.append(r)
         if batch:
-            self.eng.admit([r.slot for r in batch], [r.rid for r in batch], [r.embeds for r in batch], [r.trailing for r in batch])
+            args = ([r.slot for r in batch], [r.rid for r in batch], [r.embeds for r in batch], [r.trailing for r in batch])
+            if any(r.sampling is not None for r in batch):
+                self.eng.admit(*args, sampling=[r.sampling for r in batch])   # None entries: the session's parameters
+            else:
+                self.eng.admit(*args)
             for r in batch:
                 self.running[r.slot] = r
             if self.cstream is not None:

@@ -4,8 +4,11 @@ Full 1.7B talker and default codec shapes with seeded random weights, suppress_e
 staggered so that requests leave at different steps and new ones are admitted into running sessions.  For each
 n_slots it reports the AR and codec milliseconds per step, the time from submit() to a request's first audio chunk,
 and the aggregate audio seconds produced per wall second, with the card name and power limit read in the same run.
+With --mix the requests carry their own sampling parameters: every fourth one top-p 0.8 (talker and subtalker, the
+generic sampler path), every fourth one greedy, the rest the session's; comparing with a run without it gives what
+such rows cost the whole session.
 
-    python tools/serve_probe.py [--slots 8 32] [--requests-per-slot 3] [--packet 4]
+    python tools/serve_probe.py [--slots 8 32] [--requests-per-slot 3] [--packet 4] [--mix]
 
 Prints one JSON line.  Writes nothing.
 """
@@ -37,7 +40,17 @@ def card():
     return {"name": name, "power_limit_w": limit}
 
 
-def run_session(eng, codec, pad, sp, prompts, n_slots, packet, horizons, timed):
+def mixed_sampling(sp, i):
+    """--mix: request i's own parameters (None = the session's)."""
+    import dataclasses
+    if i % 4 == 0:
+        return dataclasses.replace(sp, top_p=0.8, subtalker_top_p=0.8, seed=sp.seed + i)
+    if i % 4 == 1:
+        return dataclasses.replace(sp, do_sample=False, subtalker_dosample=False)
+    return None
+
+
+def run_session(eng, codec, pad, sp, prompts, n_slots, packet, horizons, timed, mix=False):
     """One session: n_slots requests at once, then one more per step until all are in.  Returns the measurements."""
     from qwen3_tts_b200.scheduler import ContinuousBatcher
     cb = ContinuousBatcher(eng, pad, sp, n_slots=n_slots, packet_frames=packet, codec=codec)
@@ -60,7 +73,8 @@ def run_session(eng, codec, pad, sp, prompts, n_slots, packet, horizons, timed):
     todo = list(range(len(prompts)))
 
     def submit(i):
-        rid = cb.submit(prompts[i], None, key=i, max_frames=horizons[i % len(horizons)])
+        rid = cb.submit(prompts[i], None, key=i, max_frames=horizons[i % len(horizons)],
+                        sampling=mixed_sampling(sp, i) if mix else None)
         submitted[rid] = time.perf_counter()
 
     for i in todo[:n_slots]:
@@ -93,6 +107,7 @@ def main():
     ap.add_argument("--requests-per-slot", type=int, default=3)
     ap.add_argument("--packet", type=int, default=4)
     ap.add_argument("--prompt-len", type=int, default=24)
+    ap.add_argument("--mix", action="store_true", help="per-request parameters: 1/4 top-p 0.8, 1/4 greedy, the rest the session's")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("serve_probe needs a CUDA device")
@@ -113,12 +128,14 @@ def main():
     sp = q.SamplingParams(do_sample=True, subtalker_dosample=True, max_new_tokens=max(HORIZONS) + 1, suppress_eos=True, seed=7)
     out = {"what": "ContinuousBatcher.stream(): 1.7B talker + default codec, seeded random weights, suppress_eos, "
                    f"{args.packet}-frame packets, horizons {list(HORIZONS)} frames, n_slots requests at once then one "
-                   "more per step", "card": card(), "results": {}}
+                   "more per step", "sampling": "mixed: 1/4 top-p 0.8, 1/4 greedy, 1/2 session (top-k 50, T 0.9)" if args.mix
+           else "uniform: top-k 50, T 0.9", "card": card(), "results": {}}
     for S in args.slots:
         n_req = S * args.requests_per_slot
         prompts = [(torch.randn(args.prompt_len, H, generator=g) * 0.5).bfloat16() for _ in range(n_req)]
-        run_session(eng, codec, pad, sp, prompts[:S], S, args.packet, (8,), timed=False)   # warm-up: every shape
-        out["results"][f"n_slots={S}"] = run_session(eng, codec, pad, sp, prompts, S, args.packet, HORIZONS, timed=True)
+        run_session(eng, codec, pad, sp, prompts[:S], S, args.packet, (8,), timed=False, mix=args.mix)   # warm-up: every shape
+        out["results"][f"n_slots={S}"] = run_session(eng, codec, pad, sp, prompts, S, args.packet, HORIZONS, timed=True,
+                                                     mix=args.mix)
     out["card_after"] = card()
     print(json.dumps(out))
     codec.close()
