@@ -97,7 +97,9 @@ int q3_engine_finalize(q3_engine* e); /* verifies that every tensor is present *
  * :2239-2254, is equivalent to per-sequence positions 0..len-1).  lens: host int32[B].
  * trailing: bf16 [B][trailing_stride][H] (row b valid for trailing_lens[b] steps, then tts_pad, :1689-1692);
  * tts_pad: bf16 [H].  Resets all per-request state (per request, never on a module: SURVEY F10) and samples
- * codebook-0 of frame 0. */
+ * codebook-0 of frame 0: the batch is a session of B slots whose rows are all admitted at frame 0 with the Philox row
+ * keys 0..B-1 and the parameters sp.  Every row is checked before any state changes: a rejected call leaves the
+ * running batch as it was. */
 int q3_prefill(q3_engine* e, int32_t B, const void* embeds_dev, const int32_t* lens_host,
                const void* trailing_dev, const int32_t* trailing_lens_host, int32_t trailing_stride,
                const void* tts_pad_dev, const q3_sampling* sp, void* stream);
@@ -126,7 +128,9 @@ int q3_admit(q3_engine* e, int32_t n, const int32_t* slots_host, const uint32_t*
  * (sp_host[r].seed, keys_host[r]), so it generates what it would generate alone in a session whose parameters are
  * sp_host[r].  A row without a running request (never admitted, finished, released) samples with the session's sp.
  * All n entries are checked (q3_sampling_check) before any other argument and any device work; a bad one fails the
- * whole call with an error naming the request index and the field, and no slot, key or parameter changes. */
+ * whole call with an error naming the request index and the field.  Then every row (slot, prompt and trailing length,
+ * trailing text) is checked before any state changes: a rejected call admits no row, and no slot, key or parameter
+ * changes. */
 int q3_admit_with_sampling(q3_engine* e, int32_t n, const int32_t* slots_host, const uint32_t* keys_host,
                            const q3_sampling* sp_host, const void* embeds_dev, const int32_t* lens_host,
                            const void* trailing_dev, const int32_t* trailing_lens_host, int32_t trailing_stride,

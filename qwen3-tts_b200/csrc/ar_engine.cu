@@ -241,8 +241,8 @@ struct q3_engine {
   bf16* proj_tab = nullptr;   // small_to_mtp_projection(cp.codec_embedding) [(G-1)*Vc][Hc], built once at finalize
   std::vector<Phase> prog_head, prog_frame;
   int off_head = 0, off_frame = 0;
-  q3_sampling sp{};           // the batch's parameters (static path) / the session's default (continuous batching)
-  q3_sampling row_sp[MAXB]{}; // each row's own parameters (a session's admitted requests; sp everywhere else)
+  q3_sampling sp{};           // default parameters: those of a static batch / a session's, and of rows without a request
+  q3_sampling row_sp[MAXB]{}; // each admitted row's own parameters
   bool finalized = false;
   int B = 0;
   int codes_stride = 0;
@@ -751,15 +751,37 @@ static int launch_program(q3_engine* e, int off, int n, int mode, int max_iters,
   return 0;
 }
 
-// Prefill of `n` prompts (packed back to back in embeds_dev) into the engine slots slots[0..n): wgmma GEMMs over all
-// their tokens at once, K/V into the slots' cache rows, then the head GEMV + the first codebook-0 sample of exactly
-// those rows (admit_mask).  Shared by the static batch (q3_prefill) and by continuous batching (q3_admit).
-static int prefill_rows(q3_engine* e, int n, const int* slots, const void* embeds_dev, const int32_t* lens_host, cudaStream_t stream) {
-  const int H = e->cfg.talker.hidden_size;
+// One admission of n requests: request r enters engine slot slots[r] with the Philox row key keys[r] and the sampling
+// parameters sp[r] (sp == nullptr: the default e->sp); its prompt is lens[r] rows of embeds (packed back to back), its
+// trailing text the first tl[r] rows of trailing[r] ([n][stride][H]; tl == nullptr: none).
+struct Admission {
+  int n;
+  const int32_t* slots;
+  const uint32_t* keys;
+  const q3_sampling* sp;
+  const void* embeds;
+  const int32_t* lens;
+  const void* trailing;
+  const int32_t* tl;
+  int stride;
+};
+
+// Prefill of an admission into its slots: the index kernel resets the rows' device state and gathers their trailing
+// text, wgmma GEMMs run over all their tokens at once, K/V go into the slots' cache rows, then the head GEMV + the first
+// codebook-0 sample of exactly those rows (`mask`: the admitted slots).
+static int prefill_rows(q3_engine* e, const Admission& A, unsigned int mask, cudaStream_t stream) {
+  const int n = A.n, H = e->cfg.talker.hidden_size;
   PfLens pl{};
+  PfRows pr{};
   pl.B = n;
-  unsigned int mask = 0;
-  for (int r = 0; r < n; ++r) { pl.start[r + 1] = pl.start[r] + lens_host[r]; pl.slot[r] = slots[r]; mask |= 1u << slots[r]; }
+  pr.src = reinterpret_cast<const bf16*>(A.trailing); pr.dst = e->trailing; pr.stride = A.stride; pr.cap = e->trailing_cap; pr.H = H;
+  const int V = e->cfg.talker.vocab_size;
+  int row_work = V;  // index-kernel threads per row: its seen bytes or its trailing elements
+  for (int r = 0; r < n; ++r) {
+    pl.start[r + 1] = pl.start[r] + A.lens[r]; pl.slot[r] = A.slots[r];
+    pr.trailing_len[r] = A.tl ? A.tl[r] : 0;
+    row_work = std::max(row_work, pr.trailing_len[r] * H);
+  }
   const int ntok = pl.start[n];
   const q3_stack_cfg& tc = e->cfg.talker;
   const int nh = tc.num_heads, nkv = tc.num_kv_heads, I = tc.intermediate_size, QKV = (nh + 2 * nkv) * HD;
@@ -774,8 +796,8 @@ static int prefill_rows(q3_engine* e, int n, const int* slots, const void* embed
       return 1;
     e->pf_cap = cap;
   }
-  pf_index_kernel<<<(ntok + 255) / 256, 256, 0, stream>>>(pl, e->pf_seq, e->pf_pos);
-  Q3_CUDA(cudaMemcpyAsync(e->pf_x, embeds_dev, (size_t)ntok * H * 2, cudaMemcpyDeviceToDevice, stream));
+  pf_index_kernel<<<dim3((std::max(ntok, row_work) + 255) / 256, n), 256, 0, stream>>>(pl, pr, e->st, e->seen, V, e->pf_seq, e->pf_pos);
+  Q3_CUDA(cudaMemcpyAsync(e->pf_x, A.embeds, (size_t)ntok * H * 2, cudaMemcpyDeviceToDevice, stream));
   const int mt = (ntok + 127) / 128;
   const int zero = 0;
   auto gemm = [&](const bf16* a, int K, const std::string& wname, int N, GemmEpilogue ep) -> int {
@@ -843,6 +865,64 @@ static int check_sampling(const q3_sampling& s) {
   return 0;
 }
 
+// Every check of admission A into a batch of B slots with a trailing capacity of cap rows, where `running` marks the
+// slots whose request is still generating.  Writes nothing, so a rejected admission leaves the engine as it was.
+static int check_admission(const q3_engine* e, const Admission& A, int B, int cap, unsigned int running) {
+  for (int r = 0; r < A.n; ++r) {
+    const int b = A.slots[r], tl = A.tl ? A.tl[r] : 0;
+    Q3_REQUIRE(b >= 0 && b < B, "slot %d out of range", b);
+    Q3_REQUIRE(!((running >> b) & 1u), "slot %d is still running (q3_release_slots it first)", b);
+    for (int q = 0; q < r; ++q) Q3_REQUIRE(A.slots[q] != b, "slot %d admitted twice", b);
+    Q3_REQUIRE(A.lens[r] >= 1 && A.lens[r] < e->cfg.max_ctx, "prompt length %d out of range", A.lens[r]);
+    Q3_REQUIRE(tl >= 0 && tl <= A.stride && tl <= cap, "trailing length %d exceeds the stride %d or the capacity %d", tl, A.stride, cap);
+    Q3_REQUIRE(tl == 0 || A.trailing, "request %d has a trailing length of %d but no trailing text", r, tl);
+  }
+  return 0;
+}
+
+// A batch of B slots, every row finished (an empty slot is a finished row: it keeps stepping, like HF's padded rows, and
+// is ignored), sampling with the default sp, room for max_trailing rows of trailing text per slot.
+static int reset_rows(q3_engine* e, int B, int max_trailing, const void* tts_pad_dev, const q3_sampling& sp, bool session,
+                      cudaStream_t stream) {
+  if (build_programs(e, B)) return 1;
+  e->B = B; e->sp = sp; e->session = session;
+  DevState hs;
+  memset(&hs, 0, sizeof(hs));
+  hs.B = B;
+  for (int b = 0; b < MAXB; ++b) {
+    hs.finished[b] = 1; hs.len0[b] = 1;
+    e->len0[b] = 1; e->frame0[b] = 0; e->row_key[b] = (unsigned int)b; e->trailing_len[b] = 0; e->active[b] = false;
+  }
+  e->max_len0 = 1;
+  Q3_CUDA(cudaMemcpyAsync(e->st, &hs, sizeof(hs), cudaMemcpyHostToDevice, stream));
+  Q3_CUDA(cudaMemsetAsync(e->seen, 0, (size_t)MAXB * e->cfg.talker.vocab_size, stream));
+  Q3_CUDA(cudaMemcpyAsync(e->tts_pad, tts_pad_dev, (size_t)e->cfg.talker.hidden_size * 2, cudaMemcpyDeviceToDevice, stream));
+  if (max_trailing > 0 && ensure_trailing(e, max_trailing, stream)) return 1;
+  e->trailing_cap = max_trailing;
+  return 0;
+}
+
+// Admission A at global frame F (frames completed so far): all rows are checked before any state changes.  `running`
+// marks the slots whose request is still generating; they keep their state.
+static int admit_rows(q3_engine* e, const Admission& A, int F, unsigned int running, cudaStream_t stream) {
+  if (check_admission(e, A, e->B, e->trailing_cap, running)) return 1;
+  unsigned int admitted = 0;
+  for (int r = 0; r < A.n; ++r) {
+    const int b = A.slots[r];
+    e->len0[b] = A.lens[r] - F; e->frame0[b] = F; e->row_key[b] = A.keys[r]; e->trailing_len[b] = A.tl ? A.tl[r] : 0;
+    e->row_sp[b] = A.sp ? A.sp[r] : e->sp;
+    admitted |= 1u << b;
+  }
+  e->frames_issued = F;
+  e->max_len0 = 1;
+  for (int b = 0; b < e->B; ++b) {
+    e->active[b] = ((running | admitted) >> b) & 1u;
+    if (e->active[b]) e->max_len0 = std::max(e->max_len0, e->len0[b]);
+  }
+  return prefill_rows(e, A, admitted, stream);
+}
+
+// A static batch is a session of B slots whose rows are all admitted at frame 0 with the Philox keys 0..B-1.
 extern "C" int q3_prefill(q3_engine* e, int32_t B, const void* embeds_dev, const int32_t* lens_host,
                           const void* trailing_dev, const int32_t* trailing_lens_host, int32_t trailing_stride,
                           const void* tts_pad_dev, const q3_sampling* sp, void* stream_) {
@@ -850,40 +930,15 @@ extern "C" int q3_prefill(q3_engine* e, int32_t B, const void* embeds_dev, const
   Q3_REQUIRE(sp, "null argument");
   if (check_sampling(*sp)) return 1;
   Q3_REQUIRE(B >= 1 && B <= e->cfg.max_batch, "batch %d out of range", B);
-  Q3_REQUIRE(embeds_dev && lens_host && tts_pad_dev && sp, "null argument");
+  Q3_REQUIRE(embeds_dev && lens_host && tts_pad_dev, "null argument");
+  int32_t slots[MAXB]; uint32_t keys[MAXB];
+  for (int b = 0; b < B; ++b) { slots[b] = b; keys[b] = (uint32_t)b; }
+  const Admission A{B, slots, keys, nullptr, embeds_dev, lens_host, trailing_dev, trailing_lens_host, trailing_stride};
+  if (check_admission(e, A, B, trailing_stride, 0)) return 1;
   Q3_CUDA(cudaSetDevice(e->cfg.device));
   cudaStream_t stream = (cudaStream_t)stream_;
-  if (build_programs(e, B)) return 1;
-  e->B = B; e->sp = *sp; e->session = false;
-  for (int b = 0; b < MAXB; ++b) e->row_sp[b] = *sp;
-  const int H = e->cfg.talker.hidden_size;
-  // per-request state reset
-  DevState hs;
-  memset(&hs, 0, sizeof(hs));
-  hs.B = B;
-  int slots[MAXB];
-  for (int b = 0; b < MAXB; ++b) { e->frame0[b] = 0; e->row_key[b] = (unsigned int)b; e->active[b] = b < B; }
-  for (int b = 0; b < B; ++b) {
-    Q3_REQUIRE(lens_host[b] >= 1 && lens_host[b] < e->cfg.max_ctx, "prompt length %d out of range", lens_host[b]);
-    hs.len0[b] = lens_host[b];
-    e->len0[b] = lens_host[b];
-    e->max_len0 = b == 0 ? lens_host[b] : std::max(e->max_len0, lens_host[b]);
-    hs.trailing_len[b] = trailing_lens_host ? trailing_lens_host[b] : 0;
-    e->trailing_len[b] = hs.trailing_len[b];
-    Q3_REQUIRE(hs.trailing_len[b] <= trailing_stride, "trailing length exceeds stride");
-    slots[b] = b;
-  }
-  Q3_CUDA(cudaMemcpyAsync(e->st, &hs, sizeof(hs), cudaMemcpyHostToDevice, stream));
-  Q3_CUDA(cudaMemsetAsync(e->seen, 0, (size_t)MAXB * e->cfg.talker.vocab_size, stream));
-  Q3_CUDA(cudaMemcpyAsync(e->tts_pad, tts_pad_dev, (size_t)H * 2, cudaMemcpyDeviceToDevice, stream));
-  if (trailing_stride > 0 && trailing_dev) {
-    if (ensure_trailing(e, trailing_stride, stream)) return 1;
-    Q3_CUDA(cudaMemcpyAsync(e->trailing, trailing_dev, (size_t)B * trailing_stride * H * 2, cudaMemcpyDeviceToDevice, stream));
-  }
-  e->trailing_cap = trailing_stride;
-  e->codes_stride = 0;
-  e->frames_issued = 0;
-  return prefill_rows(e, B, slots, embeds_dev, lens_host, stream);
+  if (reset_rows(e, B, trailing_stride, tts_pad_dev, *sp, false, stream)) return 1;
+  return admit_rows(e, A, 0, 0, stream);
 }
 
 // ---- continuous batching (SURVEY §8f-4): a session of n_slots rows that start and finish independently ------------
@@ -895,27 +950,7 @@ extern "C" int q3_session_begin(q3_engine* e, int32_t n_slots, int32_t max_trail
   Q3_REQUIRE(n_slots >= 1 && n_slots <= e->cfg.max_batch, "n_slots %d out of range", n_slots);
   Q3_REQUIRE(tts_pad_dev && sp && max_trailing >= 0, "bad argument");
   Q3_CUDA(cudaSetDevice(e->cfg.device));
-  cudaStream_t stream = (cudaStream_t)stream_;
-  if (build_programs(e, n_slots)) return 1;
-  e->B = n_slots; e->sp = *sp; e->session = true;
-  DevState hs;
-  memset(&hs, 0, sizeof(hs));
-  hs.B = n_slots;
-  for (int b = 0; b < MAXB; ++b) {
-    hs.finished[b] = 1;  // an empty slot is a finished row: it keeps stepping (like HF's padded rows) and is ignored
-    hs.len0[b] = 1;
-    e->len0[b] = 1; e->frame0[b] = 0; e->row_key[b] = (unsigned int)b; e->trailing_len[b] = 0; e->active[b] = false;
-    e->row_sp[b] = *sp;
-  }
-  e->max_len0 = 1;
-  Q3_CUDA(cudaMemcpyAsync(e->st, &hs, sizeof(hs), cudaMemcpyHostToDevice, stream));
-  Q3_CUDA(cudaMemsetAsync(e->seen, 0, (size_t)MAXB * e->cfg.talker.vocab_size, stream));
-  Q3_CUDA(cudaMemcpyAsync(e->tts_pad, tts_pad_dev, (size_t)e->cfg.talker.hidden_size * 2, cudaMemcpyDeviceToDevice, stream));
-  if (max_trailing > 0 && ensure_trailing(e, max_trailing, stream)) return 1;
-  e->trailing_cap = max_trailing;
-  e->codes_stride = 0;
-  e->frames_issued = 0;
-  return 0;
+  return reset_rows(e, n_slots, max_trailing, tts_pad_dev, *sp, true, (cudaStream_t)stream_);
 }
 
 extern "C" int q3_sampling_check(const q3_sampling* sp) {
@@ -930,7 +965,7 @@ extern "C" int q3_admit_with_sampling(q3_engine* e, int32_t n, const int32_t* sl
                                       void* stream_) {
   Q3_REQUIRE(e && e->finalized && e->session, "q3_session_begin first");
   Q3_REQUIRE(n >= 1 && n <= e->B && slots_host && keys_host && embeds_dev && lens_host, "bad argument");
-  // every request's parameters before anything else: one bad entry fails the whole admission and changes nothing
+  // every request's parameters before anything else: one bad entry fails the whole admission before any device work
   for (int r = 0; sp_host && r < n; ++r)
     if (check_sampling(sp_host[r])) {
       const std::string why = g_q3_err;
@@ -943,35 +978,11 @@ extern "C" int q3_admit_with_sampling(q3_engine* e, int32_t n, const int32_t* sl
   Q3_CUDA(cudaStreamSynchronize(stream));
   Q3_CUDA(cudaMemcpy(&hs, e->st, sizeof(hs), cudaMemcpyDeviceToHost));
   Q3_REQUIRE(hs.error == 0, "device-side error %d", hs.error);
-  const int F = hs.step;
-  e->frames_issued = F;
-  const int H = e->cfg.talker.hidden_size;
-  AdmitRows A{};
-  A.n = n;
-  int slots[MAXB];
-  for (int r = 0; r < n; ++r) {
-    const int b = slots_host[r];
-    Q3_REQUIRE(b >= 0 && b < e->B, "slot %d out of range", b);
-    Q3_REQUIRE(hs.finished[b] != 0 || !e->active[b], "slot %d is still running (q3_release_slots it first)", b);
-    for (int q = 0; q < r; ++q) Q3_REQUIRE(slots_host[q] != b, "slot %d admitted twice", b);
-    Q3_REQUIRE(lens_host[r] >= 1 && lens_host[r] < e->cfg.max_ctx, "prompt length %d out of range", lens_host[r]);
-    const int tl = trailing_lens_host ? trailing_lens_host[r] : 0;
-    Q3_REQUIRE(tl <= trailing_stride && tl <= e->trailing_cap, "trailing length %d exceeds the session's max_trailing %d", tl, e->trailing_cap);
-    slots[r] = b;
-    A.slot[r] = b; A.len0[r] = lens_host[r]; A.trailing_len[r] = tl;
-    e->len0[b] = lens_host[r] - F; e->frame0[b] = F; e->row_key[b] = keys_host[r]; e->trailing_len[b] = tl; e->active[b] = true;
-    if (tl > 0)
-      Q3_CUDA(cudaMemcpyAsync(e->trailing + (size_t)b * e->trailing_cap * H, reinterpret_cast<const bf16*>(trailing_dev) + (size_t)r * trailing_stride * H,
-                              (size_t)tl * H * 2, cudaMemcpyDeviceToDevice, stream));
-  }
-  for (int r = 0; r < n; ++r) e->row_sp[slots[r]] = sp_host ? sp_host[r] : e->sp;
+  unsigned int running = 0;
   for (int b = 0; b < e->B; ++b)
-    if (hs.finished[b] && !std::count(slots, slots + n, b)) e->active[b] = false;
-  e->max_len0 = 1;
-  for (int b = 0; b < e->B; ++b)
-    if (e->active[b]) e->max_len0 = std::max(e->max_len0, e->len0[b]);
-  admit_state_kernel<<<n, 256, 0, stream>>>(e->st, A, e->seen, e->cfg.talker.vocab_size);
-  return prefill_rows(e, n, slots, embeds_dev, lens_host, stream);
+    if (e->active[b] && !hs.finished[b]) running |= 1u << b;
+  const Admission A{n, slots_host, keys_host, sp_host, embeds_dev, lens_host, trailing_dev, trailing_lens_host, trailing_stride};
+  return admit_rows(e, A, hs.step, running, stream);
 }
 
 extern "C" int q3_admit(q3_engine* e, int32_t n, const int32_t* slots_host, const uint32_t* keys_host, const void* embeds_dev,
@@ -1014,7 +1025,7 @@ extern "C" int q3_append_trailing(q3_engine* e, int32_t slot, const void* rows_d
 extern "C" int q3_release_slots(q3_engine* e, int32_t n, const int32_t* slots_host, void* stream_) {
   Q3_REQUIRE(e && e->session && slots_host && n >= 0 && n <= MAXB, "bad argument");
   Q3_CUDA(cudaSetDevice(e->cfg.device));
-  AdmitRows A{};
+  SlotList A{};
   A.n = n;
   for (int r = 0; r < n; ++r) {
     Q3_REQUIRE(slots_host[r] >= 0 && slots_host[r] < e->B, "slot %d out of range", slots_host[r]);

@@ -42,13 +42,27 @@ __global__ void pf_rmsnorm_kernel(const bf16* __restrict__ x, const bf16* __rest
 // packed-token index (row, position) of all prompt tokens, built on the device from the prompt lengths (passed by
 // value: no host staging buffer, no synchronisation), and the gather of every row's last hidden state
 struct PfLens { int B; int start[MAXB + 1]; int slot[MAXB]; };  // row r of the packed prompt batch lives in engine slot slot[r]
-__global__ void pf_index_kernel(PfLens L, int* __restrict__ tok_seq, int* __restrict__ tok_pos) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= L.start[L.B]) return;
-  int b = 0;
-  while (i >= L.start[b + 1]) ++b;
-  tok_seq[i] = L.slot[b];
-  tok_pos[i] = i - L.start[b];
+// the admitted rows' trailing lengths and text [r][stride][H], gathered into the engine's copy [slot][cap][H]
+struct PfRows {
+  int trailing_len[MAXB];
+  const bf16* src; bf16* dst; int stride, cap, H;
+};
+// grid (x, row r): slice r resets row r's device state and seen bytes and gathers its trailing text (element-wise: the
+// source may be any bf16 pointer); slice 0 also writes the token index
+__global__ void pf_index_kernel(PfLens L, PfRows R, DevState* st, unsigned char* seen, int V, int* tok_seq, int* tok_pos) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x, r = blockIdx.y, b = L.slot[r];
+  if (r == 0 && i < L.start[L.B]) {
+    int s = 0;
+    while (i >= L.start[s + 1]) ++s;
+    tok_seq[i] = L.slot[s];
+    tok_pos[i] = i - L.start[s];
+  }
+  if (i == 0) {
+    st->finished[b] = 0; st->n_valid[b] = 0; st->n_gen[b] = 0; st->c0[b] = 0;
+    st->len0[b] = L.start[r + 1] - L.start[r]; st->trailing_len[b] = R.trailing_len[r];
+  }
+  if (i < V) seen[(size_t)b * V + i] = 0;
+  if (i < R.trailing_len[r] * R.H) R.dst[(size_t)b * R.cap * R.H + i] = R.src[(size_t)r * R.stride * R.H + i];
 }
 __global__ void pf_gather_last_kernel(PfLens L, const bf16* __restrict__ x, bf16* __restrict__ h_last, int H) {
   const int b = blockIdx.x;
@@ -57,19 +71,9 @@ __global__ void pf_gather_last_kernel(PfLens L, const bf16* __restrict__ x, bf16
   for (int i = threadIdx.x; i < H / 8; i += blockDim.x) dst[i] = src[i];
 }
 
-// continuous batching: (re)initialise the device-side state of the slots that receive a new request
-struct AdmitRows { int n; int slot[MAXB]; int len0[MAXB]; int trailing_len[MAXB]; };
-__global__ void admit_state_kernel(DevState* st, AdmitRows A, unsigned char* seen, int V) {
-  const int r = blockIdx.x, b = A.slot[r];
-  if (threadIdx.x == 0) {
-    st->finished[b] = 0; st->n_valid[b] = 0; st->n_gen[b] = 0; st->c0[b] = 0;
-    st->len0[b] = A.len0[r]; st->trailing_len[b] = A.trailing_len[r];
-  }
-  for (int i = threadIdx.x; i < V; i += blockDim.x) seen[(size_t)b * V + i] = 0;
-}
-
 // a row that is abandoned at its frame horizon: mark it finished (it keeps stepping like any finished row)
-__global__ void release_state_kernel(DevState* st, AdmitRows A) {
+struct SlotList { int n; int slot[MAXB]; };
+__global__ void release_state_kernel(DevState* st, SlotList A) {
   if ((int)threadIdx.x < A.n && !st->finished[A.slot[threadIdx.x]]) {
     st->finished[A.slot[threadIdx.x]] = 1;
     st->n_valid[A.slot[threadIdx.x]] = 0x3fffffff;  // "never sampled EOS": the host caps it at the frames it asked for

@@ -134,32 +134,32 @@ class AREngine:
         if lib.q3_sampling_check(C.byref(s)) != 0:
             raise ValueError(lib.q3_last_error().decode())
 
+    def _pack(self, inputs_embeds, trailing_text, stride=0):
+        """The prompts packed back to back [sum(lens)][H] with their lengths, and the trailing texts as [n][stride][H]
+        (stride at least the longest) with their lengths.  The engine reads row i's first tl[i] rows only."""
+        H = self.cfg.talker.hidden_size
+        n = len(inputs_embeds)
+        emb = torch.cat([e.reshape(-1, H) for e in inputs_embeds], 0).to(self.device, torch.bfloat16).contiguous()
+        lens = (C.c_int32 * n)(*[int(e.reshape(-1, H).shape[0]) for e in inputs_embeds])
+        tl = [int(t.reshape(-1, H).shape[0]) for t in trailing_text]
+        stride = max([int(stride)] + tl)
+        tr = torch.zeros(n, stride, H, dtype=torch.bfloat16, device=self.device)  # stride 0: empty, no row is read
+        for i, t in enumerate(trailing_text):
+            tr[i, :tl[i]] = t.reshape(-1, H).to(self.device, torch.bfloat16)
+        return emb, lens, tr, (C.c_int32 * n)(*tl), stride
+
     def prefill(self, inputs_embeds: Sequence[torch.Tensor], trailing_text: Sequence[torch.Tensor],
                 tts_pad_embed: torch.Tensor, sp: SamplingParams, trailing_capacity: int = 0):
         """`trailing_capacity` > longest trailing text reserves room for append_trailing() (streaming text input)."""
         B = len(inputs_embeds)
-        H = self.cfg.talker.hidden_size
-        dev = self.device
-        emb = torch.cat([e.reshape(-1, H) for e in inputs_embeds], 0).to(dev, torch.bfloat16).contiguous()
-        lens = (C.c_int32 * B)(*[int(e.reshape(-1, H).shape[0]) for e in inputs_embeds])
-        tl = [int(t.reshape(-1, H).shape[0]) for t in trailing_text]
-        Tt = max(max(tl) if tl else 0, int(trailing_capacity))
-        pad = tts_pad_embed.reshape(H).to(dev, torch.bfloat16).contiguous()
-        if Tt > 0:
-            tr = pad.expand(B, Tt, H).clone()
-            for i, t in enumerate(trailing_text):
-                if tl[i]:
-                    tr[i, :tl[i]] = t.reshape(-1, H).to(dev, torch.bfloat16)
-            trp = tr.data_ptr()
-        else:
-            tr, trp = None, None
-        tlen = (C.c_int32 * B)(*tl)
+        emb, lens, tr, tl, stride = self._pack(inputs_embeds, trailing_text, trailing_capacity)
+        pad = tts_pad_embed.reshape(self.cfg.talker.hidden_size).to(self.device, torch.bfloat16).contiguous()
         s = self._sampling(sp)
-        stream = torch.cuda.current_stream(dev).cuda_stream
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        _lib.check(self.lib.q3_prefill(self.h, B, emb.data_ptr(), lens, tr.data_ptr(), tl, stride,
+                                       pad.data_ptr(), C.byref(s), C.c_void_p(stream)))
         self._B = B
         self._hold = (emb, tr, pad)
-        _lib.check(self.lib.q3_prefill(self.h, B, emb.data_ptr(), lens, trp, tlen, Tt, pad.data_ptr(), C.byref(s),
-                                       C.c_void_p(stream)))
 
     # ------------------------------------------------------------------ continuous batching (low level)
     def session_begin(self, n_slots: int, tts_pad_embed: torch.Tensor, sp: SamplingParams, max_trailing: int = 0):
@@ -185,25 +185,12 @@ class AREngine:
             if len(sampling) != n:
                 raise ValueError(f"sampling has {len(sampling)} entries for {n} requests")
             sps = (_lib.Sampling * n)(*[self._sampling(self._session_sp if s is None else s) for s in sampling])
-        H = self.cfg.talker.hidden_size
-        dev = self.device
-        emb = torch.cat([e.reshape(-1, H) for e in inputs_embeds], 0).to(dev, torch.bfloat16).contiguous()
-        lens = (C.c_int32 * n)(*[int(e.reshape(-1, H).shape[0]) for e in inputs_embeds])
-        tl = [int(t.reshape(-1, H).shape[0]) for t in trailing_text]
-        Tt = max(tl) if tl else 0
-        if Tt > 0:
-            tr = torch.zeros(n, Tt, H, dtype=torch.bfloat16, device=dev)
-            for i, t in enumerate(trailing_text):
-                if tl[i]:
-                    tr[i, :tl[i]] = t.reshape(-1, H).to(dev, torch.bfloat16)
-            trp = tr.data_ptr()
-        else:
-            tr, trp = None, None
-        stream = torch.cuda.current_stream(dev).cuda_stream
+        emb, lens, tr, tl, stride = self._pack(inputs_embeds, trailing_text)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
         self._hold = self._hold + (emb, tr)
         _lib.check(self.lib.q3_admit_with_sampling(self.h, n, (C.c_int32 * n)(*[int(x) for x in slots]),
                                                    (C.c_uint32 * n)(*[int(k) & 0xffffffff for k in keys]), sps,
-                                                   emb.data_ptr(), lens, trp, (C.c_int32 * n)(*tl), Tt, C.c_void_p(stream)))
+                                                   emb.data_ptr(), lens, tr.data_ptr(), tl, stride, C.c_void_p(stream)))
 
     def append_trailing(self, slot: int, rows: torch.Tensor):
         """Streaming text input: more trailing_text_hidden rows (n, H) for a row that is already generating."""

@@ -58,6 +58,73 @@ def test_admitted_row_equals_alone_and_static():
     eng.close()
 
 
+def _alone(eng, pad, sp, emb, trail, key, frames):
+    """What one request generates alone: a one-slot session whose Philox row key is `key`."""
+    from qwen3_tts_b200.scheduler import ContinuousBatcher
+    cb = ContinuousBatcher(eng, pad, sp, n_slots=1, packet_frames=4)
+    cb.submit(emb, trail, key=key, max_frames=frames)
+    return cb.run()[key].cpu().numpy()
+
+
+def test_rejected_admission_changes_nothing():
+    """An admission that fails on its second row changes no row: its first row (a prompt of max_ctx - 1 positions,
+    which would overflow the KV cache at the next decode) is not admitted, the running request and a later valid
+    admission generate what each generates alone."""
+    import qwen3_tts_b200 as q
+    cfg, eng, embs, trail, pad = _setup()
+    sp = q.SamplingParams(do_sample=True, subtalker_dosample=True, top_k=50, temperature=0.9, subtalker_top_k=50,
+                          subtalker_temperature=0.9, repetition_penalty=1.05, max_new_tokens=25, suppress_eos=True, seed=5)
+    G, H, max_trailing = cfg.num_code_groups, cfg.talker.hidden_size, 4
+    g = torch.Generator().manual_seed(23)
+    long = (torch.randn(eng.max_ctx - 1, H, generator=g) * 0.5).bfloat16()
+    empty = torch.zeros(0, H, dtype=torch.bfloat16)
+    too_long = (torch.randn(max_trailing + 1, H, generator=g) * 0.1).bfloat16()
+    eng.session_begin(4, pad, sp, max_trailing=max_trailing)
+    codes = torch.zeros(4, 32, G, dtype=torch.int32, device=DEV)
+    eng.admit([3], [0], [embs[0]], [trail[0]])
+    eng.decode(4, codes)
+    rejected = [  # (slots, prompts, trailing texts, error)
+        ([0, 0, 1], [long, embs[1], embs[2]], [trail[0], trail[1], trail[2]], "slot 0 admitted twice"),
+        ([0, 1, 2], [long, empty, embs[2]], [trail[0], trail[1], trail[2]], "prompt length 0 out of range"),
+        ([0, 1, 2], [long, embs[1], embs[2]], [trail[0], too_long, trail[2]], f"trailing length {max_trailing + 1} exceeds"),
+    ]
+    for slots, prompts, trails, err in rejected:
+        with pytest.raises(RuntimeError, match=err):
+            eng.admit(slots, [10, 11, 12], prompts, trails)
+        eng.decode(4, codes)   # no progress() in between: it would clear a stale `active` flag of row 0
+    eng.admit([1], [1], [embs[1]], [trail[1]])
+    eng.decode(8, codes)
+    torch.cuda.synchronize()
+    got = codes.cpu().numpy()
+    for slot, key, frames in ((3, 0, 24), (1, 1, 8)):
+        ref = _alone(eng, pad, sp, embs[key], trail[key], key, frames)
+        assert (got[slot, :frames] == ref).all(), f"request {key} differs from its solo run at {np.argwhere(got[slot, :frames] != ref)[0]}"
+    eng.close()
+
+
+def test_rejected_prefill_changes_nothing():
+    """A static batch of another size rejected for its second row leaves the running batch's decode bit-identical."""
+    import dataclasses
+    import qwen3_tts_b200 as q
+    cfg, eng, embs, trail, pad = _setup()
+    sp = q.SamplingParams(do_sample=True, subtalker_dosample=True, top_k=50, temperature=0.9, max_new_tokens=9,
+                          suppress_eos=True, seed=5)
+    G, H = cfg.num_code_groups, cfg.talker.hidden_size
+    ref = torch.zeros(2, 8, G, dtype=torch.int32, device=DEV)
+    eng.prefill(embs[:2], trail[:2], pad, sp)
+    eng.decode(8, ref)
+    codes = torch.zeros(2, 8, G, dtype=torch.int32, device=DEV)
+    eng.prefill(embs[:2], trail[:2], pad, sp)
+    eng.decode(4, codes)
+    with pytest.raises(RuntimeError, match="prompt length 0 out of range"):
+        eng.prefill([embs[2], torch.zeros(0, H, dtype=torch.bfloat16), embs[3]], trail[2:5], pad,
+                    dataclasses.replace(sp, seed=99))
+    eng.decode(4, codes)
+    torch.cuda.synchronize()
+    assert (codes.cpu().numpy() == ref.cpu().numpy()).all()
+    eng.close()
+
+
 def test_eos_frees_the_slot_and_trims():
     """Rows that sample EOS leave the session at their own frame; their codes are trimmed like :2283-2290."""
     import qwen3_tts_b200 as q
