@@ -229,6 +229,17 @@ int q3_codec_stream_reset(q3_codec_stream* s, void* stream);
 int q3_codec_stream_reset_rows(q3_codec_stream* s, int32_t n, const int32_t* rows_host, void* stream);
 int q3_codec_stream_position(q3_codec_stream* s);
 int q3_codec_stream_row_position(q3_codec_stream* s, int32_t row);
+/* copy_rows: for i < n, row dst_rows_host[i] of dst becomes exactly row src_rows_host[i] of src (host int32 [n]): its
+ *   decoder state (the history of every buffer: conv tails, ConvTranspose overlap rows, each layer's K/V window) and
+ *   its position.  The destination row's previous state is replaced, so a running row needs no reset first.  Both
+ *   streams come from the same codec; their B and max_packet_frames may differ.  A source row may be listed more than
+ *   once (it is forked); a destination row may not.  One kernel launch, asynchronous on `stream`, no host sync.
+ *   Voice cloning decodes cat(ref_code, generated codes) and keeps the generated part (qwen3_tts_model.py:612-631):
+ *   decode the reference prefix once in a private stream, then copy its rows into the serving stream's rows.
+ *   Bad arguments (null or equal streams, different codecs, n outside [0, dst B], a row out of range, a destination
+ *   row listed twice) are rejected before any device work and change nothing. */
+int q3_codec_stream_copy_rows(q3_codec_stream* dst, const q3_codec_stream* src, int32_t n, const int32_t* src_rows_host,
+                              const int32_t* dst_rows_host, void* stream);
 void q3_codec_stream_close(q3_codec_stream* s);
 int q3_codec_total_upsample(q3_codec* c);
 /* kernels launched by the last q3_codec_forward or q3_codec_stream_step (bench.py's gpu_launches bookkeeping) */

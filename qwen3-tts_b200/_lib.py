@@ -67,6 +67,7 @@ CODEC_SYMBOLS = ["q3_codec_create", "q3_codec_destroy", "q3_codec_load_tensor", 
                  "q3_codec_forward", "q3_codec_total_upsample", "q3_codec_last_launch_count", "q3_codec_debug_capture",
                  "q3_codec_stream_open", "q3_codec_stream_step", "q3_codec_stream_reset", "q3_codec_stream_position", "q3_codec_stream_close",
                  "q3_codec_stream_step_rows", "q3_codec_stream_reset_rows", "q3_codec_stream_row_position",
+                 "q3_codec_stream_copy_rows",
                  "q3_codec_enc_create", "q3_codec_enc_destroy", "q3_codec_enc_load_tensor", "q3_codec_enc_finalize",
                  "q3_codec_enc_encode", "q3_codec_enc_frames", "q3_codec_enc_hop", "q3_codec_enc_last_launch_count",
                  "q3_codec_enc_debug_capture",
@@ -136,6 +137,7 @@ def load():
         lib.q3_codec_stream_step_rows.argtypes = [vp, vp, i32, C.POINTER(i32), vp, vp]
         lib.q3_codec_stream_reset_rows.argtypes = [vp, i32, C.POINTER(i32), vp]
         lib.q3_codec_stream_row_position.argtypes = [vp, i32]
+        lib.q3_codec_stream_copy_rows.argtypes = [vp, vp, i32, C.POINTER(i32), C.POINTER(i32), vp]
         lib.q3_codec_stream_close.argtypes = [vp]
         lib.q3_codec_stream_close.restype = None
         lib.q3_codec_total_upsample.argtypes = [vp]

@@ -22,6 +22,28 @@ def _kpad(k):
     return (k + 63) // 64 * 64
 
 
+SEED_PACKET_FRAMES = 32   # capacity of the private stream that decodes reference prefixes (CodecStream.seed)
+
+
+def check_ref_codes(cfg: CodecConfig, codes, max_len: int, what: str = "reference codes") -> int:
+    """Validate an utterance prefix in the layout of VoiceClonePromptItem.ref_code / encode().audio_codes: an integer
+    (L, num_quantizers) tensor with 1 <= L <= max_len and every code in [0, codebook_size) (an out-of-range code would
+    index past the codebook in the RVQ gather).  Raises ValueError; returns L."""
+    K = int(cfg.num_quantizers)
+    if not isinstance(codes, torch.Tensor) or codes.dim() != 2 or int(codes.shape[1]) != K:
+        shape = tuple(codes.shape) if isinstance(codes, torch.Tensor) else type(codes).__name__
+        raise ValueError(f"{what}: expected an (L, {K}) tensor, got {shape}")
+    if codes.dtype.is_floating_point or codes.dtype.is_complex or codes.dtype == torch.bool:
+        raise ValueError(f"{what}: expected integer codes, got {codes.dtype}")
+    L = int(codes.shape[0])
+    if not 1 <= L <= max_len:
+        raise ValueError(f"{what}: {L} frames outside [1, {max_len}]")
+    lo, hi = (int(v) for v in torch.aminmax(codes.to(torch.int64)))
+    if lo < 0 or hi >= int(cfg.codebook_size):
+        raise ValueError(f"{what}: codes must lie in [0, {cfg.codebook_size}), got values in [{lo}, {hi}]")
+    return L
+
+
 class CodecDecoder:
     def __init__(self, cfg: CodecConfig, weights, device="cuda:0", max_frames=1024, max_batch=32):
         self.lib = _lib.load()
@@ -271,6 +293,7 @@ class CodecStream:
         h = C.c_void_p()
         _lib.check(dec.lib.q3_codec_stream_open(dec.h, self.B, self.nmax, C.byref(h)))
         self.h = h
+        self._seeder: Optional["CodecStream"] = None   # private stream of seed(), opened on first use
 
     @property
     def position(self) -> int:
@@ -322,7 +345,44 @@ class CodecStream:
             rows = [int(r) for r in rows]
             _lib.check(self.dec.lib.q3_codec_stream_reset_rows(self.h, len(rows), (C.c_int32 * max(len(rows), 1))(*rows), stream))
 
+    @torch.no_grad()
+    def seed(self, rows: Sequence[int], codes: Sequence[torch.Tensor]):
+        """Start utterances in `rows` that continue the prefixes `codes` ((L_i, K) integer tensors, the layout of
+        VoiceClonePromptItem.ref_code): afterwards row rows[i] is at position L_i with exactly the state of reset +
+        a push of those L_i frames, so its next push decodes as cat(codes[i], next codes) would, and the prefix's own
+        audio is never produced here.  The prefixes are decoded together in a private stream of packets of
+        SEED_PACKET_FRAMES frames, whose rows are then copied over (q3_codec_stream_copy_rows); the other rows of this
+        stream are untouched.  Bad input raises ValueError before any device work."""
+        dec = self.dec
+        rows = [int(r) for r in rows]
+        if len(rows) != len(codes):
+            raise ValueError(f"{len(rows)} rows for {len(codes)} code prefixes")
+        for r in rows:
+            if not 0 <= r < self.B:
+                raise ValueError(f"seed row {r} out of range [0, {self.B})")
+        if len(set(rows)) != len(rows):
+            raise ValueError(f"seed rows {rows} are not distinct")
+        lens = [check_ref_codes(dec.cfg, c, dec.max_frames, f"row {r}: reference codes") for r, c in zip(rows, codes)]
+        n = len(rows)
+        if n == 0:
+            return
+        if self._seeder is None or self._seeder.B < n:
+            if self._seeder is not None:
+                self._seeder.close()
+            self._seeder = CodecStream(dec, n, min(SEED_PACKET_FRAMES, dec.max_frames))
+        sd = self._seeder
+        pkt = torch.zeros(sd.B, dec.cfg.num_quantizers, max(lens), dtype=torch.int32, device=dec.device)
+        for i, c in enumerate(codes):
+            pkt[i, :, :lens[i]] = c.to(dec.device, torch.int32).T
+        sd.reset()
+        sd.push(pkt, lens + [0] * (sd.B - n))   # the prefixes' audio is discarded
+        stream = C.c_void_p(torch.cuda.current_stream(dec.device).cuda_stream)
+        _lib.check(dec.lib.q3_codec_stream_copy_rows(self.h, sd.h, n, (C.c_int32 * n)(*range(n)), (C.c_int32 * n)(*rows), stream))
+
     def close(self):
+        if getattr(self, "_seeder", None) is not None:
+            self._seeder.close()
+            self._seeder = None
         if getattr(self, "h", None):
             self.dec.lib.q3_codec_stream_close(self.h)
             self.h = None

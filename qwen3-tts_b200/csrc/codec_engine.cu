@@ -228,6 +228,22 @@ __global__ void reset_history_kernel(RollTable tb, const int* __restrict__ rp, i
   for (int i = threadIdx.x; i < nv; i += blockDim.x) base[i] = make_uint4(0u, 0u, 0u, 0u);
 }
 
+// copy the history rows of listed batch rows from one stream's buffers to another's (same codec, so the entries of
+// both tables correspond one to one; B and the capacity, hence bs_rows, may differ).  rows[i] is the source row and
+// rows[ld + i] the destination row of pair i; block = (entry, pair).  Destination rows are distinct, so no two blocks
+// write the same bytes.
+struct CopyEntry { bf16* dst; const bf16* src; int hist, C, dst_bs_rows, src_bs_rows; };
+struct CopyTable { int n; CopyEntry e[kRollMax]; };
+static_assert(sizeof(CopyTable) + 2 * sizeof(void*) + 2 * sizeof(int) <= 4096, "copy_rows_kernel parameters exceed 4 KB");
+__global__ void copy_rows_kernel(CopyTable tb, const int* __restrict__ rows, int ld, int n) {
+  const CopyEntry E = tb.e[blockIdx.x / n];
+  const int i = blockIdx.x % n;
+  const uint4* src = reinterpret_cast<const uint4*>(E.src + (size_t)rows[i] * E.src_bs_rows * E.C);
+  uint4* dst = reinterpret_cast<uint4*>(E.dst + (size_t)rows[ld + i] * E.dst_bs_rows * E.C);
+  const int nv = E.hist * E.C / 8;
+  for (int v = threadIdx.x; v < nv; v += blockDim.x) dst[v] = src[v];
+}
+
 // final causal conv k=7, C -> 1, + clamp(-1,1) (…v2.py:863,884); one thread per output sample.  The T samples of a row
 // are `up` per frame; the samples of frames past the row's count are written as zeros.
 __global__ void final_conv_kernel(const bf16* __restrict__ x, const float* __restrict__ w /*[7][C]*/, const float* __restrict__ bias_p,
@@ -803,6 +819,40 @@ extern "C" int q3_codec_stream_reset_rows(q3_codec_stream* s, int32_t n, const i
   reset_history_kernel<<<tb.n * s->B, 128, 0, stream>>>(tb, s->rp, s->B);
   Q3_CUDA(cudaGetLastError());
   for (int b = 0; b < s->B; ++b) if (mask[b]) s->pos[b] = 0;
+  return 0;
+}
+
+// row dst_rows[i] of dst becomes row src_rows[i] of src: every history buffer's `hist` rows and the position.  Used to
+// seed a row with a reference prefix decoded elsewhere (qwen3_tts_model.py:612-631 decodes cat(ref_code, codes)).  The
+// source rows' pairs go up through dst's rp buffer ([0, n) source rows, [B, B + n) destination rows).
+extern "C" int q3_codec_stream_copy_rows(q3_codec_stream* dst, const q3_codec_stream* src, int32_t n, const int32_t* src_rows_host,
+                                         const int32_t* dst_rows_host, void* stream_) {
+  Q3_REQUIRE(dst && src, "null stream");
+  Q3_REQUIRE(src != dst, "source and destination are the same stream");
+  Q3_REQUIRE(src->c == dst->c, "source and destination streams belong to different codecs");
+  Q3_REQUIRE(n >= 0 && n <= dst->B, "%d rows to copy, the destination stream has %d", n, dst->B);
+  if (n == 0) return 0;
+  Q3_REQUIRE(src_rows_host && dst_rows_host, "null argument");
+  for (int i = 0; i < n; ++i) {
+    Q3_REQUIRE(src_rows_host[i] >= 0 && src_rows_host[i] < src->B, "source row %d out of range [0, %d)", src_rows_host[i], src->B);
+    Q3_REQUIRE(dst_rows_host[i] >= 0 && dst_rows_host[i] < dst->B, "destination row %d out of range [0, %d)", dst_rows_host[i], dst->B);
+    for (int j = 0; j < i; ++j) Q3_REQUIRE(dst_rows_host[i] != dst_rows_host[j], "destination row %d listed twice", dst_rows_host[i]);
+  }
+  const RollTable td = hist_table(dst), ts = hist_table(src);
+  Q3_REQUIRE(td.n == ts.n, "history tables differ (%d and %d buffers)", td.n, ts.n);
+  CopyTable tb{};
+  tb.n = td.n;
+  for (int k = 0; k < td.n; ++k) {
+    Q3_REQUIRE(td.e[k].hist == ts.e[k].hist && td.e[k].C == ts.e[k].C, "history buffer %d differs between the streams", k);
+    tb.e[k] = CopyEntry{td.e[k].p, ts.e[k].p, td.e[k].hist, td.e[k].C, td.e[k].bs_rows, ts.e[k].bs_rows};
+  }
+  Q3_CUDA(cudaSetDevice(dst->c->cfg.device));
+  cudaStream_t stream = (cudaStream_t)stream_;
+  for (int i = 0; i < n; ++i) { dst->rp_h[i] = src_rows_host[i]; dst->rp_h[dst->B + i] = dst_rows_host[i]; }
+  Q3_CUDA(cudaMemcpyAsync(dst->rp, dst->rp_h.data(), (size_t)2 * dst->B * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+  copy_rows_kernel<<<tb.n * n, 256, 0, stream>>>(tb, dst->rp, dst->B, n);
+  Q3_CUDA(cudaGetLastError());
+  for (int i = 0; i < n; ++i) dst->pos[dst_rows_host[i]] = src->pos[src_rows_host[i]];
   return 0;
 }
 

@@ -781,10 +781,11 @@ class Qwen3TTSModel:
                     x_vector_only_mode=[it.x_vector_only_mode for it in items], icl_mode=[it.icl_mode for it in items])
 
     # ---- :469-633
-    def generate_voice_clone(self, text, language=None, ref_audio=None, ref_text=None, x_vector_only_mode=False,
-                             voice_clone_prompt=None, non_streaming_mode=False, **kwargs):
+    def _voice_clone_inputs(self, text, language, ref_audio, ref_text, x_vector_only_mode, voice_clone_prompt, caller):
+        """generate_voice_clone's input handling (:469-603): list-ify and broadcast, validate, build the prompt from
+        raw audio when none is given, tokenise.  Returns (input_ids, ref_ids, voice_clone_prompt dict, languages)."""
         if self.model.tts_model_type != "base":
-            raise ValueError(f"model type {self.model.tts_model_type} does not support generate_voice_clone")
+            raise ValueError(f"model type {self.model.tts_model_type} does not support {caller}")
         texts = self._ensure_list(text)
         languages = self._ensure_list(language) if isinstance(language, list) else (
             [language] * len(texts) if language is not None else ["Auto"] * len(texts))
@@ -811,6 +812,26 @@ class Qwen3TTSModel:
         if ref_texts is not None:
             ref_ids = [None if (rt is None or rt == "") else self._tokenize_texts([self._build_ref_text(rt)])[0]
                        for rt in ref_texts]
+        return input_ids, ref_ids, vcp, languages
+
+    def build_voice_clone_requests(self, text, language=None, ref_audio=None, ref_text=None, x_vector_only_mode=False,
+                                   voice_clone_prompt=None, non_streaming_mode=False):
+        """generate_voice_clone's inputs as requests for the streaming paths (ContinuousBatcher.submit,
+        TTSEngine.stream_synthesize): ([(inputs_embeds, trailing_text, ref_code or None)] per text, tts_pad_embed).
+        A request's ref_code is what generate_voice_clone decodes in front of its codes; pass it as `ref_codes` so the
+        streamed audio is the part generate_voice_clone keeps."""
+        input_ids, ref_ids, vcp, languages = self._voice_clone_inputs(text, language, ref_audio, ref_text, x_vector_only_mode,
+                                                                      voice_clone_prompt, "build_voice_clone_requests")
+        embeds, trailing, pad = self.model.build_prefill(input_ids, ref_ids=ref_ids, voice_clone_prompt=vcp, languages=languages,
+                                                         non_streaming_mode=non_streaming_mode)
+        ref_codes = vcp.get("ref_code", None)
+        refs = [None if ref_codes is None else ref_codes[i] for i in range(len(embeds))]
+        return list(zip(embeds, trailing, refs)), pad
+
+    def generate_voice_clone(self, text, language=None, ref_audio=None, ref_text=None, x_vector_only_mode=False,
+                             voice_clone_prompt=None, non_streaming_mode=False, **kwargs):
+        input_ids, ref_ids, vcp, languages = self._voice_clone_inputs(text, language, ref_audio, ref_text, x_vector_only_mode,
+                                                                      voice_clone_prompt, "generate_voice_clone")
         codes, _ = self.model.generate(input_ids=input_ids, ref_ids=ref_ids, voice_clone_prompt=vcp, languages=languages,
                                        non_streaming_mode=non_streaming_mode, **self._merge_generate_kwargs(**kwargs))
         ref_codes = vcp.get("ref_code", None)

@@ -8,7 +8,7 @@ from typing import List, Sequence
 import numpy as np
 import torch
 
-from .codec import CodecDecoder
+from .codec import CodecDecoder, check_ref_codes
 from .config import CodecConfig, SamplingParams, TTSConfig
 from .engine import AREngine
 
@@ -55,13 +55,17 @@ class TTSEngine:
 
     @torch.no_grad()
     def stream_synthesize(self, inputs_embeds, trailing_text, tts_pad_embed, sp: SamplingParams, packet_frames: int = 4,
-                          left_context="stateful"):
+                          left_context="stateful", ref_codes=None):
         """Streaming OUTPUT (new surface: the reference returns audio whole, SURVEY F1).  Yields, per packet of
         `packet_frames` frames (4 frames = 320 ms, Qwen3-TTS report §3.4), a list with one fp32 numpy waveform chunk per
         row.  Default: the STATEFUL codec stream (q3_codec_stream_*) — each packet costs its own frames only and the
         concatenated chunks equal the one-shot causal decode.  `left_context=25` decodes every packet together with 25
         already-emitted frames, exactly like the reference's chunked_decode does between chunks (…v2.py:886-896);
-        `left_context=None` re-decodes the whole prefix."""
+        `left_context=None` re-decodes the whole prefix.
+        `ref_codes`: one entry per row, the (L, K) reference codes of a voice-clone row (VoiceClonePromptItem.ref_code)
+        or None.  A row's audio is then decoded as cat(ref_codes, generated codes) is (qwen3_tts_model.py:612-631):
+        the stateful stream seeds the row with its reference, the windowed modes start its history with it.  The
+        chunks hold the generated audio only."""
         dev = self.device
         emb = [e.to(dev, non_blocking=True) for e in inputs_embeds]
         tr = [t.to(dev, non_blocking=True) for t in trailing_text]
@@ -69,6 +73,14 @@ class TTSEngine:
         K = self.codec_cfg.num_quantizers
         up = self.codec.total_upsample
         B = len(emb)
+        refs = [None] * B
+        if ref_codes is not None:
+            if len(ref_codes) != B:
+                raise ValueError(f"ref_codes has {len(ref_codes)} entries for {B} rows")
+            for b, r in enumerate(ref_codes):
+                if r is not None:
+                    check_ref_codes(self.codec_cfg, r, self.codec.max_frames, f"row {b}: ref_codes")
+                    refs[b] = r.to(dev, torch.int64)
         if left_context == "stateful":
             key = (B, int(packet_frames))
             if getattr(self, "_cstream_key", None) != key:
@@ -78,6 +90,9 @@ class TTSEngine:
                 self._cstream_key = key
             cs = self._cstream
             cs.reset()
+            seeded = [b for b in range(B) if refs[b] is not None]
+            if seeded:
+                cs.seed(seeded, [refs[b] for b in seeded])
             for pkt in self.ar.stream(emb, tr, pad, sp, packet_frames=packet_frames):
                 n_new = [int(p.shape[0]) for p in pkt]
                 n = max(n_new) if n_new else 0
@@ -89,10 +104,12 @@ class TTSEngine:
                 for b, p in enumerate(pkt):
                     if p.shape[0]:
                         codes[b, :p.shape[0]] = p
-                wav = cs.push(codes.transpose(1, 2).contiguous())[:, 0].to(torch.float32).cpu().numpy()
+                # a seeded row starts past position 0: it takes its own frames only, so that padding never walks it
+                # past the RoPE table
+                wav = cs.push(codes.transpose(1, 2).contiguous(), n_new if seeded else None)[:, 0].to(torch.float32).cpu().numpy()
                 yield [wav[b, :n_new[b] * up] for b in range(B)]
             return
-        hist = [torch.zeros(0, K, dtype=torch.int64, device=dev) for _ in emb]
+        hist = [torch.zeros(0, K, dtype=torch.int64, device=dev) if r is None else r for r in refs]
         for pkt in self.ar.stream(emb, tr, pad, sp, packet_frames=packet_frames):
             out = [np.zeros(0, dtype=np.float32) for _ in pkt]
             # rows whose window has the same shape (the normal case: every live row got `packet_frames` new frames on top

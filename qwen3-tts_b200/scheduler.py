@@ -18,6 +18,12 @@ With a codec the batcher also streams audio: one codec stream of `n_slots` rows 
 reset when a request enters it, and after every decode each running slot pushes its new frames as its own count (idle
 slots push none).  A request's concatenated chunks equal the one-shot decode of its codes alone
 (tests/test_gpu_scheduler_audio.py).
+
+A request may carry reference codes (voice cloning, `ref_codes` of submit): the reference decodes cat(ref_code,
+generated codes) and cuts the reference's audio off (qwen3_tts_model.py:612-631), so the generated frames are decoded
+with the reference as their causal left context.  At admission such a slot's codec row is seeded with its reference
+(CodecStream.seed, one call for all seeded slots of the admission) instead of reset; its chunks and `done` entry hold
+the generated part only (tests/test_gpu_scheduler_voice_clone.py).
 """
 from collections import deque
 from dataclasses import dataclass, field
@@ -26,7 +32,7 @@ from typing import Deque, Dict, Iterator, List, Optional, Tuple
 import numpy as np
 import torch
 
-from .codec import CodecDecoder
+from .codec import CodecDecoder, check_ref_codes
 from .config import SamplingParams
 from .engine import AREngine
 
@@ -38,6 +44,7 @@ class _Request:
     trailing: torch.Tensor
     max_frames: int
     sampling: Optional[SamplingParams] = None
+    ref_codes: Optional[torch.Tensor] = None
     slot: int = -1
     emitted: int = 0
     chunks: List[torch.Tensor] = field(default_factory=list)
@@ -63,11 +70,19 @@ class ContinuousBatcher:
 
     # ------------------------------------------------------------------ API
     def submit(self, inputs_embeds: torch.Tensor, trailing_text: Optional[torch.Tensor] = None, key: Optional[int] = None,
-               max_frames: Optional[int] = None, sampling: Optional[SamplingParams] = None) -> int:
+               max_frames: Optional[int] = None, sampling: Optional[SamplingParams] = None,
+               ref_codes: Optional[torch.Tensor] = None) -> int:
         """Queue one request; returns its id (also its Philox row key unless `key` is given).  `sampling`: the
         request's own generation parameters (default: the session's); its max_new_tokens bounds the request's horizon
-        and may not exceed the session's.  Bad parameters raise ValueError here, never in a later step()."""
+        and may not exceed the session's.  `ref_codes`: (L, num_quantizers) reference codes of a voice-clone request
+        (VoiceClonePromptItem.ref_code); its audio is decoded after them, and the horizon leaves the codec's RoPE
+        table room for them.  Bad parameters raise ValueError here, never in a later step()."""
         H = self.eng.cfg.talker.hidden_size
+        L_ref = 0
+        if ref_codes is not None:
+            if self.codec is None:
+                raise ValueError("ref_codes need a ContinuousBatcher built with a codec")
+            L_ref = check_ref_codes(self.codec.cfg, ref_codes, self.codec.max_frames - 1, "ref_codes")
         limit = self.max_frames   # frames the request may generate: HF emits max_new_tokens - 1 complete frames
         if sampling is not None:
             self.eng.check_sampling(sampling)
@@ -87,8 +102,8 @@ class ContinuousBatcher:
             raise ValueError(f"prompt of {L} positions does not fit max_ctx={self.eng.max_ctx}")
         horizon = min(max_frames or limit, limit, room)
         if self.codec is not None:
-            horizon = min(horizon, self.codec.max_frames)  # a codec row's position may not pass its RoPE table
-        self.pending.append(_Request(rid, inputs_embeds, tr, horizon, sampling))
+            horizon = min(horizon, self.codec.max_frames - L_ref)  # a codec row's position may not pass its RoPE table
+        self.pending.append(_Request(rid, inputs_embeds, tr, horizon, sampling, ref_codes))
         return rid
 
     def step(self) -> List[int]:
@@ -121,7 +136,11 @@ class ContinuousBatcher:
             for r in batch:
                 self.running[r.slot] = r
             if self.cstream is not None:
-                self.cstream.reset([r.slot for r in batch])
+                seeded = [r for r in batch if r.ref_codes is not None]
+                if len(seeded) < len(batch):
+                    self.cstream.reset([r.slot for r in batch if r.ref_codes is None])
+                if seeded:
+                    self.cstream.seed([r.slot for r in seeded], [r.ref_codes for r in seeded])
         if not self.running:
             return {}, []
         n = min([self.packet] + [r.max_frames - r.emitted for r in self.running.values()])

@@ -7,8 +7,13 @@ and the aggregate audio seconds produced per wall second, with the card name and
 With --mix the requests carry their own sampling parameters: every fourth one top-p 0.8 (talker and subtalker, the
 generic sampler path), every fourth one greedy, the rest the session's; comparing with a run without it gives what
 such rows cost the whole session.
+With --voice-clone every second request carries a 3 s reference (38 frames of random valid codes) and a prompt longer
+by those frames, as an ICL voice-clone prompt is: its codec row is seeded with the reference at admission
+(CodecStream.seed).  The probe then also reports the seed time per admission, the first-chunk times of voice-clone and
+plain requests apart, and, for comparison in the same run, the time to push one reference through an n_slots-row
+stream of the session's packet size, which is what seeding through the session's own stream would stall it for.
 
-    python tools/serve_probe.py [--slots 8 32] [--requests-per-slot 3] [--packet 4] [--mix]
+    python tools/serve_probe.py [--slots 8 32] [--requests-per-slot 3] [--packet 4] [--mix] [--voice-clone]
 
 Prints one JSON line.  Writes nothing.
 """
@@ -25,6 +30,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 HORIZONS = (40, 64, 88, 112)   # frames; staggered so that slots free up at different steps
+REF_FRAMES = 38                # a 3 s voice-clone reference at 12.5 frames/s
 SAMPLE_RATE = 24000
 
 
@@ -50,11 +56,13 @@ def mixed_sampling(sp, i):
     return None
 
 
-def run_session(eng, codec, pad, sp, prompts, n_slots, packet, horizons, timed, mix=False):
-    """One session: n_slots requests at once, then one more per step until all are in.  Returns the measurements."""
+def run_session(eng, codec, pad, sp, prompts, n_slots, packet, horizons, timed, mix=False, refs=None):
+    """One session: n_slots requests at once, then one more per step until all are in.  refs[i]: request i's
+    reference codes or None.  Returns the measurements."""
     from qwen3_tts_b200.scheduler import ContinuousBatcher
     cb = ContinuousBatcher(eng, pad, sp, n_slots=n_slots, packet_frames=packet, codec=codec)
-    t_ar, t_codec = [], []
+    t_ar, t_codec, t_seed = [], [], []
+    refs = refs or [None] * len(prompts)
 
     def clocked(fn, acc):
         def call(*a, **k):
@@ -69,12 +77,13 @@ def run_session(eng, codec, pad, sp, prompts, n_slots, packet, horizons, timed, 
     if timed:
         eng.decode = clocked(type(eng).decode.__get__(eng), t_ar)
         cb.cstream.push = clocked(cb.cstream.push, t_codec)
+        cb.cstream.seed = clocked(cb.cstream.seed, t_seed)
     submitted, first, samples = {}, {}, 0
     todo = list(range(len(prompts)))
 
     def submit(i):
         rid = cb.submit(prompts[i], None, key=i, max_frames=horizons[i % len(horizons)],
-                        sampling=mixed_sampling(sp, i) if mix else None)
+                        sampling=mixed_sampling(sp, i) if mix else None, ref_codes=refs[i])
         submitted[rid] = time.perf_counter()
 
     for i in todo[:n_slots]:
@@ -94,11 +103,40 @@ def run_session(eng, codec, pad, sp, prompts, n_slots, packet, horizons, timed, 
             del eng.decode
         cb.cstream.close()
     wall = time.perf_counter() - t0
-    ms = lambda v: {"median": float(np.median(v)) * 1e3, "p90": float(np.percentile(v, 90)) * 1e3}  # noqa: E731
-    return {"requests": len(prompts), "steps": len(t_ar), "ar_ms_per_step": ms(t_ar) if t_ar else None,
-            "codec_ms_per_step": ms(t_codec) if t_codec else None,
-            "first_chunk_ms": ms(list(first.values())), "audio_s": samples / SAMPLE_RATE, "wall_s": wall,
-            "audio_s_per_wall_s": samples / SAMPLE_RATE / wall}
+    ms = lambda v: {"median": float(np.median(v)) * 1e3, "p90": float(np.percentile(v, 90)) * 1e3} if v else None  # noqa: E731
+    out = {"requests": len(prompts), "steps": len(t_ar), "ar_ms_per_step": ms(t_ar), "codec_ms_per_step": ms(t_codec),
+           "first_chunk_ms": ms(list(first.values())), "audio_s": samples / SAMPLE_RATE, "wall_s": wall,
+           "audio_s_per_wall_s": samples / SAMPLE_RATE / wall}
+    if any(r is not None for r in refs):
+        out["first_chunk_ms_voice_clone"] = ms([t for rid, t in first.items() if refs[rid] is not None])
+        out["first_chunk_ms_plain"] = ms([t for rid, t in first.items() if refs[rid] is None])
+        # the first admission also opens the private seed stream (device allocation): reported apart
+        out["seed_ms_first_admission"] = t_seed[0] * 1e3 if t_seed else None
+        out["seed_ms_per_admission"] = ms(t_seed[1:])
+        out["seed_admissions"] = len(t_seed)
+    return out
+
+
+def naive_seed_ms(codec, n_slots, packet, ref, reps=5):
+    """The path seeding avoids: one reference pushed through an n_slots-row stream of the session's packet size (every
+    row computed each step, the other rows with count 0).  Sync-clocked; median over `reps` after one warm-up."""
+    st = codec.open_stream(n_slots, max_packet_frames=packet)
+    codes = torch.zeros(n_slots, ref.shape[1], ref.shape[0], dtype=torch.int32, device=codec.device)
+    codes[0] = ref.T.to(codec.device, torch.int32)
+    counts = [ref.shape[0]] + [0] * (n_slots - 1)
+    ts = []
+    try:
+        for r in range(reps + 1):
+            st.reset([0])
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            st.push(codes, counts)
+            torch.cuda.synchronize()
+            if r:
+                ts.append(time.perf_counter() - t0)
+    finally:
+        st.close()
+    return {"median": float(np.median(ts)) * 1e3, "p90": float(np.percentile(ts, 90)) * 1e3}
 
 
 def main():
@@ -108,6 +146,8 @@ def main():
     ap.add_argument("--packet", type=int, default=4)
     ap.add_argument("--prompt-len", type=int, default=24)
     ap.add_argument("--mix", action="store_true", help="per-request parameters: 1/4 top-p 0.8, 1/4 greedy, the rest the session's")
+    ap.add_argument("--voice-clone", action="store_true",
+                    help=f"every second request carries a {REF_FRAMES}-frame reference and a prompt longer by it")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("serve_probe needs a CUDA device")
@@ -118,10 +158,11 @@ def main():
     dev = "cuda:0"
     cfg, ccfg = synthetic.cfg_1p7b(), q.CodecConfig()
     max_b = max(args.slots)
+    extra = REF_FRAMES if args.voice_clone else 0   # the reference's frames in the prompt and in the codec row
     eng = AREngine(cfg, synthetic.random_tts_weights(cfg, device="cpu", seed=0), device=dev, max_batch=max_b,
-                   max_ctx=args.prompt_len + max(HORIZONS) + 8)
+                   max_ctx=args.prompt_len + extra + max(HORIZONS) + 8)
     codec = CodecDecoder(ccfg, synthetic.random_codec_weights(ccfg, device="cpu", seed=0), device=dev,
-                         max_frames=max(HORIZONS) + 8, max_batch=max_b)
+                         max_frames=extra + max(HORIZONS) + 8, max_batch=max_b)
     H = cfg.talker.hidden_size
     g = torch.Generator().manual_seed(0)
     pad = (torch.randn(H, generator=g) * 0.1).bfloat16()
@@ -130,12 +171,21 @@ def main():
                    f"{args.packet}-frame packets, horizons {list(HORIZONS)} frames, n_slots requests at once then one "
                    "more per step", "sampling": "mixed: 1/4 top-p 0.8, 1/4 greedy, 1/2 session (top-k 50, T 0.9)" if args.mix
            else "uniform: top-k 50, T 0.9", "card": card(), "results": {}}
+    if args.voice_clone:
+        out["voice_clone"] = (f"every second request: {REF_FRAMES}-frame reference of random valid codes, prompt "
+                              f"{args.prompt_len + REF_FRAMES} positions instead of {args.prompt_len}")
     for S in args.slots:
         n_req = S * args.requests_per_slot
-        prompts = [(torch.randn(args.prompt_len, H, generator=g) * 0.5).bfloat16() for _ in range(n_req)]
-        run_session(eng, codec, pad, sp, prompts[:S], S, args.packet, (8,), timed=False, mix=args.mix)   # warm-up: every shape
-        out["results"][f"n_slots={S}"] = run_session(eng, codec, pad, sp, prompts, S, args.packet, HORIZONS, timed=True,
-                                                     mix=args.mix)
+        refs = [torch.randint(0, ccfg.codebook_size, (REF_FRAMES, ccfg.num_quantizers), generator=g)
+                if args.voice_clone and i % 2 == 1 else None for i in range(n_req)]
+        prompts = [(torch.randn(args.prompt_len + (0 if r is None else REF_FRAMES), H, generator=g) * 0.5).bfloat16()
+                   for r in refs]
+        run_session(eng, codec, pad, sp, prompts[:S], S, args.packet, (8,), timed=False, mix=args.mix,
+                    refs=refs[:S])   # warm-up: every shape
+        res = run_session(eng, codec, pad, sp, prompts, S, args.packet, HORIZONS, timed=True, mix=args.mix, refs=refs)
+        if args.voice_clone:
+            res["naive_push_ms_per_admission"] = naive_seed_ms(codec, S, args.packet, refs[1])
+        out["results"][f"n_slots={S}"] = res
     out["card_after"] = card()
     print(json.dumps(out))
     codec.close()
