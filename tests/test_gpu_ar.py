@@ -301,17 +301,18 @@ def test_full_shape_headline_variants(model, B, N):
 
 def test_long_context_cross_cta_split_attention():
     """ctx > 128 with few rows => the talker attention is split across CTAs (flash-decoding style) and combined by
-    the last arriver; checked against the oracle at ctx ~ 300 and ~ 600 (3 and 5 splits)."""
+    the last arriver; checked against the oracle at ctx ~ 300 and ~ 600 (3 and 5 splits) and at ctx >= 1921, where one
+    row reaches MAXSPLIT = 16 splits."""
     cfg = _tiny()
     Wb, Wf = Hh.bf16_weights(OT.random_weights(cfg, seed=8))
-    for lens in ([300], [600, 150]):
+    for lens, max_ctx in (([300], 1024), ([600, 150], 1024), ([1930], 2048)):
         B = len(lens)
         embs, trail, pad = Hh.make_inputs(cfg, lens, [0] * B, seed=13)
         N = 3
         sp = OT.SamplingCfg(do_sample=False, subtalker_dosample=False, max_new_tokens=N + 1, suppress_eos=True)
         ref = OT.generate(Wf, cfg, [e.float() for e in embs], [t.float() for t in trail], pad.float(), sp, record_logits=True)
         forced = torch.stack(ref.codes).numpy()
-        eng = _engine(cfg, Wb, max_ctx=1024)
+        eng = _engine(cfg, Wb, max_ctx=max_ctx)
         codes, tl, cl, prog = Hh.run_engine_forced(eng, embs, trail, pad, Hh.to_pkg_sampling(sp), forced, DEV)
         assert prog[0] == N
         for f in range(N + 1):
