@@ -6,115 +6,20 @@
 // The output is DISCRETE (argmin over 2048 centroids, 16 residual levels deep), so this path computes in fp32 end to
 // end: a bf16 tensor-core pipeline would flip nearest-centroid decisions relative to the fp32 reference and every
 // flip cascades down the residual chain.  Activations are [B][C][T] fp32 (time contiguous, the reference's own
-// layout); every Conv1d / Linear is one launch of a register-tiled direct convolution with the preceding ELU, the
-// bias, GELU, LayerScale and the residual add fused in.  It is a first correct version: ~12 GFLOP per 3 s of
-// audio on CUDA cores; moving the strided convolutions onto wgmma (tf32) is the follow-up once parity is pinned.
+// layout); every Conv1d / Linear is one launch of the register-tiled direct convolution of conv_f32.cu, which the
+// speaker encoder shares, with the preceding ELU, the bias, GELU, LayerScale and the residual add fused in.  It is a
+// first correct version: ~12 GFLOP per 3 s of audio on CUDA cores; moving the strided convolutions onto wgmma (tf32) is
+// the follow-up once parity is pinned.
 #include "common.cuh"
+#include "conv_f32.cuh"
+#include "dev_store.h"
 #include "../../include/qwen3tts_b200.h"
 
 #include <algorithm>
-#include <map>
 #include <string>
 #include <vector>
 
 namespace {
-
-constexpr int CT = 64;   // output channels per block
-constexpr int TT = 64;   // output time steps per block
-constexpr int CI = 8;    // input channels staged per iteration
-
-struct ConvArgs {
-  const float* x;      // [B][Cin][Tin]
-  const float* w;      // [Cout][Cin][k]
-  const float* bias;   // [Cout] or null
-  const float* scale;  // [Cout] or null (LayerScale): y = res + scale * (conv + bias)
-  const float* res;    // [B][Cout][Tout] or null
-  float* y;            // [B][Cout][Tout]
-  int Cin, Cout, Tin, Tout, k, stride, dil, pad_left;
-  int replicate;       // pad mode: 0 zeros, 1 edge replication (left and right)
-  int elu_in;          // ELU applied to x on load (the nn.ELU() in front of the conv)
-  int gelu_out;        // exact (erf) GELU on the result
-};
-
-__device__ __forceinline__ float elu1(float v) { return v > 0.f ? v : expm1f(v); }
-__device__ __forceinline__ float gelu_erf(float v) { return 0.5f * v * (1.f + erff(v * 0.70710678118654752440f)); }
-
-// y[b][co][t] = epi( bias[co] + sum_{ci,j} w[co][ci][j] * x~[b][ci][t*stride + j*dil - pad_left] )
-// block = 256 threads = 16 (channel groups of 4) x 16 (time lanes; each owns t = lane + 16*i, i < 4)
-__global__ void __launch_bounds__(256) conv1d_f32_kernel(const ConvArgs a) {
-  extern __shared__ float sm[];
-  const int XW = (TT - 1) * a.stride + (a.k - 1) * a.dil + 1;
-  float* xs = sm;                 // [CI][XW]
-  float* ws = sm + CI * XW;       // [CT][CI][k]
-  const int b = blockIdx.z, co0 = blockIdx.y * CT, t0 = blockIdx.x * TT;
-  const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
-  const int in0 = t0 * a.stride - a.pad_left;  // input index of xs[.][0]
-  const float* xb = a.x + (size_t)b * a.Cin * a.Tin;
-  float acc[4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-
-  for (int c0 = 0; c0 < a.Cin; c0 += CI) {
-    __syncthreads();
-#pragma unroll 4
-    for (int e = tid; e < CI * XW; e += 256) {
-      const int ci = e / XW, p = e - ci * XW;
-      float v = 0.f;
-      if (c0 + ci < a.Cin) {
-        int ti = in0 + p;
-        if (a.replicate) ti = min(max(ti, 0), a.Tin - 1);
-        if (ti >= 0 && ti < a.Tin) {
-          v = xb[(size_t)(c0 + ci) * a.Tin + ti];
-          if (a.elu_in) v = elu1(v);
-        }
-      }
-      xs[e] = v;
-    }
-    const int wk = CI * a.k;
-#pragma unroll 4
-    for (int e = tid; e < CT * wk; e += 256) {
-      const int co = e / wk, r = e - co * wk, ci = r / a.k, j = r - ci * a.k;
-      float v = 0.f;
-      if (co0 + co < a.Cout && c0 + ci < a.Cin) v = a.w[((size_t)(co0 + co) * a.Cin + c0 + ci) * a.k + j];
-      ws[e] = v;
-    }
-    __syncthreads();
-    for (int ci = 0; ci < CI; ++ci) {
-      const float* xr = xs + ci * XW;
-      for (int j = 0; j < a.k; ++j) {
-        float wv[4], xv[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) wv[i] = ws[((ty * 4 + i) * CI + ci) * a.k + j];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) xv[i] = xr[(tx + 16 * i) * a.stride + j * a.dil];
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-          for (int q = 0; q < 4; ++q) acc[i][q] = fmaf(wv[i], xv[q], acc[i][q]);
-      }
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int co = co0 + ty * 4 + i;
-    if (co >= a.Cout) continue;
-    const float bv = a.bias ? a.bias[co] : 0.f;
-    const float sc = a.scale ? a.scale[co] : 1.f;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const int t = t0 + tx + 16 * q;
-      if (t >= a.Tout) continue;
-      float v = acc[i][q] + bv;
-      if (a.gelu_out) v = gelu_erf(v);
-      const size_t o = ((size_t)b * a.Cout + co) * a.Tout + t;
-      if (a.scale) v = sc * v;
-      if (a.res) v = a.res[o] + v;
-      a.y[o] = v;
-    }
-  }
-}
 
 // LayerNorm over channels of x [B][C][T] (nn.LayerNorm(hidden), modeling_mimi.py:933-934).  Block = 32 time steps x 8
 // channel groups: loads stay coalesced along t, each thread reduces C/8 channels, groups combine through shared memory.
@@ -281,17 +186,11 @@ __global__ void __launch_bounds__(256) rvq_encode_kernel(const RvqArgs a) {
   }
 }
 
-struct DevT {
-  float* p = nullptr;
-  int64_t numel = 0;
-};
-
 }  // namespace
 
 struct q3_codec_enc {
   q3_codec_enc_cfg cfg;
-  std::map<std::string, DevT> t;
-  std::vector<void*> allocs;
+  DevStore store{"codec encoder"};
   float* buf[3] = {nullptr, nullptr, nullptr};
   size_t buf_elems = 0;
   const float** d_ptrs = nullptr;  // [3][nq] device pointer tables (E, ET, E2)
@@ -299,17 +198,6 @@ struct q3_codec_enc {
   bool finalized = false;
   int launches = 0;
   int hop = 1;
-
-  int alloc_bytes(void** p, size_t bytes) {
-    cudaError_t e = cudaMalloc(p, bytes);
-    if (e != cudaSuccess) return q3_set_err("cudaMalloc(%zu B) failed: %s", bytes, cudaGetErrorString(e));
-    allocs.push_back(*p);
-    return 0;
-  }
-  const DevT* get(const std::string& n) const {
-    auto it = t.find(n);
-    return it == t.end() ? nullptr : &it->second;
-  }
 };
 
 extern "C" int q3_codec_enc_create(const q3_codec_enc_cfg* cfg, q3_codec_enc** out) {
@@ -325,20 +213,16 @@ extern "C" int q3_codec_enc_create(const q3_codec_enc_cfg* cfg, q3_codec_enc** o
                  cfg->num_quantizers <= 64, "bad quantizer counts");
   Q3_REQUIRE(cfg->codebook_dim <= 1024, "codebook_dim > 1024 unsupported");
   Q3_REQUIRE(cfg->max_frames >= 1, "max_frames (rope table rows) must be positive");
+  if (conv_f32_init()) return 1;
   q3_codec_enc* e = new q3_codec_enc();
   e->cfg = *cfg;
   e->hop = cfg->downsample_stride;
   for (int i = 0; i < cfg->n_ratios; ++i) e->hop *= cfg->ratios[i];
-  Q3_CUDA(cudaFuncSetAttribute(conv1d_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
   *out = e;
   return 0;
 }
 
-extern "C" void q3_codec_enc_destroy(q3_codec_enc* e) {
-  if (!e) return;
-  for (void* p : e->allocs) cudaFree(p);
-  delete e;
-}
+extern "C" void q3_codec_enc_destroy(q3_codec_enc* e) { delete e; }
 
 extern "C" int q3_codec_enc_hop(q3_codec_enc* e) { return e ? e->hop : 0; }
 extern "C" int q3_codec_enc_last_launch_count(q3_codec_enc* e) { return e ? e->launches : 0; }
@@ -346,23 +230,8 @@ extern "C" int q3_codec_enc_last_launch_count(q3_codec_enc* e) { return e ? e->l
 extern "C" int q3_codec_enc_load_tensor(q3_codec_enc* e, const char* name, const float* dev, const int64_t* shape, int32_t ndim) {
   Q3_REQUIRE(e && name && dev && shape, "null argument");
   Q3_CUDA(cudaSetDevice(e->cfg.device));
-  int64_t n = 1;
-  for (int i = 0; i < ndim; ++i) n *= shape[i];
-  DevT d;
-  d.numel = n;
-  void* p = nullptr;
-  if (e->alloc_bytes(&p, ((size_t)n * 4 + 255) & ~(size_t)255)) return 1;
-  d.p = reinterpret_cast<float*>(p);
-  Q3_CUDA(cudaMemcpy(d.p, dev, (size_t)n * 4, cudaMemcpyDeviceToDevice));
-  e->t[name] = d;
-  return 0;
+  return e->store.load(name, dev, shape, ndim, DT_F32);
 }
-
-#define ENEED(var, nm, cnt)                                                                           \
-  const DevT* var = e->get(nm);                                                                       \
-  Q3_REQUIRE(var, "codec encoder: missing tensor %s", std::string(nm).c_str());                       \
-  Q3_REQUIRE(var->numel == (int64_t)(cnt), "codec encoder: tensor %s has %lld elements, expected %lld", \
-             std::string(nm).c_str(), (long long)var->numel, (long long)(cnt))
 
 extern "C" int q3_codec_enc_finalize(q3_codec_enc* e) {
   Q3_REQUIRE(e, "null encoder");
@@ -370,23 +239,20 @@ extern "C" int q3_codec_enc_finalize(q3_codec_enc* e) {
   Q3_CUDA(cudaSetDevice(g.device));
   const int nq = g.num_quantizers, K = g.codebook_size, D = g.codebook_dim;
   std::vector<const float*> tab(3 * nq);
+  const DevStore& S = e->store;
   for (int q = 0; q < nq; ++q) {
     const std::string p = "rvq." + std::to_string(q);
-    ENEED(a, p + ".e", (int64_t)K * D);
-    ENEED(b, p + ".et", (int64_t)K * D);
-    ENEED(c, p + ".e2", (int64_t)K);
-    tab[q] = a->p; tab[nq + q] = b->p; tab[2 * nq + q] = c->p;
+    if (!(tab[q] = S.need<float>(p + ".e", (int64_t)K * D)) || !(tab[nq + q] = S.need<float>(p + ".et", (int64_t)K * D)) ||
+        !(tab[2 * nq + q] = S.need<float>(p + ".e2", K)))
+      return 1;
   }
-  {
-    ENEED(a, "rope.cos", (int64_t)g.max_frames * (g.head_dim / 2));
-    ENEED(b, "rope.sin", (int64_t)g.max_frames * (g.head_dim / 2));
-    ENEED(c, "rvq.sem.proj.w", (int64_t)D * g.hidden_size);
-    ENEED(d, "rvq.ac.proj.w", (int64_t)D * g.hidden_size);
-    ENEED(f, "down.w", (int64_t)g.hidden_size * g.hidden_size * 2 * g.downsample_stride);
-    (void)a; (void)b; (void)c; (void)d; (void)f;
-  }
+  if (!S.need<float>("rope.cos", (int64_t)g.max_frames * (g.head_dim / 2)) ||
+      !S.need<float>("rope.sin", (int64_t)g.max_frames * (g.head_dim / 2)) || !S.need<float>("rvq.sem.proj.w", (int64_t)D * g.hidden_size) ||
+      !S.need<float>("rvq.ac.proj.w", (int64_t)D * g.hidden_size) ||
+      !S.need<float>("down.w", (int64_t)g.hidden_size * g.hidden_size * 2 * g.downsample_stride))
+    return 1;
   void* p = nullptr;
-  if (e->alloc_bytes(&p, tab.size() * sizeof(float*))) return 1;
+  if (e->store.alloc(&p, tab.size() * sizeof(float*))) return 1;
   e->d_ptrs = reinterpret_cast<const float**>(p);
   Q3_CUDA(cudaMemcpy(p, tab.data(), tab.size() * sizeof(float*), cudaMemcpyHostToDevice));
   e->finalized = true;
@@ -413,33 +279,20 @@ struct EncRunner {
 
   int conv(const std::string& wname, const float* x, float* y, int Cin, int Cout, int Tin, int k, int stride, int replicate,
            bool elu_in, bool gelu_out, const float* res, const std::string& scale_name, bool has_bias, int* Tout_) {
-    const DevT* w = e->get(wname + ".w");
-    Q3_REQUIRE(w, "codec encoder: missing tensor %s.w", wname.c_str());
-    Q3_REQUIRE(w->numel == (int64_t)Cout * Cin * k, "codec encoder: tensor %s.w has %lld elements, expected %lld", wname.c_str(),
-               (long long)w->numel, (long long)Cout * Cin * k);
-    const float* bias = nullptr;
-    if (has_bias) {
-      const DevT* bt = e->get(wname + ".b");
-      Q3_REQUIRE(bt && bt->numel == Cout, "codec encoder: missing/ill-shaped tensor %s.b", wname.c_str());
-      bias = bt->p;
-    }
-    const float* scale = nullptr;
-    if (!scale_name.empty()) {
-      const DevT* s = e->get(scale_name);
-      Q3_REQUIRE(s && s->numel == Cout, "codec encoder: missing/ill-shaped tensor %s", scale_name.c_str());
-      scale = s->p;
-    }
-    ConvArgs a{};
-    a.x = x; a.w = w->p; a.bias = bias; a.scale = scale; a.res = res; a.y = y;
+    const DevStore& S = e->store;
+    ConvF32Args a{};
+    if (!(a.w = S.need<float>(wname + ".w", (int64_t)Cout * Cin * k))) return 1;
+    if (has_bias && !(a.bias = S.need<float>(wname + ".b", Cout))) return 1;
+    if (!scale_name.empty() && !(a.scale = S.need<float>(scale_name, Cout))) return 1;
+    a.x = x; a.res = res; a.y = y;
+    a.xC = Cin; a.yC = Cout;
     a.Cin = Cin; a.Cout = Cout; a.Tin = Tin; a.k = k; a.stride = stride; a.dil = 1;
     a.pad_left = k - stride;                       // causal: padding_total on the left (modeling_mimi.py:343-345)
     a.Tout = (Tin + stride - 1) / stride;          // right "extra padding" up to a stride multiple (:273-285)
-    a.replicate = replicate; a.elu_in = elu_in ? 1 : 0; a.gelu_out = gelu_out ? 1 : 0;
-    const int XW = (TT - 1) * stride + (k - 1) + 1;
-    const size_t smem = (size_t)(CI * XW + CT * CI * k) * sizeof(float);
-    Q3_REQUIRE(smem <= 96 * 1024, "conv tile needs %zu B of shared memory", smem);
-    dim3 grid((a.Tout + TT - 1) / TT, (Cout + CT - 1) / CT, B);
-    conv1d_f32_kernel<<<grid, 256, smem, st>>>(a);
+    a.pad = replicate ? PAD_REPLICATE : PAD_ZERO;
+    a.act_in = elu_in ? IN_ELU : IN_NONE;
+    a.act_out = gelu_out ? OUT_GELU : OUT_NONE;
+    if (conv_f32_launch(a, B, st)) return 1;
     ++e->launches;
     if (Tout_) *Tout_ = a.Tout;
     return 0;
@@ -481,11 +334,9 @@ extern "C" int q3_codec_enc_encode(q3_codec_enc* e, const float* wav_dev, int32_
     need *= (size_t)B;
   }
   if (need > e->buf_elems) {
-    for (int i = 0; i < 3; ++i) {
-      void* p = nullptr;
-      if (e->alloc_bytes(&p, need * 4)) return 1;
-      e->buf[i] = reinterpret_cast<float*>(p);
-    }
+    e->buf_elems = 0;
+    for (float*& b : e->buf)
+      if (e->store.grow(&b, need * 4, st)) return 1;
     e->buf_elems = need;
   }
   float *X = e->buf[0], *Y = e->buf[1], *Z = e->buf[2];
@@ -509,21 +360,24 @@ extern "C" int q3_codec_enc_encode(q3_codec_enc* e, const float* wav_dev, int32_
   r.capture(Y, g.hidden_size, t);
   // ---- transformer (:926-993): h lives in Y; X = normed / attention output, Z = qkv / mlp hidden
   const int C = g.hidden_size, nh = g.num_heads, hd = g.head_dim, I = g.intermediate_size;
-  const DevT *cosT = e->get("rope.cos"), *sinT = e->get("rope.sin");
+  const float* cosT = e->store.need<float>("rope.cos", (int64_t)g.max_frames * (hd / 2));
+  const float* sinT = e->store.need<float>("rope.sin", (int64_t)g.max_frames * (hd / 2));
+  if (!cosT || !sinT) return 1;
   float* H = Y;
   float* A = X;
   for (int l = 0; l < g.num_layers; ++l) {
     const std::string p = "tr." + std::to_string(l);
-    const DevT *l1w = e->get(p + ".ln1.w"), *l1b = e->get(p + ".ln1.b"), *l2w = e->get(p + ".ln2.w"), *l2b = e->get(p + ".ln2.b");
-    Q3_REQUIRE(l1w && l1b && l2w && l2b && l1w->numel == C && l1b->numel == C && l2w->numel == C && l2b->numel == C,
-               "codec encoder: missing/ill-shaped LayerNorm tensors of %s", p.c_str());
+    const DevStore& S = e->store;
+    const float *l1w = S.need<float>(p + ".ln1.w", C), *l1b = S.need<float>(p + ".ln1.b", C), *l2w = S.need<float>(p + ".ln2.w", C),
+                *l2b = S.need<float>(p + ".ln2.b", C);
+    if (!l1w || !l1b || !l2w || !l2b) return 1;
     dim3 lg((t + 31) / 32, B);
-    layernorm_ct_kernel<<<lg, 256, 0, st>>>(H, l1w->p, l1b->p, A, C, t, g.norm_eps);
+    layernorm_ct_kernel<<<lg, 256, 0, st>>>(H, l1w, l1b, A, C, t, g.norm_eps);
     if (r.conv(p + ".qkv", A, Z, C, 3 * C, t, 1, 1, 0, false, false, nullptr, "", false, &to)) return 1;
-    rope_ct_kernel<<<dim3((t + 127) / 128, 2 * nh * (hd / 2), B), 128, 0, st>>>(Z, cosT->p, sinT->p, C, t, nh, hd);
+    rope_ct_kernel<<<dim3((t + 127) / 128, 2 * nh * (hd / 2), B), 128, 0, st>>>(Z, cosT, sinT, C, t, nh, hd);
     swa_ct_kernel<64><<<dim3((t + 127) / 128, nh, B), 128, 0, st>>>(Z, A, C, t, hd, g.sliding_window, 1.0f / sqrtf((float)hd));
     if (r.conv(p + ".o", A, H, C, C, t, 1, 1, 0, false, false, H, p + ".ls1", false, &to)) return 1;  // h += ls1 * o_proj(attn)
-    layernorm_ct_kernel<<<lg, 256, 0, st>>>(H, l2w->p, l2b->p, A, C, t, g.norm_eps);
+    layernorm_ct_kernel<<<lg, 256, 0, st>>>(H, l2w, l2b, A, C, t, g.norm_eps);
     if (r.conv(p + ".fc1", A, Z, C, I, t, 1, 1, 0, false, true, nullptr, "", false, &to)) return 1;
     if (r.conv(p + ".fc2", Z, H, I, C, t, 1, 1, 0, false, false, H, p + ".ls2", false, &to)) return 1;  // h += ls2 * fc2(gelu(fc1))
     e->launches += 4;

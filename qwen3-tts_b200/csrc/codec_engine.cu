@@ -7,36 +7,15 @@
 // Small row-wise ops (RVQ gather, RMSNorm, RoPE, 72-frame sliding-window attention, depthwise conv + LayerNorm,
 // the final 96->1 conv + clamp) are plain CUDA kernels: they are <2 % of the FLOPs and HBM-trivial.
 #include "common.cuh"
+#include "dev_store.h"
 #include "gemm_sm90.cuh"
 #include "../../include/qwen3tts_b200.h"
 
 #include <algorithm>
-#include <map>
 #include <string>
 #include <vector>
 
 #include "codec_kernels.cuh"
-
-namespace {
-
-struct DevTensor {
-  void* p = nullptr;
-  int dtype = 0;  // 0 = bf16, 1 = f32
-  int64_t numel = 0;
-};
-
-}  // namespace
-
-// =================================================================================================
-// cudaMalloc `bytes` (zeroed if `zero`) and register the block in `allocs`, which its owner frees
-static int dev_alloc(std::vector<void*>& allocs, void** p, size_t bytes, bool zero) {
-  cudaError_t e = cudaMalloc(p, bytes);
-  if (e != cudaSuccess) return q3_set_err("cudaMalloc(%zu B) failed: %s", bytes, cudaGetErrorString(e));
-  allocs.push_back(*p);
-  if (zero && (e = cudaMemset(*p, 0, bytes)) != cudaSuccess)
-    return q3_set_err("cudaMemset(%zu B) failed: %s", bytes, cudaGetErrorString(e));
-  return 0;
-}
 
 // per-(row, frame) element high-water mark of the decoder's scratch tensors over all stages
 static size_t scratch_per_frame(const q3_codec_cfg& g) {
@@ -50,20 +29,16 @@ static size_t scratch_per_frame(const q3_codec_cfg& g) {
   return per_frame;
 }
 
-// the decoder's four scratch buffers X, Y, Z, W of `elems` bf16 each
-static int alloc_scratch(std::vector<void*>& allocs, bf16* buf[4], size_t elems) {
-  for (int i = 0; i < 4; ++i) {
-    void* p;
-    if (dev_alloc(allocs, &p, elems * 2 + 1024, false)) return 1;
-    buf[i] = reinterpret_cast<bf16*>(p);
-  }
+// (re)allocate the decoder's four scratch buffers X, Y, Z, W to `elems` bf16 each
+static int alloc_scratch(DevStore& store, bf16* buf[4], size_t elems, cudaStream_t stream) {
+  for (int i = 0; i < 4; ++i)
+    if (store.grow(&buf[i], elems * 2 + 1024, stream)) return 1;
   return 0;
 }
 
 struct q3_codec {
   q3_codec_cfg cfg;
-  std::map<std::string, DevTensor> t;
-  std::vector<void*> allocs;
+  DevStore store{"codec"};
   bf16* buf[4] = {nullptr, nullptr, nullptr, nullptr};
   size_t buf_elems = 0;
   bool finalized = false;
@@ -71,11 +46,6 @@ struct q3_codec {
   int launches = 0;
   struct Capture { int stage; bf16* dst; int64_t capacity; };
   std::vector<Capture> captures;  // test hook (q3_codec_debug_capture): stage ordinal -> destination of the next forward
-
-  const DevTensor* get(const std::string& n) const {
-    auto it = t.find(n);
-    return it == t.end() ? nullptr : &it->second;
-  }
 };
 
 extern "C" int q3_codec_create(const q3_codec_cfg* cfg, q3_codec** out) {
@@ -105,11 +75,7 @@ extern "C" int q3_codec_create(const q3_codec_cfg* cfg, q3_codec** out) {
   return 0;
 }
 
-extern "C" void q3_codec_destroy(q3_codec* c) {
-  if (!c) return;
-  for (void* p : c->allocs) cudaFree(p);
-  delete c;
-}
+extern "C" void q3_codec_destroy(q3_codec* c) { delete c; }
 
 extern "C" int q3_codec_total_upsample(q3_codec* c) { return c ? c->total_up : 0; }
 extern "C" int q3_codec_last_launch_count(q3_codec* c) { return c ? c->launches : 0; }
@@ -139,23 +105,8 @@ static bool name_is_bf16(const std::string& n) {
 extern "C" int q3_codec_load_tensor(q3_codec* c, const char* name, const void* dev, const int64_t* shape, int32_t ndim) {
   Q3_REQUIRE(c && name && dev && shape, "null argument");
   Q3_CUDA(cudaSetDevice(c->cfg.device));
-  int64_t n = 1;
-  for (int i = 0; i < ndim; ++i) n *= shape[i];
-  DevTensor d;
-  d.dtype = name_is_bf16(name) ? 0 : 1;
-  d.numel = n;
-  const size_t bytes = (size_t)n * (d.dtype == 0 ? 2 : 4);
-  if (dev_alloc(c->allocs, &d.p, (bytes + 255) & ~(size_t)255, false)) return 1;
-  Q3_CUDA(cudaMemcpy(d.p, dev, bytes, cudaMemcpyDeviceToDevice));
-  c->t[name] = d;
-  return 0;
+  return c->store.load(name, dev, shape, ndim, name_is_bf16(name) ? DT_BF16 : DT_F32);
 }
-
-#define NEED(var, nm, cnt)                                                                          \
-  const DevTensor* var = c->get(nm);                                                                \
-  Q3_REQUIRE(var, "codec: missing tensor %s", std::string(nm).c_str());                             \
-  Q3_REQUIRE(var->numel == (int64_t)(cnt), "codec: tensor %s has %lld elements, expected %lld",     \
-             std::string(nm).c_str(), (long long)var->numel, (long long)(cnt))
 
 static int kpad(int k) { return (k + 63) / 64 * 64; }
 
@@ -163,12 +114,10 @@ extern "C" int q3_codec_finalize(q3_codec* c) {
   Q3_REQUIRE(c, "null codec");
   const q3_codec_cfg& g = c->cfg;
   // spot-check the tensors whose absence would otherwise only surface mid-forward
-  {
-    NEED(a, "rvq.table", (int64_t)g.num_quantizers * g.codebook_size * (g.codebook_dim / 2));
-    NEED(b, "rvq.proj", (int64_t)g.codebook_dim * kpad(g.codebook_dim));
-    NEED(d, "dec.out.w", (int64_t)7 * (g.decoder_dim >> g.n_upsample_rates));
-    (void)a; (void)b; (void)d;
-  }
+  if (!c->store.need<bf16>("rvq.table", (int64_t)g.num_quantizers * g.codebook_size * (g.codebook_dim / 2)) ||
+      !c->store.need<bf16>("rvq.proj", (int64_t)g.codebook_dim * kpad(g.codebook_dim)) ||
+      !c->store.need<float>("dec.out.w", (int64_t)7 * (g.decoder_dim >> g.n_upsample_rates)))
+    return 1;
   c->finalized = true;
   return 0;
 }
@@ -186,16 +135,13 @@ struct Runner {
   void gemm(const bf16* a, int T, int K, int64_t a_bs, const char* wname, int N, int ntaps, const int* shifts, GemmEpilogue ep,
             const GemmViews& v) {
     if (err) return;
-    const DevTensor* w = c->get(wname);
     const int Kp = kpad(K);
-    if (!w || w->numel != (int64_t)N * ntaps * Kp) {
-      err = q3_set_err("codec: tensor %s missing or wrong size (want %lld)", wname, (long long)N * ntaps * Kp);
-      return;
-    }
+    const bf16* w = need<bf16>(wname, (int64_t)N * ntaps * Kp);
+    if (!w) return;
     if (ep.cmod == 0) ep.cmod = N;
     GemmPlan plan;
     const int mt = (T + 127) / 128;
-    if (gemm_make_plan_v(&plan, a, B, T, K, K, a_bs, reinterpret_cast<const bf16*>(w->p), N, Kp, ntaps, shifts,
+    if (gemm_make_plan_v(&plan, a, B, T, K, K, a_bs, w, N, Kp, ntaps, shifts,
                          gemm_pick_bn(N, mt, B), ep, v)) { err = 1; return; }
     if (gemm_launch(plan, stream)) { err = 1; return; }
     c->launches++;
@@ -210,15 +156,12 @@ struct Runner {
           err = q3_set_err("codec: capture of stage %d failed", stage);
       }
   }
-  const float* f32(const std::string& n, int64_t cnt) {
-    const DevTensor* d = c->get(n);
-    if (!d || d->numel != cnt || d->dtype != 1) { if (!err) err = q3_set_err("codec: fp32 tensor %s missing/wrong size", n.c_str()); return nullptr; }
-    return reinterpret_cast<const float*>(d->p);
-  }
-  const bf16* b16(const std::string& n, int64_t cnt) {
-    const DevTensor* d = c->get(n);
-    if (!d || d->numel != cnt || d->dtype != 0) { if (!err) err = q3_set_err("codec: bf16 tensor %s missing/wrong size", n.c_str()); return nullptr; }
-    return reinterpret_cast<const bf16*>(d->p);
+  // a tensor of the store; a missing or ill-shaped one fails the forward
+  template <class T>
+  const T* need(const std::string& n, int64_t cnt) {
+    const T* p = c->store.need<T>(n, cnt);
+    if (!p) err = 1;
+    return p;
   }
 };
 
@@ -251,7 +194,7 @@ struct q3_codec_stream {
   std::vector<int> pos;       // frames pushed per row since its last reset
   std::vector<int32_t> rp_h;  // host image of rp: [0, B) positions, [B, 2B) counts of the next step (reset mask of a reset)
   int32_t* rp = nullptr;      // device int32 [2][B], uploaded with one copy per step or reset
-  std::vector<void*> allocs;
+  DevStore store{"codec stream"};
   HistBuf pre, in, out;
   std::vector<HistBuf> dw, ct, kv;
   std::vector<std::vector<HistBuf>> c1;
@@ -295,7 +238,7 @@ static int decode_frames(q3_codec* c, const q3_codec_stream* s, const int32_t* c
 
   // ---- RVQ decode -> X [B][n][codebook_dim]; projection -> pre_conv's input
   const int D = g.codebook_dim / 2;
-  rvq_gather_kernel<<<B * n, 128, 0, stream>>>(codes, R.b16("rvq.table", (int64_t)g.num_quantizers * g.codebook_size * D), X, B,
+  rvq_gather_kernel<<<B * n, 128, 0, stream>>>(codes, R.need<bf16>("rvq.table", (int64_t)g.num_quantizers * g.codebook_size * D), X, B,
                                                g.num_quantizers, n, D, g.codebook_size, rp);
   c->launches++;
   if (R.err) return 1;
@@ -303,36 +246,36 @@ static int decode_frames(q3_codec* c, const q3_codec_stream* s, const int32_t* c
   { GemmEpilogue e = none; e.out_raw = pre.cur(); GemmViews v; v.raw_bs = pre.bs();
     R.gemm(X, n, g.codebook_dim, (int64_t)n * g.codebook_dim, "rvq.proj", g.codebook_dim, 1, &zero, e, v); }
   // ---- pre_conv k=3 (…v2.py:839-843,874)
-  { const int sh[3] = {-2, -1, 0}; GemmEpilogue e = none; e.bias = R.f32("pre_conv.b", Cl); e.out_raw = X;
+  { const int sh[3] = {-2, -1, 0}; GemmEpilogue e = none; e.bias = R.need<float>("pre_conv.b", Cl); e.out_raw = X;
     R.gemm(pre.p, n, g.codebook_dim, pre.bs(), "pre_conv.w", Cl, 3, sh, e, view_in(pre, n)); }
   capture(0, X, (int64_t)B * n * Cl);
   // ---- pre_transformer (…v2.py:501-575); the stream keeps a K/V window per layer
-  { GemmEpilogue e = none; e.bias = R.f32("tr.in.b", Hh); e.out_raw = Y; R.gemm(X, n, Cl, (int64_t)n * Cl, "tr.in.w", Hh, 1, &zero, e, {}); }
+  { GemmEpilogue e = none; e.bias = R.need<float>("tr.in.b", Hh); e.out_raw = Y; R.gemm(X, n, Cl, (int64_t)n * Cl, "tr.in.w", Hh, 1, &zero, e, {}); }
   bf16* xres = Y;  // residual stream [B][n][Hh]
   const int rows = B * n;
-  const bf16* cosT = R.b16("rope.cos", (int64_t)g.max_frames * (hd / 2));
-  const bf16* sinT = R.b16("rope.sin", (int64_t)g.max_frames * (hd / 2));
+  const bf16* cosT = R.need<bf16>("rope.cos", (int64_t)g.max_frames * (hd / 2));
+  const bf16* sinT = R.need<bf16>("rope.sin", (int64_t)g.max_frames * (hd / 2));
   for (int l = 0; l < g.num_layers && !R.err; ++l) {
     const std::string p = "tr." + std::to_string(l);
-    rmsnorm_rows_kernel<<<(rows + 7) / 8, 256, 0, stream>>>(xres, R.b16(p + ".ln1", Hh), X, rows, Hh, g.rms_eps);
+    rmsnorm_rows_kernel<<<(rows + 7) / 8, 256, 0, stream>>>(xres, R.need<bf16>(p + ".ln1", Hh), X, rows, Hh, g.rms_eps);
     { GemmEpilogue e = none; e.out_raw = Z; R.gemm(X, n, Hh, (int64_t)n * Hh, (p + ".qkv.w").c_str(), 3 * nh * hd, 1, &zero, e, {}); }
     // keys and values: the stream appends them to the layer's window buffer, the one-shot attends over qkv itself
     const HistBuf kv = s ? s->kv[l] : HistBuf{Z + nh * hd, 0, 3 * nh * hd, n};
     rope_append_kernel<<<296, 256, 0, stream>>>(Z, cosT, sinT, s ? kv.p : nullptr, B, n, nh, hd, rp, kv.hist, kv.bs_rows());
     swa_stream_kernel<<<(rows * nh + 7) / 8, 256, 0, stream>>>(Z, kv.p, kv.C, kv.bs_rows(), kv.hist, X, B, n, nh, hd,
                                                                 g.sliding_window, rp);
-    { GemmEpilogue e = none; e.scale = R.f32(p + ".ls1", Hh); e.resid = xres; e.out_raw = W;
+    { GemmEpilogue e = none; e.scale = R.need<float>(p + ".ls1", Hh); e.resid = xres; e.out_raw = W;
       R.gemm(X, n, nh * hd, (int64_t)n * nh * hd, (p + ".o.w").c_str(), Hh, 1, &zero, e, {}); }
-    rmsnorm_rows_kernel<<<(rows + 7) / 8, 256, 0, stream>>>(W, R.b16(p + ".ln2", Hh), X, rows, Hh, g.rms_eps);
+    rmsnorm_rows_kernel<<<(rows + 7) / 8, 256, 0, stream>>>(W, R.need<bf16>(p + ".ln2", Hh), X, rows, Hh, g.rms_eps);
     { GemmEpilogue e = none; e.act = ACT_SWIGLU_PAIR; e.out_act = Z;
       R.gemm(X, n, Hh, (int64_t)n * Hh, (p + ".gate_up.w").c_str(), 2 * I, 1, &zero, e, {}); }
-    { GemmEpilogue e = none; e.scale = R.f32(p + ".ls2", Hh); e.resid = W; e.out_raw = xres;
+    { GemmEpilogue e = none; e.scale = R.need<float>(p + ".ls2", Hh); e.resid = W; e.out_raw = xres;
       R.gemm(Z, n, I, (int64_t)n * I, (p + ".down.w").c_str(), Hh, 1, &zero, e, {}); }
     c->launches += 4;
   }
-  rmsnorm_rows_kernel<<<(rows + 7) / 8, 256, 0, stream>>>(xres, R.b16("tr.norm", Hh), X, rows, Hh, g.rms_eps);
+  rmsnorm_rows_kernel<<<(rows + 7) / 8, 256, 0, stream>>>(xres, R.need<bf16>("tr.norm", Hh), X, rows, Hh, g.rms_eps);
   c->launches++;
-  { GemmEpilogue e = none; e.bias = R.f32("tr.out.b", Cl); e.out_raw = Z; R.gemm(X, n, Hh, (int64_t)n * Hh, "tr.out.w", Cl, 1, &zero, e, {}); }
+  { GemmEpilogue e = none; e.bias = R.need<float>("tr.out.b", Cl); e.out_raw = Z; R.gemm(X, n, Hh, (int64_t)n * Hh, "tr.out.w", Cl, 1, &zero, e, {}); }
   capture(1, Z, (int64_t)B * n * Cl);
   // ---- upsample: ConvT(k=s=f) (no overlap) + ConvNeXt (depthwise k7) (…v2.py:845-855,878-880)
   bf16* cur = Z;  // [B][Tc][Cl] contiguous
@@ -341,19 +284,19 @@ static int decode_frames(q3_codec* c, const q3_codec_stream* s, const int32_t* c
     const int f = g.upsampling_ratios[i];
     const std::string p = "up." + std::to_string(i);
     const HistBuf dw = s ? s->dw[i] : HistBuf{Y, 0, Cl, Tc * f};
-    { GemmEpilogue e = none; e.bias = R.f32(p + ".ct.b", Cl); e.cmod = Cl; e.out_raw = dw.cur(); GemmViews v; v.raw_bs = dw.bs();
+    { GemmEpilogue e = none; e.bias = R.need<float>(p + ".ct.b", Cl); e.cmod = Cl; e.out_raw = dw.cur(); GemmViews v; v.raw_bs = dw.bs();
       R.gemm(cur, Tc, Cl, (int64_t)Tc * Cl, (p + ".ct.w").c_str(), f * Cl, 1, &zero, e, v); }
     Tc *= f;
-    const float *dww = R.f32(p + ".dw.w", (int64_t)Cl * 7), *dwb = R.f32(p + ".dw.b", Cl), *lw = R.f32(p + ".ln_g", Cl),
-                *lb = R.f32(p + ".ln_beta", Cl);
+    const float *dww = R.need<float>(p + ".dw.w", (int64_t)Cl * 7), *dwb = R.need<float>(p + ".dw.b", Cl), *lw = R.need<float>(p + ".ln_g", Cl),
+                *lb = R.need<float>(p + ".ln_beta", Cl);
     if (R.err) break;
     dwconv_ln_kernel<<<B * Tc, 256, (Cl + 64) * sizeof(float), stream>>>(dw.p, dww, dwb, lw, lb, X, B, Tc, Cl, dw.bs_rows(), dw.hist);
     c->launches++;
-    { GemmEpilogue e = none; e.bias = R.f32(p + ".pw1.b", 4 * Cl); e.act = ACT_GELU; e.out_act = W;
+    { GemmEpilogue e = none; e.bias = R.need<float>(p + ".pw1.b", 4 * Cl); e.act = ACT_GELU; e.out_act = W;
       R.gemm(X, Tc, Cl, (int64_t)Tc * Cl, (p + ".pw1.w").c_str(), 4 * Cl, 1, &zero, e, {}); }
     // the stream's last stage writes decoder.0's input; every other stage writes Z, whose input `cur` is consumed
     const HistBuf o = (s && i + 1 == g.n_upsampling_ratios) ? s->in : HistBuf{Z, 0, Cl, Tc};
-    { GemmEpilogue e = none; e.bias = R.f32(p + ".pw2.b", Cl); e.scale = R.f32(p + ".gamma", Cl); e.resid = dw.cur(); e.out_raw = o.cur();
+    { GemmEpilogue e = none; e.bias = R.need<float>(p + ".pw2.b", Cl); e.scale = R.need<float>(p + ".gamma", Cl); e.resid = dw.cur(); e.out_raw = o.cur();
       GemmViews v; v.resid_bs = dw.bs(); v.raw_bs = o.bs();
       R.gemm(W, Tc, 4 * Cl, (int64_t)Tc * 4 * Cl, (p + ".pw2.w").c_str(), Cl, 1, &zero, e, v); }
     cur = o.cur();
@@ -365,8 +308,8 @@ static int decode_frames(q3_codec* c, const q3_codec_stream* s, const int32_t* c
   {
     const HistBuf o = block_in(0, C, Tc);
     const int sh[7] = {-6, -5, -4, -3, -2, -1, 0};
-    GemmEpilogue e = none; e.bias = R.f32("dec.in.b", C); e.act = ACT_SNAKE; e.snake_ea = R.f32("dec.0.snake_ea", C);
-    e.snake_ib = R.f32("dec.0.snake_ib", C); e.out_act = o.cur();
+    GemmEpilogue e = none; e.bias = R.need<float>("dec.in.b", C); e.act = ACT_SNAKE; e.snake_ea = R.need<float>("dec.0.snake_ea", C);
+    e.snake_ib = R.need<float>("dec.0.snake_ib", C); e.out_act = o.cur();
     GemmViews v = view_in(in, Tc); v.act_bs = o.bs();
     R.gemm(in.p, Tc, Cl, in.bs(), "dec.in.w", C, 7, sh, e, v);
     capture(3, o.cur(), (int64_t)B * Tc * C);  // SnakeBeta(decoder.0 output) with block 0's leading activation
@@ -379,8 +322,8 @@ static int decode_frames(q3_codec* c, const q3_codec_stream* s, const int32_t* c
     {
       const HistBuf a = block_in(bi, C, Tc), o = unit_in(bi, 0, Co, Tc * r);
       const int sh[2] = {0, -1};
-      GemmEpilogue e = none; e.bias = R.f32(p + ".ct.b", Co); e.cmod = Co; e.out_raw = Y; e.act = ACT_SNAKE;
-      e.snake_ea = R.f32(p + ".0.s1_ea", Co); e.snake_ib = R.f32(p + ".0.s1_ib", Co); e.out_act = o.cur();
+      GemmEpilogue e = none; e.bias = R.need<float>(p + ".ct.b", Co); e.cmod = Co; e.out_raw = Y; e.act = ACT_SNAKE;
+      e.snake_ea = R.need<float>(p + ".0.s1_ea", Co); e.snake_ib = R.need<float>(p + ".0.s1_ib", Co); e.out_act = o.cur();
       GemmViews v = view_in(a, Tc); v.act_bs = o.bs();
       R.gemm(a.p, Tc, C, a.bs(), (p + ".ct.w").c_str(), r * Co, 2, sh, e, v);
     }
@@ -393,8 +336,8 @@ static int decode_frames(q3_codec* c, const q3_codec_stream* s, const int32_t* c
         const HistBuf a = unit_in(bi, u, C, Tc);
         int sh[7];
         for (int j = 0; j < 7; ++j) sh[j] = -(6 - j) * dil;
-        GemmEpilogue e = none; e.bias = R.f32(q + ".c1.b", C); e.act = ACT_SNAKE; e.snake_ea = R.f32(q + ".s2_ea", C);
-        e.snake_ib = R.f32(q + ".s2_ib", C); e.out_act = Z;
+        GemmEpilogue e = none; e.bias = R.need<float>(q + ".c1.b", C); e.act = ACT_SNAKE; e.snake_ea = R.need<float>(q + ".s2_ea", C);
+        e.snake_ib = R.need<float>(q + ".s2_ib", C); e.out_act = Z;
         R.gemm(a.p, Tc, C, a.bs(), (q + ".c1.w").c_str(), C, 7, sh, e, view_in(a, Tc));
       }
       {
@@ -403,8 +346,8 @@ static int decode_frames(q3_codec* c, const q3_codec_stream* s, const int32_t* c
                                  : (bi + 1 < nr ? ("dec." + std::to_string(bi + 1) + ".snake") : std::string("dec.out.snake"));
         const HistBuf o = (u < 2) ? unit_in(bi, u + 1, C, Tc) : block_in(bi + 1, C, Tc);
         // in place: the epilogue thread that writes a residual element has read it first
-        GemmEpilogue e = none; e.bias = R.f32(q + ".c2.b", C); e.resid = Y; e.out_raw = Y; e.act = ACT_SNAKE;
-        e.snake_ea = R.f32(nx + "_ea", C); e.snake_ib = R.f32(nx + "_ib", C); e.out_act = o.cur();
+        GemmEpilogue e = none; e.bias = R.need<float>(q + ".c2.b", C); e.resid = Y; e.out_raw = Y; e.act = ACT_SNAKE;
+        e.snake_ea = R.need<float>(nx + "_ea", C); e.snake_ib = R.need<float>(nx + "_ib", C); e.out_act = o.cur();
         GemmViews v; v.act_bs = o.bs();
         R.gemm(Z, Tc, C, (int64_t)Tc * C, (q + ".c2.w").c_str(), C, 1, &zero, e, v);
       }
@@ -415,8 +358,8 @@ static int decode_frames(q3_codec* c, const q3_codec_stream* s, const int32_t* c
   // ---- final conv k7 + clamp
   {
     const HistBuf a = block_in(nr, C, Tc);
-    const float* w = R.f32("dec.out.w", (int64_t)7 * C);
-    const float* bsrc = R.f32("dec.out.b", 1);
+    const float* w = R.need<float>("dec.out.w", (int64_t)7 * C);
+    const float* bsrc = R.need<float>("dec.out.b", 1);
     if (R.err) return 1;
     final_conv_kernel<<<1184, 256, 0, stream>>>(a.p, w, bsrc, wav, B, Tc, C, a.bs_rows(), a.hist, rp, c->total_up);  // bias read on the device
     c->launches++;
@@ -431,18 +374,20 @@ extern "C" int q3_codec_forward(q3_codec* c, const int32_t* codes_dev, int32_t B
   Q3_REQUIRE(T <= c->cfg.max_frames, "T=%d exceeds max_frames=%d", T, c->cfg.max_frames);
   Q3_CUDA(cudaSetDevice(c->cfg.device));
   const size_t need = scratch_per_frame(c->cfg) * (size_t)B * T;
+  cudaStream_t stream = (cudaStream_t)stream_;
   if (need > c->buf_elems) {
-    if (alloc_scratch(c->allocs, c->buf, need)) return 1;
+    c->buf_elems = 0;
+    if (alloc_scratch(c->store, c->buf, need, stream)) return 1;
     c->buf_elems = need;
   }
-  return decode_frames(c, nullptr, codes_dev, B, T, nullptr, c->buf, wav_dev, (cudaStream_t)stream_);
+  return decode_frames(c, nullptr, codes_dev, B, T, nullptr, c->buf, wav_dev, stream);
 }
 
 static int hist_alloc(q3_codec_stream* s, HistBuf* h, int hist, int C, int cap) {
   *h = HistBuf{nullptr, hist, C, cap};
   void* p = nullptr;
   // zero history == the causal left padding of a fresh stream
-  if (dev_alloc(s->allocs, &p, (size_t)s->B * h->bs_rows() * C * 2 + 256, true)) return 1;
+  if (s->store.alloc(&p, (size_t)s->B * h->bs_rows() * C * 2 + 256, true)) return 1;
   h->p = reinterpret_cast<bf16*>(p);
   return 0;
 }
@@ -477,23 +422,19 @@ extern "C" int q3_codec_stream_open(q3_codec* c, int32_t B, int32_t max_packet_f
     for (int u = 0; u < 3 && !rc; ++u) rc = hist_alloc(s, &s->c1[bi][u], 6 * dil[u], C, Tc);
   }
   if (!rc) rc = hist_alloc(s, &s->out, 6, C, Tc);
-  if (!rc) rc = alloc_scratch(s->allocs, s->buf, scratch_per_frame(g) * (size_t)B * n);
+  if (!rc) rc = alloc_scratch(s->store, s->buf, scratch_per_frame(g) * (size_t)B * n, nullptr);
   void* rp = nullptr;
-  if (!rc) rc = dev_alloc(s->allocs, &rp, (size_t)2 * B * sizeof(int32_t), true);
+  if (!rc) rc = s->store.alloc(&rp, (size_t)2 * B * sizeof(int32_t), true);
   s->rp = reinterpret_cast<int32_t*>(rp);
   s->pos.assign(B, 0);
   s->rp_h.assign(2 * B, 0);
-  if (rc) { for (void* p : s->allocs) cudaFree(p); delete s; return 1; }
+  if (rc) { delete s; return 1; }
   Q3_CUDA(cudaDeviceSynchronize());
   *out = s;
   return 0;
 }
 
-extern "C" void q3_codec_stream_close(q3_codec_stream* s) {
-  if (!s) return;
-  for (void* p : s->allocs) cudaFree(p);
-  delete s;
-}
+extern "C" void q3_codec_stream_close(q3_codec_stream* s) { delete s; }
 
 // the history buffers of a stream as a table for the roll and reset kernels.  A buffer's capacity is max_packet_frames
 // times its stage's rows per frame, so its factor is cap / nmax.  q3_codec_stream_open bounds the number of buffers.

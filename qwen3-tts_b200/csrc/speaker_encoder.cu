@@ -6,113 +6,19 @@
 // Checked against the CPU oracle by tests/test_gpu_speaker_encoder.py (log-mel, ECAPA embedding and the
 // waveform-to-embedding path at tiny and default shapes, golden vectors).
 //
-// fp32 throughout, activations [B][C][T] (time contiguous).  One generalised direct-convolution kernel serves every
-// Conv1d: reflect "same" padding with dilation, channel-sliced input/output (Res2Net chunks and the multi-layer feature
-// concatenation are views into one buffer, never copies), an optional second input added on load (Res2Net's
-// `part + previous output`), tanh-on-load, ReLU / sigmoid epilogues.  The STFT is a direct 1024-point DFT per frame
+// fp32 throughout, activations [B][C][T] (time contiguous).  Every Conv1d is one launch of the direct convolution of
+// conv_f32.cu, which the codec encoder shares: reflect "same" padding with dilation, channel-sliced input/output (Res2Net
+// chunks and the multi-layer feature concatenation are views into one buffer, never copies), an optional second input
+// added on load (Res2Net's `part + previous output`), tanh-on-load, ReLU / sigmoid epilogues.  The STFT is a direct 1024-point DFT per frame
 // against an exact periodic twiddle table (the Hann window is applied on load) fused with the mel projection and log.
 #include "common.cuh"
+#include "conv_f32.cuh"
+#include "dev_store.h"
 #include "../../include/qwen3tts_b200.h"
 
-#include <algorithm>
-#include <map>
 #include <string>
-#include <vector>
 
 namespace {
-
-constexpr int CT = 64, TT = 64, CI = 8;
-
-struct SConv {
-  const float* x;   // [B][xC][Tin]  (channels [x_off, x_off + Cin) are read)
-  const float* x2;  // optional second input added to x on load, [B][x2C][Tin] at channel offset x2_off
-  const float* w;   // [Cout][Cin][k]
-  const float* bias;
-  float* y;         // [B][yC][T]    (channels [y_off, y_off + Cout) are written)
-  int xC, x_off, x2C, x2_off, yC, y_off;
-  int Cin, Cout, T, k, dil;
-  int act_in;       // 0 none, 1 tanh applied to x on load
-  int act_out;      // 0 none, 1 ReLU, 2 sigmoid
-};
-
-__device__ __forceinline__ int reflect_idx(int i, int T) {
-  // torch "reflect" padding (no edge repetition); valid while the pad is < T
-  if (i < 0) i = -i;
-  if (i >= T) i = 2 * (T - 1) - i;
-  return min(max(i, 0), T - 1);
-}
-
-// y[b][y_off+co][t] = act_out( bias[co] + sum_{ci,j} w[co][ci][j] * X[b][ci][reflect(t + j*dil - left)] ),  left = dil*(k-1)/2
-// X = act_in(x [+ x2]).  nn.Conv1d(padding="same", padding_mode="reflect"): total pad dil*(k-1), left = total / 2.
-__global__ void __launch_bounds__(256) sconv_kernel(const SConv a) {
-  extern __shared__ float sm[];
-  const int XW = TT + (a.k - 1) * a.dil;
-  float* xs = sm;             // [CI][XW]
-  float* ws = sm + CI * XW;   // [CT][CI][k]
-  const int b = blockIdx.z, co0 = blockIdx.y * CT, t0 = blockIdx.x * TT;
-  const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
-  const int left = (a.dil * (a.k - 1)) / 2;
-  const float* xb = a.x + ((size_t)b * a.xC + a.x_off) * a.T;
-  const float* x2b = a.x2 ? a.x2 + ((size_t)b * a.x2C + a.x2_off) * a.T : nullptr;
-  float acc[4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-  for (int c0 = 0; c0 < a.Cin; c0 += CI) {
-    __syncthreads();
-#pragma unroll 4
-    for (int e = tid; e < CI * XW; e += 256) {
-      const int ci = e / XW, p = e - ci * XW;
-      float v = 0.f;
-      if (c0 + ci < a.Cin) {
-        const int ti = reflect_idx(t0 + p - left, a.T);
-        v = xb[(size_t)(c0 + ci) * a.T + ti];
-        if (x2b) v += x2b[(size_t)(c0 + ci) * a.T + ti];
-        if (a.act_in == 1) v = tanhf(v);
-      }
-      xs[e] = v;
-    }
-    const int wk = CI * a.k;
-#pragma unroll 4
-    for (int e = tid; e < CT * wk; e += 256) {
-      const int co = e / wk, r = e - co * wk, ci = r / a.k, j = r - ci * a.k;
-      float v = 0.f;
-      if (co0 + co < a.Cout && c0 + ci < a.Cin) v = a.w[((size_t)(co0 + co) * a.Cin + c0 + ci) * a.k + j];
-      ws[e] = v;
-    }
-    __syncthreads();
-    for (int ci = 0; ci < CI; ++ci) {
-      const float* xr = xs + ci * XW;
-      for (int j = 0; j < a.k; ++j) {
-        float wv[4], xv[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) wv[i] = ws[((ty * 4 + i) * CI + ci) * a.k + j];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) xv[i] = xr[tx + 16 * i + j * a.dil];
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-          for (int q = 0; q < 4; ++q) acc[i][q] = fmaf(wv[i], xv[q], acc[i][q]);
-      }
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int co = co0 + ty * 4 + i;
-    if (co >= a.Cout) continue;
-    const float bv = a.bias ? a.bias[co] : 0.f;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const int t = t0 + tx + 16 * q;
-      if (t >= a.T) continue;
-      float v = acc[i][q] + bv;
-      if (a.act_out == 1) v = fmaxf(v, 0.f);
-      else if (a.act_out == 2) v = 1.f / (1.f + expf(-v));
-      a.y[((size_t)b * a.yC + a.y_off + co) * a.T + t] = v;
-    }
-  }
-}
 
 // log-mel front end (:396-448): one block per (frame, batch row).  Reflect-pad (n_fft - hop)/2 both sides, Hann window,
 // |DFT| = sqrt(re^2 + im^2 + 1e-9) for bins 0..n_fft/2, mel projection with the librosa-style filterbank (host-computed,
@@ -220,32 +126,15 @@ __global__ void asp_pool_kernel(const float* __restrict__ x, const float* __rest
   if (lane == 0) { pooled[(size_t)b * 2 * C + c] = mean; pooled[(size_t)b * 2 * C + C + c] = sd; }
 }
 
-struct DevT {
-  float* p = nullptr;
-  int64_t numel = 0;
-};
-
 }  // namespace
 
 struct q3_spk {
   q3_spk_cfg cfg;
-  std::map<std::string, DevT> t;
-  std::vector<void*> allocs;
+  DevStore store{"speaker encoder"};
   float* ws = nullptr;
   size_t ws_elems = 0;
   bool finalized = false;
   int launches = 0;
-
-  int alloc_bytes(void** p, size_t bytes) {
-    cudaError_t e = cudaMalloc(p, bytes);
-    if (e != cudaSuccess) return q3_set_err("cudaMalloc(%zu B) failed: %s", bytes, cudaGetErrorString(e));
-    allocs.push_back(*p);
-    return 0;
-  }
-  const DevT* get(const std::string& n) const {
-    auto it = t.find(n);
-    return it == t.end() ? nullptr : &it->second;
-  }
 };
 
 extern "C" int q3_spk_create(const q3_spk_cfg* cfg, q3_spk** out) {
@@ -265,45 +154,29 @@ extern "C" int q3_spk_create(const q3_spk_cfg* cfg, q3_spk** out) {
     cat += cfg->channels[i];
   }
   Q3_REQUIRE(cat == cfg->channels[cfg->n_blocks - 1], "enc_channels[-1] must equal the sum of the SE-Res2Net block widths");
+  if (conv_f32_init()) return 1;
+  Q3_CUDA(cudaFuncSetAttribute(melspec_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
   q3_spk* e = new q3_spk();
   e->cfg = *cfg;
-  Q3_CUDA(cudaFuncSetAttribute(sconv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-  Q3_CUDA(cudaFuncSetAttribute(melspec_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
   *out = e;
   return 0;
 }
 
-extern "C" void q3_spk_destroy(q3_spk* e) {
-  if (!e) return;
-  for (void* p : e->allocs) cudaFree(p);
-  delete e;
-}
+extern "C" void q3_spk_destroy(q3_spk* e) { delete e; }
 
 extern "C" int q3_spk_load_tensor(q3_spk* e, const char* name, const float* dev, const int64_t* shape, int32_t ndim) {
   Q3_REQUIRE(e && name && dev && shape, "null argument");
   Q3_CUDA(cudaSetDevice(e->cfg.device));
-  int64_t n = 1;
-  for (int i = 0; i < ndim; ++i) n *= shape[i];
-  DevT d;
-  d.numel = n;
-  void* p = nullptr;
-  if (e->alloc_bytes(&p, ((size_t)n * 4 + 255) & ~(size_t)255)) return 1;
-  d.p = reinterpret_cast<float*>(p);
-  Q3_CUDA(cudaMemcpy(d.p, dev, (size_t)n * 4, cudaMemcpyDeviceToDevice));
-  e->t[name] = d;
-  return 0;
+  return e->store.load(name, dev, shape, ndim, DT_F32);
 }
 
 extern "C" int q3_spk_finalize(q3_spk* e) {
   Q3_REQUIRE(e, "null speaker encoder");
   const q3_spk_cfg& g = e->cfg;
-  const char* names[] = {"mel.window", "mel.cos", "mel.sin"};
-  for (const char* n : names) {
-    const DevT* t = e->get(n);
-    Q3_REQUIRE(t && t->numel == g.n_fft, "speaker encoder: missing/ill-shaped tensor %s", n);
-  }
-  const DevT* fb = e->get("mel.fbT");
-  Q3_REQUIRE(fb && fb->numel == (int64_t)(g.n_fft / 2 + 1) * g.mel_dim, "speaker encoder: missing/ill-shaped tensor mel.fbT");
+  const DevStore& S = e->store;
+  if (!S.need<float>("mel.window", g.n_fft) || !S.need<float>("mel.cos", g.n_fft) || !S.need<float>("mel.sin", g.n_fft) ||
+      !S.need<float>("mel.fbT", (int64_t)(g.n_fft / 2 + 1) * g.mel_dim))
+    return 1;
   e->finalized = true;
   return 0;
 }
@@ -323,20 +196,17 @@ struct SpkRunner {
   int B, T;
 
   int conv(const std::string& name, const float* x, int xC, int x_off, const float* x2, int x2C, int x2_off, float* y, int yC,
-           int y_off, int Cin, int Cout, int k, int dil, int act_in, int act_out, int T_) {
-    const DevT *w = e->get(name + ".weight"), *b = e->get(name + ".bias");
-    Q3_REQUIRE(w && b, "speaker encoder: missing tensor %s.weight/.bias", name.c_str());
-    Q3_REQUIRE(w->numel == (int64_t)Cout * Cin * k && b->numel == Cout, "speaker encoder: tensor %s has the wrong shape", name.c_str());
+           int y_off, int Cin, int Cout, int k, int dil, ConvActIn act_in, ConvActOut act_out, int T_) {
+    ConvF32Args a{};
+    if (!(a.w = e->store.need<float>(name + ".weight", (int64_t)Cout * Cin * k)) || !(a.bias = e->store.need<float>(name + ".bias", Cout)))
+      return 1;
     Q3_REQUIRE(dil * (k - 1) / 2 < T_ || k == 1, "input too short (%d frames) for reflect padding of %s", T_, name.c_str());
-    SConv a{};
-    a.x = x; a.x2 = x2; a.w = w->p; a.bias = b->p; a.y = y;
+    // nn.Conv1d(padding="same", padding_mode="reflect"): total pad dil*(k-1), left = total / 2
+    a.x = x; a.x2 = x2; a.y = y;
     a.xC = xC; a.x_off = x_off; a.x2C = x2C; a.x2_off = x2_off; a.yC = yC; a.y_off = y_off;
-    a.Cin = Cin; a.Cout = Cout; a.T = T_; a.k = k; a.dil = dil; a.act_in = act_in; a.act_out = act_out;
-    const int XW = TT + (k - 1) * dil;
-    const size_t smem = (size_t)(CI * XW + CT * CI * k) * sizeof(float);
-    Q3_REQUIRE(smem <= 96 * 1024, "conv tile needs %zu B of shared memory", smem);
-    dim3 grid((T_ + TT - 1) / TT, (Cout + CT - 1) / CT, B);
-    sconv_kernel<<<grid, 256, smem, st>>>(a);
+    a.Cin = Cin; a.Cout = Cout; a.Tin = T_; a.Tout = T_; a.k = k; a.stride = 1; a.dil = dil; a.pad_left = dil * (k - 1) / 2;
+    a.pad = PAD_REFLECT; a.act_in = act_in; a.act_out = act_out;
+    if (conv_f32_launch(a, B, st)) return 1;
     ++e->launches;
     return 0;
   }
@@ -349,9 +219,12 @@ static int run_mel(q3_spk* e, const float* wav, int B, int T, float* mel, int fr
   const q3_spk_cfg& g = e->cfg;
   Q3_REQUIRE(frames >= 1, "waveform too short for one STFT frame");
   Q3_REQUIRE((g.n_fft - g.hop) / 2 < T, "waveform shorter than the reflect padding");
+  const DevStore& S = e->store;
+  const float *window = S.need<float>("mel.window", g.n_fft), *twc = S.need<float>("mel.cos", g.n_fft),
+              *tws = S.need<float>("mel.sin", g.n_fft), *fbT = S.need<float>("mel.fbT", (int64_t)(g.n_fft / 2 + 1) * g.mel_dim);
+  if (!window || !twc || !tws || !fbT) return 1;
   const size_t smem = (size_t)(3 * g.n_fft + g.n_fft / 2 + 1) * sizeof(float);
-  melspec_kernel<<<dim3(frames, B), 256, smem, st>>>(wav, T, e->get("mel.window")->p, e->get("mel.cos")->p, e->get("mel.sin")->p,
-                                                      e->get("mel.fbT")->p, mel, g.n_fft, g.hop, g.mel_dim, frames);
+  melspec_kernel<<<dim3(frames, B), 256, smem, st>>>(wav, T, window, twc, tws, fbT, mel, g.n_fft, g.hop, g.mel_dim, frames);
   ++e->launches;
   return 0;
 }
@@ -384,9 +257,8 @@ extern "C" int q3_spk_embed(q3_spk* e, const float* wav_dev, int32_t B, int32_t 
   const size_t small = (size_t)B * (C + g.se_channels + C + 2 * Ccat);
   const size_t need = nMel + nF0 + nCat + 3 * nC + nCat + 3 * nCat + nAH + nCat + small;
   if (need > e->ws_elems) {
-    void* p = nullptr;
-    if (e->alloc_bytes(&p, need * 4)) return 1;
-    e->ws = reinterpret_cast<float*>(p);
+    e->ws_elems = 0;
+    if (e->store.grow(&e->ws, need * 4, st)) return 1;
     e->ws_elems = need;
   }
   float* p = e->ws;
@@ -411,43 +283,43 @@ extern "C" int q3_spk_embed(q3_spk* e, const float* wav_dev, int32_t B, int32_t 
   }
   SpkRunner r{e, st, B, L};
   // blocks.0: TDNN(mel_dim -> C0, k0, d0)
-  if (r.conv("blocks.0.conv", mel, g.mel_dim, 0, nullptr, 0, 0, F0, C0, 0, g.mel_dim, C0, g.kernel_sizes[0], g.dilations[0], 0, 1, L)) return 1;
+  if (r.conv("blocks.0.conv", mel, g.mel_dim, 0, nullptr, 0, 0, F0, C0, 0, g.mel_dim, C0, g.kernel_sizes[0], g.dilations[0], IN_NONE, OUT_RELU, L)) return 1;
   // SE-Res2Net blocks (:253-297); block i reads its input from F0 (i == 1) or from CAT slice i-2 and writes CAT slice i-1
   for (int i = 1; i < nb - 1; ++i) {
     const std::string pfx = "blocks." + std::to_string(i);
     const float* xin = (i == 1) ? F0 : CAT;
     const int xinC = (i == 1) ? C0 : Ccat, xoff = (i == 1) ? 0 : (i - 2) * C;
-    if (r.conv(pfx + ".tdnn1.conv", xin, xinC, xoff, nullptr, 0, 0, H, C, 0, g.channels[i - 1], C, 1, 1, 0, 1, L)) return 1;
+    if (r.conv(pfx + ".tdnn1.conv", xin, xinC, xoff, nullptr, 0, 0, H, C, 0, g.channels[i - 1], C, 1, 1, IN_NONE, OUT_RELU, L)) return 1;
     // Res2Net (:114-126): chunk 0 passes through; chunk j = TDNN_j(chunk j [+ output j-1])
     copy_ch_kernel<<<dim3((L + 127) / 128, Cs, B), 128, 0, st>>>(H, C, 0, R, C, 0, L);
     ++e->launches;
     for (int j = 1; j < S; ++j) {
       const std::string bn = pfx + ".res2net_block.blocks." + std::to_string(j - 1) + ".conv";
-      if (r.conv(bn, H, C, j * Cs, j >= 2 ? R : nullptr, C, (j - 1) * Cs, R, C, j * Cs, Cs, Cs, g.kernel_sizes[i], g.dilations[i], 0, 1, L))
+      if (r.conv(bn, H, C, j * Cs, j >= 2 ? R : nullptr, C, (j - 1) * Cs, R, C, j * Cs, Cs, Cs, g.kernel_sizes[i], g.dilations[i], IN_NONE, OUT_RELU, L))
         return 1;
     }
-    if (r.conv(pfx + ".tdnn2.conv", R, C, 0, nullptr, 0, 0, H2, C, 0, C, C, 1, 1, 0, 1, L)) return 1;
+    if (r.conv(pfx + ".tdnn2.conv", R, C, 0, nullptr, 0, 0, H2, C, 0, C, C, 1, 1, IN_NONE, OUT_RELU, L)) return 1;
     // squeeze-excitation gate (:150-157) and the residual (:296-297)
     mean_t_kernel<<<dim3(C, B), 32, 0, st>>>(H2, C, 0, C, L, MEAN);
     ++e->launches;
     SpkRunner r1{e, st, B, 1};
-    if (r1.conv(pfx + ".se_block.conv1", MEAN, C, 0, nullptr, 0, 0, SE1, g.se_channels, 0, C, g.se_channels, 1, 1, 0, 1, 1)) return 1;
-    if (r1.conv(pfx + ".se_block.conv2", SE1, g.se_channels, 0, nullptr, 0, 0, GATE, C, 0, g.se_channels, C, 1, 1, 0, 2, 1)) return 1;
+    if (r1.conv(pfx + ".se_block.conv1", MEAN, C, 0, nullptr, 0, 0, SE1, g.se_channels, 0, C, g.se_channels, 1, 1, IN_NONE, OUT_RELU, 1)) return 1;
+    if (r1.conv(pfx + ".se_block.conv2", SE1, g.se_channels, 0, nullptr, 0, 0, GATE, C, 0, g.se_channels, C, 1, 1, IN_NONE, OUT_SIGMOID, 1)) return 1;
     se_apply_kernel<<<dim3((L + 127) / 128, C, B), 128, 0, st>>>(H2, GATE, xin, xinC, xoff, CAT, Ccat, (i - 1) * C, C, L);
     ++e->launches;
   }
   // multi-layer feature aggregation (:381-383) on the concatenation of the SE-Res2Net outputs
-  if (r.conv("mfa.conv", CAT, Ccat, 0, nullptr, 0, 0, M, Ccat, 0, Ccat, Ccat, g.kernel_sizes[nb - 1], g.dilations[nb - 1], 0, 1, L)) return 1;
+  if (r.conv("mfa.conv", CAT, Ccat, 0, nullptr, 0, 0, M, Ccat, 0, Ccat, Ccat, g.kernel_sizes[nb - 1], g.dilations[nb - 1], IN_NONE, OUT_RELU, L)) return 1;
   // attentive statistics pooling (:203-226)
   asp_cat_kernel<<<dim3(Ccat, B), 32, 0, st>>>(M, ACAT, Ccat, L, 1e-12f);
   ++e->launches;
-  if (r.conv("asp.tdnn.conv", ACAT, 3 * Ccat, 0, nullptr, 0, 0, AH, g.attention_channels, 0, 3 * Ccat, g.attention_channels, 1, 1, 0, 1, L)) return 1;
-  if (r.conv("asp.conv", AH, g.attention_channels, 0, nullptr, 0, 0, ATT, Ccat, 0, g.attention_channels, Ccat, 1, 1, 1, 0, L)) return 1;
+  if (r.conv("asp.tdnn.conv", ACAT, 3 * Ccat, 0, nullptr, 0, 0, AH, g.attention_channels, 0, 3 * Ccat, g.attention_channels, 1, 1, IN_NONE, OUT_RELU, L)) return 1;
+  if (r.conv("asp.conv", AH, g.attention_channels, 0, nullptr, 0, 0, ATT, Ccat, 0, g.attention_channels, Ccat, 1, 1, IN_TANH, OUT_NONE, L)) return 1;
   asp_pool_kernel<<<dim3(Ccat, B), 32, 0, st>>>(M, ATT, POOL, Ccat, L, 1e-12f);
   ++e->launches;
   // final 1x1 conv (:384-393)
   SpkRunner r1{e, st, B, 1};
-  if (r1.conv("fc", POOL, 2 * Ccat, 0, nullptr, 0, 0, emb_dev, g.enc_dim, 0, 2 * Ccat, g.enc_dim, 1, 1, 0, 0, 1)) return 1;
+  if (r1.conv("fc", POOL, 2 * Ccat, 0, nullptr, 0, 0, emb_dev, g.enc_dim, 0, 2 * Ccat, g.enc_dim, 1, 1, IN_NONE, OUT_NONE, 1)) return 1;
   Q3_CUDA(cudaGetLastError());
   return 0;
 }
