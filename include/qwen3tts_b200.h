@@ -21,6 +21,8 @@
  *     The engine owns only what it allocates itself (packed weights, KV cache, workspaces).
  *   - `stream` is a cudaStream_t passed as void* (torch.cuda.current_stream().cuda_stream); work is
  *     enqueued on it, calls do not synchronise unless documented.  One engine = one device, not re-entrant.
+ *     Apart from the debug and hidden-capture buffers, which must stay valid until cleared, the engine reads caller
+ *     memory only in work it queues on `stream` during the call.
  *   - bf16 tensors are raw uint16 storage (torch.bfloat16).  No torch types cross this boundary.
  */
 #ifndef QWEN3TTS_B200_H
@@ -88,7 +90,7 @@ void q3_engine_destroy(q3_engine* e);
  *   "talker.norm", "talker.codec_head", "talker.codec_embedding", "talker.rope_cos", "talker.rope_sin"
  *   "cp.layers.<i>.*", "cp.norm", "cp.proj", "cp.proj_bias", "cp.lm_head.<j>", "cp.codec_embedding.<j>",
  *   "cp.rope_cos", "cp.rope_sin".
- * The source may be freed after the call returns (the call synchronises the copy stream). */
+ * The source may be freed after the call returns (the copy is complete by then). */
 int q3_engine_load_tensor(q3_engine* e, const char* name, const void* dev_bf16, int64_t rows, int64_t cols);
 int q3_engine_finalize(q3_engine* e); /* verifies that every tensor is present */
 

@@ -18,6 +18,7 @@
 //   * rounding points mirror the PyTorch bf16 path (linear outputs, RMSNorm, RoPE, residual adds are
 //     rounded to bf16 exactly where the reference rounds).
 #include "common.cuh"
+#include "dev_store.h"
 #include "gemm_sm90.cuh"
 #include "../../include/qwen3tts_b200.h"
 
@@ -26,6 +27,7 @@
 #include <algorithm>
 #include <cmath>
 #include <map>
+#include <memory>
 #include <vector>
 
 thread_local std::string g_q3_err;
@@ -180,6 +182,12 @@ __global__ void __launch_bounds__(CTA_THREADS, 1) q3_step_kernel(const __grid_co
   if (P.mode == 1 && blockIdx.x == 0 && tid == 0) st->step = step_base + iters_done;
 }
 
+// every instantiation, by variant (rows) and batch class 1 / 2 / 4 (columns)
+const void* const kStepKernels[3][3] = {
+    {(const void*)q3_step_kernel<1, 0>, (const void*)q3_step_kernel<2, 0>, (const void*)q3_step_kernel<4, 0>},
+    {(const void*)q3_step_kernel<1, 1>, (const void*)q3_step_kernel<2, 1>, (const void*)q3_step_kernel<4, 1>},
+    {(const void*)q3_step_kernel<1, 2>, (const void*)q3_step_kernel<2, 2>, (const void*)q3_step_kernel<4, 2>}};
+
 }  // namespace
 
 #include "ar_prefill.cuh"
@@ -199,19 +207,27 @@ struct PieceTable {
   size_t n_runs = 0;
 };
 
+// the weights one talker layer of the prefill reads: its norms and the plain [N][K] copies of its GEMM weights
+struct PfLayer {
+  const bf16 *ln1, *ln2, *qn, *kn, *qkv, *o, *gate_up, *down;
+};
+
+constexpr char kEngineName[] = "AR engine";
+
 struct q3_engine {
   q3_engine_cfg cfg;
   int sm_count = 0;
   size_t l2_bytes = 0;
   cudaStream_t copy_stream = nullptr;
+  // every device block: norms, biases, embeddings, rope tables and the plain [N][K] copies of the talker layer weights
+  // for the wgmma prefill GEMMs as named tensors; the packed GEMV weights and the buffers below as blocks
+  DevStore store{kEngineName};
   std::map<std::string, PackedW> packed;   // GEMV weights
-  std::map<std::string, bf16*> gemm_w;      // plain [N][K] copies of the talker layer weights for the wgmma prefill GEMMs
+  std::vector<PfLayer> pf_layers;          // resolved at finalize
+  const bf16 *emb_t = nullptr, *emb_cp = nullptr;  // talker / code-predictor codec embeddings, resolved at finalize
   bf16 *pf_x = nullptr, *pf_xn = nullptr, *pf_qkv = nullptr, *pf_attn = nullptr, *pf_act = nullptr;
   int *pf_seq = nullptr, *pf_pos = nullptr;
   int pf_cap = 0;
-  std::map<std::string, bf16*> plain;      // norms, biases, embeddings, rope tables
-  std::map<std::string, std::pair<int64_t, int64_t>> plain_shape;
-  std::vector<void*> allocs;
   // device buffers
   DevState* st = nullptr;
   StackDev talker{}, cp{};
@@ -255,38 +271,25 @@ struct q3_engine {
   size_t smem_bytes = 0;
   double w_talker_bytes = 0, w_cp_unique_bytes = 0, w_cp_stream_bytes = 0;
 
-  template <typename T>
-  int alloc(T** p, size_t count) {
-    void* q = nullptr;
-    cudaError_t e = cudaMalloc(&q, count * sizeof(T));
-    if (e != cudaSuccess) return q3_set_err("cudaMalloc(%zu B) failed: %s", count * sizeof(T), cudaGetErrorString(e));
-    // zero-fill ordered against everything else this engine does: same stream as the pack / copy work, then wait
-    // (allocation is a load-time or growth-time event; nothing on the per-step path allocates)
-    cudaMemsetAsync(q, 0, count * sizeof(T), copy_stream);
-    cudaStreamSynchronize(copy_stream);
-    allocs.push_back(q);
-    *p = reinterpret_cast<T*>(q);
-    return 0;
-  }
-  void release(void* q) {
-    if (!q) return;
-    for (size_t i = 0; i < allocs.size(); ++i)
-      if (allocs[i] == q) { allocs.erase(allocs.begin() + i); break; }
-    cudaFree(q);
+  ~q3_engine() {
+    if (copy_stream) cudaStreamDestroy(copy_stream);
   }
 };
 
+// the engine's own blocks are zero-filled (allocation is a load-time or growth-time event; nothing on the per-step
+// path allocates)
 static int stack_alloc(q3_engine* e, StackDev& S, const q3_stack_cfg& c, int nseq, int cap, int cols) {
   S.hidden = c.hidden_size; S.layers = c.num_layers; S.nh = c.num_heads; S.nkv = c.num_kv_heads;
   S.inter = c.intermediate_size; S.vocab = c.vocab_size; S.eps = c.rms_eps; S.cap = cap;
-  if (e->alloc(&S.h, (size_t)cols * c.hidden_size)) return 1;
-  if (e->alloc(&S.qkv, (size_t)cols * (c.num_heads + 2 * c.num_kv_heads) * HD)) return 1;
-  if (e->alloc(&S.attn, (size_t)cols * c.num_heads * HD)) return 1;
-  if (e->alloc(&S.act, (size_t)cols * c.intermediate_size)) return 1;
+  DevStore& store = e->store;
+  if (store.alloc(&S.h, (size_t)cols * c.hidden_size, true)) return 1;
+  if (store.alloc(&S.qkv, (size_t)cols * (c.num_heads + 2 * c.num_kv_heads) * HD, true)) return 1;
+  if (store.alloc(&S.attn, (size_t)cols * c.num_heads * HD, true)) return 1;
+  if (store.alloc(&S.act, (size_t)cols * c.intermediate_size, true)) return 1;
   const size_t kv = (size_t)nseq * c.num_layers * c.num_kv_heads * cap * HD;
-  if (e->alloc(&S.kc, kv)) return 1;
-  if (e->alloc(&S.vc, kv)) return 1;
-  if (e->alloc(&S.logits, (size_t)MAXB * c.vocab_size)) return 1;
+  if (store.alloc(&S.kc, kv, true)) return 1;
+  if (store.alloc(&S.vc, kv, true)) return 1;
+  if (store.alloc(&S.logits, (size_t)MAXB * c.vocab_size, true)) return 1;
   return 0;
 }
 
@@ -313,34 +316,30 @@ extern "C" int q3_engine_create(const q3_engine_cfg* cfg, q3_engine** out) {
   cudaDeviceProp prop;
   Q3_CUDA(cudaGetDeviceProperties(&prop, cfg->device));
   Q3_REQUIRE(prop.major == 9 && prop.minor == 0, "this library is built for sm_90a (H100); device is sm_%d%d", prop.major, prop.minor);
-  q3_engine* e = new q3_engine();
+  std::unique_ptr<q3_engine> e(new q3_engine());  // deleted on every failure below
   e->cfg = *cfg;
   e->sm_count = prop.multiProcessorCount;
   e->l2_bytes = (size_t)prop.l2CacheSize;
   Q3_CUDA(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
   if (gemm_init()) return 1;
-  if (e->alloc(&e->st, 1)) return 1;
-  if (stack_alloc(e, e->talker, cfg->talker, cfg->max_batch, cfg->max_ctx, MAXCOLS)) return 1;
-  if (stack_alloc(e, e->cp, cfg->cp, cfg->max_batch, 32, MAXCOLS)) return 1;
+  DevStore& store = e->store;
+  if (store.alloc(&e->st, 1, true)) return 1;
+  if (stack_alloc(e.get(), e->talker, cfg->talker, cfg->max_batch, cfg->max_ctx, MAXCOLS)) return 1;
+  if (stack_alloc(e.get(), e->cp, cfg->cp, cfg->max_batch, 32, MAXCOLS)) return 1;
   const int H = cfg->talker.hidden_size;
-  if (e->alloc(&e->x_cp, (size_t)2 * MAXB * H)) return 1;
-  if (e->alloc(&e->past_hidden, (size_t)MAXB * H)) return 1;
-  if (e->alloc(&e->h_last, (size_t)MAXB * H)) return 1;
-  if (e->alloc(&e->tts_pad, (size_t)H)) return 1;
-  if (e->alloc(&e->seen, (size_t)MAXB * cfg->talker.vocab_size)) return 1;
-  if (e->alloc(&e->split_buf, (size_t)MAXB * cfg->talker.num_kv_heads * MAXSPLIT * RMAX * 130)) return 1;
+  if (store.alloc(&e->x_cp, (size_t)2 * MAXB * H, true)) return 1;
+  if (store.alloc(&e->past_hidden, (size_t)MAXB * H, true)) return 1;
+  if (store.alloc(&e->h_last, (size_t)MAXB * H, true)) return 1;
+  if (store.alloc(&e->tts_pad, (size_t)H, true)) return 1;
+  if (store.alloc(&e->seen, (size_t)MAXB * cfg->talker.vocab_size, true)) return 1;
+  if (store.alloc(&e->split_buf, (size_t)MAXB * cfg->talker.num_kv_heads * MAXSPLIT * RMAX * 130, true)) return 1;
   static_assert(SAMPLER_SMEM <= X_MIN_BYTES && ATT_SMEM <= X_MIN_BYTES, "attention / sampler scratch must fit the x area");
   Q3_REQUIRE((size_t)SMEM_OPTIN <= (size_t)prop.sharedMemPerBlockOptin, "not enough shared memory per block");
-  *out = e;
+  *out = e.release();
   return 0;
 }
 
-extern "C" void q3_engine_destroy(q3_engine* e) {
-  if (!e) return;
-  for (void* p : e->allocs) cudaFree(p);
-  if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
-  delete e;
-}
+extern "C" void q3_engine_destroy(q3_engine* e) { delete e; }
 
 static bool is_gemv_weight(const std::string& n) {
   auto ends = [&](const char* s) { size_t l = strlen(s); return n.size() >= l && n.compare(n.size() - l, l, s) == 0; };
@@ -353,53 +352,33 @@ static bool is_gemv_weight(const std::string& n) {
 extern "C" int q3_engine_load_tensor(q3_engine* e, const char* name, const void* dev, int64_t rows, int64_t cols) {
   Q3_REQUIRE(e && name && dev, "null argument");
   Q3_CUDA(cudaSetDevice(e->cfg.device));
+  const std::string n(name);
+  const int64_t shape[2] = {rows, cols};
+  if (!is_gemv_weight(n)) return e->store.load(n, dev, shape, 2, DT_BF16);
+  Q3_REQUIRE(rows % 16 == 0 && cols % 32 == 0, "%s: GEMV weight must be [16a][32b], got [%lld][%lld]", name,
+             (long long)rows, (long long)cols);
   // `dev` may still be being produced on the caller's stream (a cat / cast queued by the framework): the ABI has
   // no stream argument here, so wait for the device once per tensor — a load-time cost only
   Q3_CUDA(cudaDeviceSynchronize());
-  std::string n(name);
-  if (is_gemv_weight(n)) {
-    Q3_REQUIRE(rows % 16 == 0 && cols % 32 == 0, "%s: GEMV weight must be [16a][32b], got [%lld][%lld]", name,
-               (long long)rows, (long long)cols);
-    PackedW pw;
-    pw.n = (int)rows; pw.k = (int)cols;
-    if (e->alloc(&pw.w, (size_t)rows * cols / 8)) return 1;
-    pack_weight_kernel<<<1024, 256, 0, e->copy_stream>>>(reinterpret_cast<const bf16*>(dev), pw.w, (int)rows, (int)cols);
-    Q3_CUDA(cudaGetLastError());
-    Q3_CUDA(cudaStreamSynchronize(e->copy_stream));
-    e->packed[n] = pw;
-    if (n.rfind("talker.layers.", 0) == 0 || (n == "cp.proj" && cols % 64 == 0)) {  // wgmma GEMM operand: [N][K] is already K-major
-      Q3_REQUIRE(cols % 64 == 0, "%s: K must be a multiple of 64 for the prefill GEMM", name);
-      bf16* g = nullptr;
-      if (e->alloc(&g, (size_t)rows * cols)) return 1;
-      Q3_CUDA(cudaMemcpyAsync(g, dev, (size_t)rows * cols * sizeof(bf16), cudaMemcpyDeviceToDevice, e->copy_stream));
-      Q3_CUDA(cudaStreamSynchronize(e->copy_stream));
-      e->gemm_w[n] = g;
-    }
-  } else {
-    bf16* p = nullptr;
-    if (e->alloc(&p, (size_t)rows * cols)) return 1;
-    Q3_CUDA(cudaMemcpyAsync(p, dev, (size_t)rows * cols * sizeof(bf16), cudaMemcpyDeviceToDevice, e->copy_stream));
-    Q3_CUDA(cudaStreamSynchronize(e->copy_stream));
-    e->plain[n] = p;
-    e->plain_shape[n] = {rows, cols};
+  PackedW pw;
+  pw.n = (int)rows; pw.k = (int)cols;
+  if (e->store.alloc(&pw.w, (size_t)rows * cols / 8, false)) return 1;  // the pack kernel writes every element
+  pack_weight_kernel<<<1024, 256, 0, e->copy_stream>>>(reinterpret_cast<const bf16*>(dev), pw.w, (int)rows, (int)cols);
+  Q3_CUDA(cudaGetLastError());
+  Q3_CUDA(cudaStreamSynchronize(e->copy_stream));
+  e->packed[n] = pw;
+  if (n.rfind("talker.layers.", 0) == 0 || (n == "cp.proj" && cols % 64 == 0)) {  // wgmma GEMM operand: [N][K] is already K-major
+    Q3_REQUIRE(cols % 64 == 0, "%s: K must be a multiple of 64 for the prefill GEMM", name);
+    return e->store.load(n, dev, shape, 2, DT_BF16);
   }
   return 0;
 }
 
 static int need_packed(q3_engine* e, const std::string& n, int rows, int cols, PackedW* out) {
   auto it = e->packed.find(n);
-  Q3_REQUIRE(it != e->packed.end(), "missing tensor %s", n.c_str());
-  Q3_REQUIRE(it->second.n == rows && it->second.k == cols, "tensor %s has shape [%d][%d], expected [%d][%d]", n.c_str(),
-             it->second.n, it->second.k, rows, cols);
-  *out = it->second;
-  return 0;
-}
-static int need_plain(q3_engine* e, const std::string& n, int64_t count, const bf16** out) {
-  auto it = e->plain.find(n);
-  Q3_REQUIRE(it != e->plain.end(), "missing tensor %s", n.c_str());
-  auto sh = e->plain_shape[n];
-  Q3_REQUIRE(sh.first * sh.second == count, "tensor %s has %lld elements, expected %lld", n.c_str(),
-             (long long)(sh.first * sh.second), (long long)count);
+  Q3_REQUIRE(it != e->packed.end(), "%s: tensor %s is missing, expected shape [%d][%d]", kEngineName, n.c_str(), rows, cols);
+  Q3_REQUIRE(it->second.n == rows && it->second.k == cols, "%s: tensor %s has shape [%d][%d], expected [%d][%d]", kEngineName,
+             n.c_str(), it->second.n, it->second.k, rows, cols);
   *out = it->second;
   return 0;
 }
@@ -424,8 +403,8 @@ static int add_layers(q3_engine* e, std::vector<Phase>& prog, const char* pfx, S
     const bf16 *ln1, *ln2, *qn, *kn;
     if (need_packed(e, p + ".qkv", QKV, Hh, &wqkv) || need_packed(e, p + ".o", Hh, S.nh * HD, &wo) ||
         need_packed(e, p + ".gate_up", 2 * S.inter, Hh, &wgu) || need_packed(e, p + ".down", Hh, S.inter, &wd) ||
-        need_plain(e, p + ".ln1", Hh, &ln1) || need_plain(e, p + ".ln2", Hh, &ln2) ||
-        need_plain(e, p + ".q_norm", HD, &qn) || need_plain(e, p + ".k_norm", HD, &kn))
+        !(ln1 = e->store.need<bf16>(p + ".ln1", Hh)) || !(ln2 = e->store.need<bf16>(p + ".ln2", Hh)) ||
+        !(qn = e->store.need<bf16>(p + ".q_norm", HD)) || !(kn = e->store.need<bf16>(p + ".k_norm", HD)))
       return 1;
     prog.push_back(gemv(wqkv, hbuf, Hh, ln1, S.eps, S.qkv, QKV, EPI_STORE, ncmode));
     Phase a{};
@@ -478,10 +457,10 @@ static int build_piece_table(q3_engine* e, const std::vector<Phase>& prog, Piece
     }
   }
   off.push_back((uint32_t)pieces.size());
-  e->release(out->runs);
-  e->release(out->off);
-  out->runs = nullptr; out->off = nullptr;
-  if (e->alloc(&out->runs, pieces.size() + 8) || e->alloc(&out->off, off.size())) return 1;
+  // the caller has drained the device: no launch still reads the old tables
+  if (e->store.grow(&out->runs, (pieces.size() + 8) * sizeof(uint2), e->copy_stream, true) ||
+      e->store.grow(&out->off, off.size() * sizeof(uint32_t), e->copy_stream, true))
+    return 1;
   out->n_runs = pieces.size();
   Q3_CUDA(cudaMemcpy(out->runs, pieces.data(), pieces.size() * sizeof(uint2), cudaMemcpyHostToDevice));
   Q3_CUDA(cudaMemcpy(out->off, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
@@ -537,13 +516,13 @@ static int build_programs(q3_engine* e, int B) {
   const int H = T.hidden, Hc = C.hidden, G = c.num_code_groups;
   const bf16 *tnorm, *cnorm;
   PackedW whead;
-  if (need_plain(e, "talker.norm", H, &tnorm) || need_plain(e, "cp.norm", Hc, &cnorm) ||
+  if (!(tnorm = e->store.need<bf16>("talker.norm", H)) || !(cnorm = e->store.need<bf16>("cp.norm", Hc)) ||
       need_packed(e, "talker.codec_head", T.vocab, H, &whead))
     return 1;
   PackedW wproj{};
   const bf16* bproj = nullptr;
   if (c.has_cp_projection) {
-    if (need_packed(e, "cp.proj", Hc, H, &wproj) || need_plain(e, "cp.proj_bias", Hc, &bproj)) return 1;
+    if (need_packed(e, "cp.proj", Hc, H, &wproj) || !(bproj = e->store.need<bf16>("cp.proj_bias", Hc))) return 1;
   }
   // ---- prefill-head program: final norm + codec_head on the last token of each row, sample frame-0 codebook-0
   e->prog_head.clear();
@@ -609,15 +588,14 @@ static int build_programs(q3_engine* e, int B) {
   if (make_smem_plan(e, e->prog_head, B, e->nt_head, &e->plan_head) || make_smem_plan(e, e->prog_frame, B, e->nt_frame, &e->plan_frame))
     return 1;
   Q3_REQUIRE((int)F.size() <= MAX_PHASES, "frame program has %d phases (max %d)", (int)F.size(), MAX_PHASES);
+  // launches may still walk the old program and its piece tables: wait for them before replacing either (a batch-size
+  // change is rare)
+  Q3_CUDA(cudaDeviceSynchronize());
   if (build_piece_table(e, e->prog_head, &e->pt_head) || build_piece_table(e, e->prog_frame, &e->pt_frame, e->cp_phases))
     return 1;
-  // upload (a batch-size change is rare: wait for launches that may still walk the old program)
-  Q3_CUDA(cudaDeviceSynchronize());
   const size_t total = e->prog_head.size() + F.size();
   if ((int)total > e->prog_cap) {
-    e->release(e->prog_dev);
-    e->prog_dev = nullptr;
-    if (e->alloc(&e->prog_dev, total + 64)) return 1;
+    if (e->store.grow(&e->prog_dev, (total + 64) * sizeof(Phase), e->copy_stream, true)) return 1;
     e->prog_cap = (int)total + 64;
   }
   e->off_head = 0;
@@ -631,36 +609,43 @@ static int build_programs(q3_engine* e, int B) {
 extern "C" int q3_engine_finalize(q3_engine* e) {
   Q3_REQUIRE(e, "null engine");
   Q3_CUDA(cudaSetDevice(e->cfg.device));
-  const bf16* p;
   const q3_engine_cfg& c = e->cfg;
-  if (need_plain(e, "talker.codec_embedding", (int64_t)c.talker.vocab_size * c.talker.hidden_size, &p)) return 1;
-  if (need_plain(e, "talker.rope_cos", (int64_t)c.max_ctx * 64, &p)) return 1;
-  e->talker.rope_cos = p;
-  if (need_plain(e, "talker.rope_sin", (int64_t)c.max_ctx * 64, &p)) return 1;
-  e->talker.rope_sin = p;
-  if (need_plain(e, "cp.rope_cos", (int64_t)32 * 64, &p)) return 1;
-  e->cp.rope_cos = p;
-  if (need_plain(e, "cp.rope_sin", (int64_t)32 * 64, &p)) return 1;
-  e->cp.rope_sin = p;
-  if (need_plain(e, "cp.codec_embedding",
-                 (int64_t)(c.num_code_groups - 1) * c.cp.vocab_size * c.talker.hidden_size, &p))
+  const DevStore& S = e->store;
+  const q3_stack_cfg& tc = c.talker;
+  if (!(e->emb_t = S.need<bf16>("talker.codec_embedding", (int64_t)tc.vocab_size * tc.hidden_size)) ||
+      !(e->talker.rope_cos = S.need<bf16>("talker.rope_cos", (int64_t)c.max_ctx * 64)) ||
+      !(e->talker.rope_sin = S.need<bf16>("talker.rope_sin", (int64_t)c.max_ctx * 64)) ||
+      !(e->cp.rope_cos = S.need<bf16>("cp.rope_cos", (int64_t)32 * 64)) ||
+      !(e->cp.rope_sin = S.need<bf16>("cp.rope_sin", (int64_t)32 * 64)) ||
+      !(e->emb_cp = S.need<bf16>("cp.codec_embedding", (int64_t)(c.num_code_groups - 1) * c.cp.vocab_size * tc.hidden_size)))
     return 1;
+  const int64_t H = tc.hidden_size, A = (int64_t)tc.num_heads * HD, QKV = A + 2LL * tc.num_kv_heads * HD, I = tc.intermediate_size;
+  e->pf_layers.resize(tc.num_layers);
+  for (int l = 0; l < tc.num_layers; ++l) {
+    const std::string p = "talker.layers." + std::to_string(l);
+    PfLayer& L = e->pf_layers[l];
+    if (!(L.ln1 = S.need<bf16>(p + ".ln1", H)) || !(L.ln2 = S.need<bf16>(p + ".ln2", H)) ||
+        !(L.qn = S.need<bf16>(p + ".q_norm", HD)) || !(L.kn = S.need<bf16>(p + ".k_norm", HD)) ||
+        !(L.qkv = S.need<bf16>(p + ".qkv", QKV * H)) || !(L.o = S.need<bf16>(p + ".o", H * A)) ||
+        !(L.gate_up = S.need<bf16>(p + ".gate_up", 2 * I * H)) || !(L.down = S.need<bf16>(p + ".down", H * I)))
+      return 1;
+  }
   // projection table: passes >= 1 of the code predictor feed small_to_mtp_projection(codec_embedding[j-1](c_j)) (:1281-1283),
   // a function of the sampled id only -> one wgmma GEMM over all (G-1)*Vc embedding rows here, no GEMV phase per pass
   // (without a GEMM copy of cp.proj, i.e. a talker hidden size that is not a multiple of 64, each pass keeps its projection GEMV)
-  if (c.has_cp_projection && e->gemm_w.count("cp.proj") && !e->proj_tab) {
-    const int H = c.talker.hidden_size, Hc = c.cp.hidden_size;
+  if (c.has_cp_projection && H % 64 == 0 && !e->proj_tab) {
+    const int Hc = c.cp.hidden_size;
     const int rows = (c.num_code_groups - 1) * c.cp.vocab_size;
-    const bf16* bproj;
-    if (need_plain(e, "cp.proj_bias", Hc, &bproj)) return 1;
+    const bf16 *bproj, *wproj;
+    if (!(bproj = S.need<bf16>("cp.proj_bias", Hc)) || !(wproj = S.need<bf16>("cp.proj", (int64_t)Hc * H))) return 1;
     float* bias_f = nullptr;
-    if (e->alloc(&bias_f, (size_t)Hc) || e->alloc(&e->proj_tab, (size_t)rows * Hc)) return 1;
+    if (e->store.alloc(&bias_f, (size_t)Hc, true) || e->store.alloc(&e->proj_tab, (size_t)rows * Hc, true)) return 1;
     bf16_to_f32_kernel<<<(Hc + 255) / 256, 256, 0, e->copy_stream>>>(bproj, bias_f, Hc);
     GemmEpilogue ep{};
     ep.bias = bias_f; ep.cmod = Hc; ep.out_raw = e->proj_tab;
     GemmPlan plan;
     const int zero = 0;
-    if (gemm_make_plan(&plan, p, 1, rows, H, H, (int64_t)rows * H, e->gemm_w["cp.proj"], Hc, H, 1, &zero,
+    if (gemm_make_plan(&plan, e->emb_cp, 1, rows, H, H, (int64_t)rows * H, wproj, Hc, H, 1, &zero,
                        gemm_pick_bn(Hc, (rows + 127) / 128, 1), ep))
       return 1;
     if (gemm_launch(plan, e->copy_stream)) return 1;
@@ -669,16 +654,15 @@ extern "C" int q3_engine_finalize(q3_engine* e) {
   // kernel attributes: all opt-in shared memory minus the kernel's static part is the dynamic budget of the plans
   {
     int stat = 0;
-    const void* fns[] = {(const void*)q3_step_kernel<1, 0>, (const void*)q3_step_kernel<2, 0>, (const void*)q3_step_kernel<4, 0>,
-                         (const void*)q3_step_kernel<1, 1>, (const void*)q3_step_kernel<2, 1>, (const void*)q3_step_kernel<4, 1>,
-                         (const void*)q3_step_kernel<1, 2>, (const void*)q3_step_kernel<2, 2>, (const void*)q3_step_kernel<4, 2>};
-    for (const void* fn : fns) {
-      cudaFuncAttributes fa;
-      Q3_CUDA(cudaFuncGetAttributes(&fa, fn));
-      stat = std::max(stat, (int)fa.sharedSizeBytes);
-    }
+    for (const auto& row : kStepKernels)
+      for (const void* fn : row) {
+        cudaFuncAttributes fa;
+        Q3_CUDA(cudaFuncGetAttributes(&fa, fn));
+        stat = std::max(stat, (int)fa.sharedSizeBytes);
+      }
     e->max_dyn_smem = SMEM_OPTIN - (stat + 127) / 128 * 128;
-    for (const void* fn : fns) Q3_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, e->max_dyn_smem));
+    for (const auto& row : kStepKernels)
+      for (const void* fn : row) Q3_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, e->max_dyn_smem));
   }
   {  // weight arena base for the 32-bit (x16 B) offsets of the phase metas
     const char *lo = nullptr, *hi = nullptr;
@@ -728,7 +712,7 @@ static int launch_program(q3_engine* e, int off, int n, int mode, int max_iters,
   P.max_len0 = e->max_len0;
   for (int b = 0; b < MAXB; ++b) { P.frame0[b] = e->frame0[b]; P.row_key[b] = e->row_key[b]; }
   P.admit_mask = e->admit_mask;
-  P.emb_t = e->plain["talker.codec_embedding"]; P.emb_cp = e->plain["cp.codec_embedding"];
+  P.emb_t = e->emb_t; P.emb_cp = e->emb_cp;
   P.x_cp = e->cfg.has_cp_projection ? e->x_cp : e->cp.h; P.past_hidden = e->past_hidden; P.trailing = e->trailing; P.trailing_stride = e->trailing_cap;
   if (e->proj_tab) { P.cp_next = e->proj_tab; P.cp_next_dst = e->cp.h; P.cp_next_w = e->cfg.cp.hidden_size; }
   else { P.cp_next = P.emb_cp; P.cp_next_dst = P.x_cp; P.cp_next_w = e->cfg.talker.hidden_size; }
@@ -742,11 +726,7 @@ static int launch_program(q3_engine* e, int off, int n, int mode, int max_iters,
   Q3_CUDA(cudaMemsetAsync(&e->st->bar_count, 0, sizeof(unsigned int), stream));
   void* args[] = {&P};
   const int var = P.prof ? 2 : P.hid_out ? 1 : 0;
-  static const void* const kfn[3][3] = {
-      {(const void*)q3_step_kernel<1, 0>, (const void*)q3_step_kernel<2, 0>, (const void*)q3_step_kernel<4, 0>},
-      {(const void*)q3_step_kernel<1, 1>, (const void*)q3_step_kernel<2, 1>, (const void*)q3_step_kernel<4, 1>},
-      {(const void*)q3_step_kernel<1, 2>, (const void*)q3_step_kernel<2, 2>, (const void*)q3_step_kernel<4, 2>}};
-  const void* fn = kfn[var][nt == 1 ? 0 : nt == 2 ? 1 : 2];
+  const void* fn = kStepKernels[var][nt == 1 ? 0 : nt == 2 ? 1 : 2];
   Q3_CUDA(cudaLaunchCooperativeKernel(fn, dim3(e->sm_count), dim3(CTA_THREADS), args, (size_t)plan.total, stream));
   return 0;
 }
@@ -786,44 +766,41 @@ static int prefill_rows(q3_engine* e, const Admission& A, unsigned int mask, cud
   const q3_stack_cfg& tc = e->cfg.talker;
   const int nh = tc.num_heads, nkv = tc.num_kv_heads, I = tc.intermediate_size, QKV = (nh + 2 * nkv) * HD;
   if (ntok > e->pf_cap) {
-    const int cap = std::max(ntok + ntok / 4, 1024);
-    Q3_CUDA(cudaStreamSynchronize(stream));  // growth only
-    for (void* q : {(void*)e->pf_x, (void*)e->pf_xn, (void*)e->pf_qkv, (void*)e->pf_attn, (void*)e->pf_act, (void*)e->pf_seq, (void*)e->pf_pos})
-      e->release(q);
-    if (e->alloc(&e->pf_x, (size_t)cap * H) || e->alloc(&e->pf_xn, (size_t)cap * H) || e->alloc(&e->pf_qkv, (size_t)cap * QKV) ||
-        e->alloc(&e->pf_attn, (size_t)cap * nh * HD) || e->alloc(&e->pf_act, (size_t)cap * I) || e->alloc(&e->pf_seq, (size_t)cap) ||
-        e->alloc(&e->pf_pos, (size_t)cap))
+    const size_t cap = std::max(ntok + ntok / 4, 1024);
+    DevStore& store = e->store;
+    e->pf_cap = 0;  // until every block has grown: a failed growth leaves a freed block behind
+    if (store.grow(&e->pf_x, cap * H * sizeof(bf16), stream, true) || store.grow(&e->pf_xn, cap * H * sizeof(bf16), stream, true) ||
+        store.grow(&e->pf_qkv, cap * QKV * sizeof(bf16), stream, true) ||
+        store.grow(&e->pf_attn, cap * nh * HD * sizeof(bf16), stream, true) ||
+        store.grow(&e->pf_act, cap * I * sizeof(bf16), stream, true) || store.grow(&e->pf_seq, cap * sizeof(int), stream, true) ||
+        store.grow(&e->pf_pos, cap * sizeof(int), stream, true))
       return 1;
-    e->pf_cap = cap;
+    e->pf_cap = (int)cap;
   }
   pf_index_kernel<<<dim3((std::max(ntok, row_work) + 255) / 256, n), 256, 0, stream>>>(pl, pr, e->st, e->seen, V, e->pf_seq, e->pf_pos);
   Q3_CUDA(cudaMemcpyAsync(e->pf_x, A.embeds, (size_t)ntok * H * 2, cudaMemcpyDeviceToDevice, stream));
   const int mt = (ntok + 127) / 128;
   const int zero = 0;
-  auto gemm = [&](const bf16* a, int K, const std::string& wname, int N, GemmEpilogue ep) -> int {
-    auto it = e->gemm_w.find(wname);
-    Q3_REQUIRE(it != e->gemm_w.end(), "missing prefill GEMM weight %s", wname.c_str());
+  auto gemm = [&](const bf16* a, int K, const bf16* w, int N, GemmEpilogue ep) -> int {
     ep.cmod = N;
     GemmPlan plan;
-    if (gemm_make_plan(&plan, a, 1, ntok, K, K, (int64_t)ntok * K, it->second, N, K, 1, &zero, gemm_pick_bn(N, mt, 1), ep)) return 1;
+    if (gemm_make_plan(&plan, a, 1, ntok, K, K, (int64_t)ntok * K, w, N, K, 1, &zero, gemm_pick_bn(N, mt, 1), ep)) return 1;
     return gemm_launch(plan, stream);
   };
   const int rows_per_blk = 8;
   for (int l = 0; l < tc.num_layers; ++l) {
-    const std::string p = "talker.layers." + std::to_string(l);
-    const bf16 *ln1 = e->plain[p + ".ln1"], *ln2 = e->plain[p + ".ln2"], *qn = e->plain[p + ".q_norm"], *kn = e->plain[p + ".k_norm"];
-    Q3_REQUIRE(ln1 && ln2 && qn && kn, "missing norm weights of %s", p.c_str());
-    pf_rmsnorm_kernel<<<(ntok + rows_per_blk - 1) / rows_per_blk, 256, 0, stream>>>(e->pf_x, ln1, e->pf_xn, ntok, H, tc.rms_eps);
-    { GemmEpilogue ep{}; ep.out_raw = e->pf_qkv; if (gemm(e->pf_xn, H, p + ".qkv", QKV, ep)) return 1; }
-    pf_qkv_post_kernel<<<(ntok * (nh + 2 * nkv) + 7) / 8, 256, 0, stream>>>(e->pf_qkv, ntok, e->pf_seq, e->pf_pos, nh, nkv, qn, kn, tc.rms_eps,
+    const PfLayer& L = e->pf_layers[l];
+    pf_rmsnorm_kernel<<<(ntok + rows_per_blk - 1) / rows_per_blk, 256, 0, stream>>>(e->pf_x, L.ln1, e->pf_xn, ntok, H, tc.rms_eps);
+    { GemmEpilogue ep{}; ep.out_raw = e->pf_qkv; if (gemm(e->pf_xn, H, L.qkv, QKV, ep)) return 1; }
+    pf_qkv_post_kernel<<<(ntok * (nh + 2 * nkv) + 7) / 8, 256, 0, stream>>>(e->pf_qkv, ntok, e->pf_seq, e->pf_pos, nh, nkv, L.qn, L.kn, tc.rms_eps,
                                                                          e->talker.rope_cos, e->talker.rope_sin, e->talker.kc,
                                                                          e->talker.vc, l, tc.num_layers, e->talker.cap);
     pf_attention_kernel<<<(ntok * nh + 7) / 8, 256, 0, stream>>>(e->pf_qkv, e->pf_attn, ntok, e->pf_seq, e->pf_pos, nh, nkv, e->talker.kc,
                                                                  e->talker.vc, l, tc.num_layers, e->talker.cap);
-    { GemmEpilogue ep{}; ep.resid = e->pf_x; ep.out_raw = e->pf_x; if (gemm(e->pf_attn, nh * HD, p + ".o", H, ep)) return 1; }
-    pf_rmsnorm_kernel<<<(ntok + rows_per_blk - 1) / rows_per_blk, 256, 0, stream>>>(e->pf_x, ln2, e->pf_xn, ntok, H, tc.rms_eps);
-    { GemmEpilogue ep{}; ep.act = ACT_SWIGLU_BLK8; ep.out_act = e->pf_act; if (gemm(e->pf_xn, H, p + ".gate_up", 2 * I, ep)) return 1; }
-    { GemmEpilogue ep{}; ep.resid = e->pf_x; ep.out_raw = e->pf_x; if (gemm(e->pf_act, I, p + ".down", H, ep)) return 1; }
+    { GemmEpilogue ep{}; ep.resid = e->pf_x; ep.out_raw = e->pf_x; if (gemm(e->pf_attn, nh * HD, L.o, H, ep)) return 1; }
+    pf_rmsnorm_kernel<<<(ntok + rows_per_blk - 1) / rows_per_blk, 256, 0, stream>>>(e->pf_x, L.ln2, e->pf_xn, ntok, H, tc.rms_eps);
+    { GemmEpilogue ep{}; ep.act = ACT_SWIGLU_BLK8; ep.out_act = e->pf_act; if (gemm(e->pf_xn, H, L.gate_up, 2 * I, ep)) return 1; }
+    { GemmEpilogue ep{}; ep.resid = e->pf_x; ep.out_raw = e->pf_x; if (gemm(e->pf_act, I, L.down, H, ep)) return 1; }
   }
   Q3_CUDA(cudaGetLastError());
   pf_gather_last_kernel<<<n, 128, 0, stream>>>(pl, e->pf_x, e->h_last, H);
@@ -837,10 +814,8 @@ static int prefill_rows(q3_engine* e, const Admission& A, unsigned int mask, cud
 static int ensure_trailing(q3_engine* e, int stride, cudaStream_t stream) {
   const size_t need = (size_t)MAXB * stride * e->cfg.talker.hidden_size;
   if (need > e->trailing_alloc) {  // (re)allocate the engine-owned copy of trailing_text_hidden
-    Q3_CUDA(cudaStreamSynchronize(stream));  // growth only: earlier launches may still read the old buffer
-    e->release(e->trailing);
-    e->trailing = nullptr;
-    if (e->alloc(&e->trailing, need)) return 1;
+    e->trailing_alloc = 0;  // until the block has grown
+    if (e->store.grow(&e->trailing, need * sizeof(bf16), stream, true)) return 1;
     e->trailing_alloc = need;
   }
   return 0;

@@ -1,4 +1,4 @@
-// Device memory of one codec-side engine (codec decoder, codec stream, codec encoder, speaker encoder): its named
+// Device memory of one engine (AR engine, codec decoder, codec stream, codec encoder, speaker encoder): its named
 // tensors and its scratch.  Every block is allocated through the store and freed when the store is destroyed.
 // Host-only.
 #pragma once
@@ -19,20 +19,32 @@ class DevStore {
   DevStore(const DevStore&) = delete;
   DevStore& operator=(const DevStore&) = delete;
 
-  // a new block of `bytes`, zero-filled if `zero`
+  // a new block of `bytes`, zero-filled if `zero`.  cudaMemset returns before the block is zero and is not ordered
+  // against non-blocking streams, so the device is drained before the block is handed out.
   int alloc(void** p, size_t bytes, bool zero = false) {
     cudaError_t e = cudaMalloc(p, bytes);
-    if (e != cudaSuccess) return q3_set_err("%s: cudaMalloc(%zu B) failed: %s", engine_, bytes, cudaGetErrorString(e));
+    if (e != cudaSuccess) {
+      cudaGetLastError();  // the failure stays ours: a later error check (ours or the framework's) must not report it
+      return q3_set_err("%s: cudaMalloc(%zu B) failed: %s", engine_, bytes, cudaGetErrorString(e));
+    }
     blocks_.push_back(*p);
-    if (zero && (e = cudaMemset(*p, 0, bytes)) != cudaSuccess)
+    if (zero && ((e = cudaMemset(*p, 0, bytes)) != cudaSuccess || (e = cudaDeviceSynchronize()) != cudaSuccess))
       return q3_set_err("%s: cudaMemset(%zu B) failed: %s", engine_, bytes, cudaGetErrorString(e));
     return 0;
   }
-
-  // replace the block *p (null, or a block of this store) by a new one of `bytes`.  Work queued on `stream` may
-  // still read the old block, so the stream is drained before it is freed.
+  // a new block of `count` elements of T
   template <class T>
-  int grow(T** p, size_t bytes, cudaStream_t stream) {
+  int alloc(T** p, size_t count, bool zero) {
+    void* q = nullptr;
+    if (alloc(&q, count * sizeof(T), zero)) return 1;
+    *p = static_cast<T*>(q);
+    return 0;
+  }
+
+  // replace the block *p (null, or a block of this store) by a new one of `bytes`, zero-filled if `zero`.  Work queued
+  // on `stream` may still read the old block, so the stream is drained before it is freed.
+  template <class T>
+  int grow(T** p, size_t bytes, cudaStream_t stream, bool zero = false) {
     if (*p) {
       Q3_CUDA(cudaStreamSynchronize(stream));
       for (size_t i = 0; i < blocks_.size(); ++i)
@@ -41,19 +53,23 @@ class DevStore {
       *p = nullptr;
     }
     void* q = nullptr;
-    if (alloc(&q, bytes)) return 1;
+    if (alloc(&q, bytes, zero)) return 1;
     *p = static_cast<T*>(q);
     return 0;
   }
 
-  // copy the device tensor `dev` (shape[ndim], elements of `dtype`) in as `name`
+  // copy the device tensor `dev` (shape[ndim], elements of `dtype`) in as `name`.  `dev` may still be being produced on
+  // the caller's stream (no stream crosses the load ABIs), so the device is drained before the copy; the copy is
+  // complete when load returns, so the caller may free `dev` then.
   int load(const std::string& name, const void* dev, const int64_t* shape, int ndim, DevDtype dtype) {
     int64_t n = 1;
     for (int i = 0; i < ndim; ++i) n *= shape[i];
     const size_t bytes = (size_t)n * dtype;
     void* p = nullptr;
     if (alloc(&p, (bytes + 255) & ~(size_t)255)) return 1;
+    Q3_CUDA(cudaDeviceSynchronize());
     Q3_CUDA(cudaMemcpy(p, dev, bytes, cudaMemcpyDeviceToDevice));
+    Q3_CUDA(cudaDeviceSynchronize());
     tensors_[name] = Tensor{p, n, dtype};
     return 0;
   }

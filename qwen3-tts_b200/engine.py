@@ -47,10 +47,8 @@ class AREngine:
         h = C.c_void_p()
         _lib.check(self.lib.q3_engine_create(C.byref(ec), C.byref(h)))
         self.h = h
-        self._keep = []
         self._load(weights)
         _lib.check(self.lib.q3_engine_finalize(self.h))
-        self._codes = None
         self._dbg = None
 
     # ------------------------------------------------------------------ weights
@@ -159,7 +157,6 @@ class AREngine:
         _lib.check(self.lib.q3_prefill(self.h, B, emb.data_ptr(), lens, tr.data_ptr(), tl, stride,
                                        pad.data_ptr(), C.byref(s), C.c_void_p(stream)))
         self._B = B
-        self._hold = (emb, tr, pad)
 
     # ------------------------------------------------------------------ continuous batching (low level)
     def session_begin(self, n_slots: int, tts_pad_embed: torch.Tensor, sp: SamplingParams, max_trailing: int = 0):
@@ -169,7 +166,6 @@ class AREngine:
         s = self._sampling(sp)
         stream = torch.cuda.current_stream(self.device).cuda_stream
         self._B = n_slots
-        self._hold = (pad,)
         self._session_sp = sp
         _lib.check(self.lib.q3_session_begin(self.h, int(n_slots), int(max_trailing), pad.data_ptr(), C.byref(s), C.c_void_p(stream)))
 
@@ -187,7 +183,6 @@ class AREngine:
             sps = (_lib.Sampling * n)(*[self._sampling(self._session_sp if s is None else s) for s in sampling])
         emb, lens, tr, tl, stride = self._pack(inputs_embeds, trailing_text)
         stream = torch.cuda.current_stream(self.device).cuda_stream
-        self._hold = self._hold + (emb, tr)
         _lib.check(self.lib.q3_admit_with_sampling(self.h, n, (C.c_int32 * n)(*[int(x) for x in slots]),
                                                    (C.c_uint32 * n)(*[int(k) & 0xffffffff for k in keys]), sps,
                                                    emb.data_ptr(), lens, tr.data_ptr(), tl, stride, C.c_void_p(stream)))
@@ -197,7 +192,6 @@ class AREngine:
         H = self.cfg.talker.hidden_size
         r = rows.reshape(-1, H).to(self.device, torch.bfloat16).contiguous()
         stream = torch.cuda.current_stream(self.device).cuda_stream
-        self._hold = self._hold + (r,)
         _lib.check(self.lib.q3_append_trailing(self.h, int(slot), r.data_ptr(), int(r.shape[0]), C.c_void_p(stream)))
 
     def release_slots(self, slots: Sequence[int]):

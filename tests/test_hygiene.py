@@ -40,6 +40,13 @@ def test_native_library_reads_no_environment_variables():
     assert not bad, f"native sources read environment variables: {bad}"
 
 
+def test_device_memory_is_allocated_and_freed_only_by_the_device_store():
+    csrc = os.path.join(ROOT, "qwen3-tts_b200", "csrc")
+    bad = [os.path.basename(f) for f in _py_files(csrc)
+           if os.path.basename(f) != "dev_store.h" and re.search(r"\bcuda(Malloc|Free)", open(f, encoding="utf-8").read())]
+    assert not bad, f"native sources that allocate or free device memory outside DevStore (csrc/dev_store.h): {bad}"
+
+
 def test_no_cpu_fallback_in_product_entry_points():
     eng = open(os.path.join(ROOT, "qwen3-tts_b200", "engine.py")).read()
     cod = open(os.path.join(ROOT, "qwen3-tts_b200", "codec.py")).read()
