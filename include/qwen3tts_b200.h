@@ -34,7 +34,7 @@
 extern "C" {
 #endif
 
-#define Q3_ABI_VERSION 1
+#define Q3_ABI_VERSION 2
 #define Q3_MAX_BATCH 32        /* sequences per engine pass (reference batches = padded batch on one GPU) */
 #define Q3_NUM_GROUPS_MAX 32
 
@@ -115,20 +115,18 @@ int q3_decode(q3_engine* e, int32_t max_frames, int32_t* codes_dev, int32_t code
 /* ---- continuous batching (SURVEY §8f-4; the reference has only the static padded batch of
  * modeling_qwen3_tts.py:2239-2254 behind a Gradio queue, cli/demo.py:629).  A session owns n_slots rows; a finished or
  * never-used slot is a row that keeps stepping and is ignored (exactly what HF does with finished rows of a batch).
- * q3_admit prefills n new requests into free slots WHILE the others keep their state: their K/V, positions, sampling
- * history and Philox streams are per row, so a request admitted at any frame generates what it would generate alone
- * (keys_host[r] is the request's Philox row key).  q3_decode / q3_get_progress are shared with the static path;
- * n_valid[b] counts the row's OWN frames, and the row's codes land at codes[b][0..n_valid).  q3_admit synchronises
- * `stream` (it needs the frame counter).  embeds_dev: the n prompts packed back to back; trailing_dev: [n][stride][H]. */
+ * q3_admit_with_sampling prefills n new requests into free slots WHILE the others keep their state: their K/V,
+ * positions, sampling history and Philox streams are per row, so a request admitted at any frame generates what it
+ * would generate alone (keys_host[r] is the request's Philox row key).  q3_decode / q3_get_progress are shared with the
+ * static path; n_valid[b] counts the row's OWN frames, and the row's codes land at codes[b][0..n_valid).
+ * q3_admit_with_sampling synchronises `stream` (it needs the frame counter).  embeds_dev: the n prompts packed back to
+ * back; trailing_dev: [n][stride][H]. */
 int q3_session_begin(q3_engine* e, int32_t n_slots, int32_t max_trailing, const void* tts_pad_dev, const q3_sampling* sp,
                      void* stream);
-int q3_admit(q3_engine* e, int32_t n, const int32_t* slots_host, const uint32_t* keys_host, const void* embeds_dev,
-             const int32_t* lens_host, const void* trailing_dev, const int32_t* trailing_lens_host,
-             int32_t trailing_stride, void* stream);
-/* q3_admit with per-request sampling parameters: request r samples (its prefill head and every frame-step) with
- * sp_host[r] (host array [n]; NULL = the session's sp for all, which is q3_admit) and the Philox key
- * (sp_host[r].seed, keys_host[r]), so it generates what it would generate alone in a session whose parameters are
- * sp_host[r].  A row without a running request (never admitted, finished, released) samples with the session's sp.
+/* Request r samples (its prefill head and every frame-step) with sp_host[r] (host array [n]; NULL = the session's sp
+ * for all) and the Philox key (sp_host[r].seed, keys_host[r]), so it generates what it would generate alone in a
+ * session whose parameters are sp_host[r].  A row without a running request (never admitted, finished, released)
+ * samples with the session's sp.
  * All n entries are checked (q3_sampling_check) before any other argument and any device work; a bad one fails the
  * whole call with an error naming the request index and the field.  Then every row (slot, prompt and trailing length,
  * trailing text) is checked before any state changes: a rejected call admits no row, and no slot, key or parameter
@@ -208,28 +206,24 @@ int q3_codec_forward(q3_codec* c, const int32_t* codes_dev, int32_t B, int32_t T
  * handle carries the decoder's causal state instead (conv tails, ConvTranspose overlap row, 71 frames of rotated K/V
  * per transformer layer), so pushing packets of any sizes yields exactly the waveform of the full causal forward
  * (…v2.py:869-884) over everything pushed, with only the NEW frames' work per packet.
- * open: B rows, packets of <= max_packet_frames frames.  step: codes_dev int32 [B][num_quantizers][n] (the next n
- * frames of every row) -> wav_dev fp32 [B][n * total_upsample]; asynchronous on `stream`.  reset: start new
- * utterances in all rows.  A row's position (frames pushed since its reset) may not pass the engine's max_frames (RoPE
- * table).
- * Per row (continuous batching: rows start and end at different frames, slots are reused):
- * step_rows: row b takes only the first counts_host[b] (0 <= counts_host[b] <= n, host int32 [B]) of the n frames in
- *   codes_dev; its audio is wav_dev[b][0, counts_host[b] * total_upsample) and the rest of its row is zeros.  Codes past
- *   a row's count are never read (any value, -1 included).  A row with count 0 keeps its state and position.
- *   q3_codec_stream_step(s, codes, n, wav, stream) is step_rows with every count n.
+ * open: B rows, packets of <= max_packet_frames frames.  A row's position (frames pushed since its reset) may not pass
+ * the engine's max_frames (RoPE table).  Every row has its own position (continuous batching: rows start and end at
+ * different frames, slots are reused):
+ * step_rows: codes_dev int32 [B][num_quantizers][n] (the next n frames of every row) -> wav_dev fp32
+ *   [B][n * total_upsample]; asynchronous on `stream`.  Row b takes only the first counts_host[b] (0 <= counts_host[b]
+ *   <= n, host int32 [B]) of the n frames; its audio is wav_dev[b][0, counts_host[b] * total_upsample) and the rest of
+ *   its row is zeros.  Codes past a row's count are never read (any value, -1 included).  A row with count 0 keeps its
+ *   state and position.
  * reset_rows: the n rows in rows_host (host int32, each in [0, B), no repeats) start new utterances at position 0;
  *   the other rows are untouched.
- * position: the common position of all rows, or -1 (q3_last_error says why) when rows differ; row_position: one row's.
+ * row_position: frames pushed to one row since its reset.
  * Bad arguments (a count outside [0, n], position + count > max_frames, a reset row out of range or listed twice, null
  * pointers) are rejected with an error naming the row before any device work, and leave every position unchanged. */
 typedef struct q3_codec_stream q3_codec_stream;
 int q3_codec_stream_open(q3_codec* c, int32_t B, int32_t max_packet_frames, q3_codec_stream** out);
-int q3_codec_stream_step(q3_codec_stream* s, const int32_t* codes_dev, int32_t n, float* wav_dev, void* stream);
 int q3_codec_stream_step_rows(q3_codec_stream* s, const int32_t* codes_dev, int32_t n, const int32_t* counts_host,
                               float* wav_dev, void* stream);
-int q3_codec_stream_reset(q3_codec_stream* s, void* stream);
 int q3_codec_stream_reset_rows(q3_codec_stream* s, int32_t n, const int32_t* rows_host, void* stream);
-int q3_codec_stream_position(q3_codec_stream* s);
 int q3_codec_stream_row_position(q3_codec_stream* s, int32_t row);
 /* copy_rows: for i < n, row dst_rows_host[i] of dst becomes exactly row src_rows_host[i] of src (host int32 [n]): its
  *   decoder state (the history of every buffer: conv tails, ConvTranspose overlap rows, each layer's K/V window) and
@@ -244,7 +238,7 @@ int q3_codec_stream_copy_rows(q3_codec_stream* dst, const q3_codec_stream* src, 
                               const int32_t* dst_rows_host, void* stream);
 void q3_codec_stream_close(q3_codec_stream* s);
 int q3_codec_total_upsample(q3_codec* c);
-/* kernels launched by the last q3_codec_forward or q3_codec_stream_step (bench.py's gpu_launches bookkeeping) */
+/* kernels launched by the last q3_codec_forward or q3_codec_stream_step_rows (bench.py's gpu_launches bookkeeping) */
 int q3_codec_last_launch_count(q3_codec* c);
 /* Test hook (tests/ only): per-stage capture of the DECODER, so that an error in one small kernel cannot hide behind the
  * waveform SNR.  The following q3_codec_forward calls copy the bf16 [B][T_stage][C_stage] tensor of `stage` into dst_dev

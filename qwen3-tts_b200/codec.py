@@ -296,11 +296,6 @@ class CodecStream:
         self._seeder: Optional["CodecStream"] = None   # private stream of seed(), opened on first use
 
     @property
-    def position(self) -> int:
-        """Frames pushed since the last reset, common to all rows (-1 when rows differ: see `positions`)."""
-        return int(self.dec.lib.q3_codec_stream_position(self.h))
-
-    @property
     def positions(self) -> List[int]:
         """Frames pushed to each row since its last reset."""
         return [int(self.dec.lib.q3_codec_stream_row_position(self.h, b)) for b in range(self.B)]
@@ -309,29 +304,26 @@ class CodecStream:
     def push(self, codes: torch.Tensor, counts: Optional[Sequence[int]] = None) -> torch.Tensor:
         """codes (B,K,n) -> wav (B,1,n*upsample).  With `counts`, row b takes only its first counts[b] frames
         (0 <= counts[b] <= n; the codes past them are never read): its audio is wav[b, 0, :counts[b]*upsample] and
-        the rest of its row is zeros."""
+        the rest of its row is zeros.  Without, every row takes all n."""
         dec = self.dec
         if codes.dim() != 3 or codes.shape[0] != self.B or codes.shape[1] != dec.cfg.num_quantizers:
             raise ValueError(f"expected codes of shape ({self.B}, {dec.cfg.num_quantizers}, n), got {tuple(codes.shape)}")
         n = int(codes.shape[2])
-        if counts is not None:
-            counts = [int(k) for k in counts]
-            if len(counts) != self.B:
-                raise ValueError(f"expected {self.B} counts, got {len(counts)}")
-            for b, k in enumerate(counts):
-                if not 0 <= k <= n:
-                    raise ValueError(f"row {b}: count {k} outside [0, {n}]")
+        counts = [n] * self.B if counts is None else [int(k) for k in counts]
+        if len(counts) != self.B:
+            raise ValueError(f"expected {self.B} counts, got {len(counts)}")
+        for b, k in enumerate(counts):
+            if not 0 <= k <= n:
+                raise ValueError(f"row {b}: count {k} outside [0, {n}]")
         out = []
         for s0 in range(0, n, self.nmax):  # longer pushes are cut into packets of the stream's capacity
             c = codes[:, :, s0:s0 + self.nmax].to(dec.device, torch.int32).contiguous()
             m = int(c.shape[2])
             wav = torch.empty(self.B, m * dec.total_upsample, dtype=torch.float32, device=dec.device)
             stream = C.c_void_p(torch.cuda.current_stream(dec.device).cuda_stream)
-            if counts is None:
-                _lib.check(dec.lib.q3_codec_stream_step(self.h, c.data_ptr(), m, wav.data_ptr(), stream))
-            else:  # a row's frames fill the packets in order: this packet holds frames s0 .. s0+m of the push
-                k = (C.c_int32 * self.B)(*[min(max(kb - s0, 0), m) for kb in counts])
-                _lib.check(dec.lib.q3_codec_stream_step_rows(self.h, c.data_ptr(), m, k, wav.data_ptr(), stream))
+            # a row's frames fill the packets in order: this packet holds frames s0 .. s0+m of the push
+            k = (C.c_int32 * self.B)(*[min(max(kb - s0, 0), m) for kb in counts])
+            _lib.check(dec.lib.q3_codec_stream_step_rows(self.h, c.data_ptr(), m, k, wav.data_ptr(), stream))
             self._keep = c
             out.append(wav)
         return torch.cat(out, 1)[:, None, :] if out else torch.zeros(self.B, 1, 0, device=dec.device)
@@ -339,11 +331,8 @@ class CodecStream:
     def reset(self, rows: Optional[Sequence[int]] = None):
         """Start new utterances in `rows` (all rows when None); the other rows keep their state."""
         stream = C.c_void_p(torch.cuda.current_stream(self.dec.device).cuda_stream)
-        if rows is None:
-            _lib.check(self.dec.lib.q3_codec_stream_reset(self.h, stream))
-        else:
-            rows = [int(r) for r in rows]
-            _lib.check(self.dec.lib.q3_codec_stream_reset_rows(self.h, len(rows), (C.c_int32 * max(len(rows), 1))(*rows), stream))
+        rows = range(self.B) if rows is None else [int(r) for r in rows]
+        _lib.check(self.dec.lib.q3_codec_stream_reset_rows(self.h, len(rows), (C.c_int32 * max(len(rows), 1))(*rows), stream))
 
     @torch.no_grad()
     def seed(self, rows: Sequence[int], codes: Sequence[torch.Tensor]):

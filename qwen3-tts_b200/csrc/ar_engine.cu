@@ -240,7 +240,7 @@ struct q3_engine {
   int frame0[MAXB] = {0};
   unsigned int row_key[MAXB] = {0};
   bool active[MAXB] = {false};
-  bool session = false;       // continuous-batching session (q3_session_begin / q3_admit)
+  bool session = false;       // continuous-batching session (q3_session_begin / q3_admit_with_sampling)
   unsigned int admit_mask = 0xffffffffu;
   unsigned char* seen = nullptr;
   float* split_buf = nullptr;
@@ -696,16 +696,27 @@ extern "C" int q3_engine_finalize(q3_engine* e) {
   return 0;
 }
 
+// field by field: q3_sampling has padding before `seed`, which memcmp would compare
+static bool same_sampling(const q3_sampling& a, const q3_sampling& b) {
+  return a.do_sample == b.do_sample && a.top_k == b.top_k && a.top_p == b.top_p && a.temperature == b.temperature &&
+         a.repetition_penalty == b.repetition_penalty && a.subtalker_dosample == b.subtalker_dosample &&
+         a.subtalker_top_k == b.subtalker_top_k && a.subtalker_top_p == b.subtalker_top_p &&
+         a.subtalker_temperature == b.subtalker_temperature && a.min_new_tokens == b.min_new_tokens &&
+         a.suppress_eos == b.suppress_eos && a.seed == b.seed;
+}
+
 static int launch_program(q3_engine* e, int off, int n, int mode, int max_iters, int nt, const SmemPlan& plan,
                           const PieceTable& pt, int* codes_dev, cudaStream_t stream) {
   KParams P{};
   P.prog = e->prog_dev + off; P.n_phases = n; P.mode = mode; P.max_iters = max_iters; P.st = e->st;
   P.talker = e->talker; P.cp = e->cp; P.G = e->cfg.num_code_groups; P.eos = e->cfg.codec_eos_token_id;
   P.has_proj = e->cfg.has_cp_projection; P.sp = e->sp;
-  // a session's rows sample with their own request's parameters; a row without a running request (never admitted,
-  // finished, released) with the session's, so that a request's settings stop costing the others once it has left
-  P.row_sampling = e->session ? 1 : 0;
-  if (e->session)
+  // rows sample with their own request's parameters; a row without a running request (never admitted, finished,
+  // released) with the default's, so that a request's settings stop costing the others once it has left.  The per-row
+  // table is used only when some running row's parameters differ from the default: otherwise every row reads P.sp.
+  for (int b = 0; b < e->B; ++b)
+    if (e->active[b] && !same_sampling(e->row_sp[b], e->sp)) P.row_sampling = 1;
+  if (P.row_sampling)
     for (int b = 0; b < MAXB; ++b) P.row_sp[b] = e->active[b] ? e->row_sp[b] : e->sp;
   P.B = e->B;
   for (int b = 0; b < MAXB; ++b) { P.len0[b] = e->len0[b]; P.trailing_len[b] = e->trailing_len[b]; }
@@ -933,7 +944,7 @@ extern "C" int q3_sampling_check(const q3_sampling* sp) {
   return check_sampling(*sp);
 }
 
-// sp_host == nullptr: every request samples with the session's parameters (q3_admit)
+// sp_host == nullptr: every request samples with the session's parameters
 extern "C" int q3_admit_with_sampling(q3_engine* e, int32_t n, const int32_t* slots_host, const uint32_t* keys_host,
                                       const q3_sampling* sp_host, const void* embeds_dev, const int32_t* lens_host,
                                       const void* trailing_dev, const int32_t* trailing_lens_host, int32_t trailing_stride,
@@ -958,13 +969,6 @@ extern "C" int q3_admit_with_sampling(q3_engine* e, int32_t n, const int32_t* sl
     if (e->active[b] && !hs.finished[b]) running |= 1u << b;
   const Admission A{n, slots_host, keys_host, sp_host, embeds_dev, lens_host, trailing_dev, trailing_lens_host, trailing_stride};
   return admit_rows(e, A, hs.step, running, stream);
-}
-
-extern "C" int q3_admit(q3_engine* e, int32_t n, const int32_t* slots_host, const uint32_t* keys_host, const void* embeds_dev,
-                        const int32_t* lens_host, const void* trailing_dev, const int32_t* trailing_lens_host,
-                        int32_t trailing_stride, void* stream_) {
-  return q3_admit_with_sampling(e, n, slots_host, keys_host, nullptr, embeds_dev, lens_host, trailing_dev, trailing_lens_host,
-                                trailing_stride, stream_);
 }
 
 extern "C" int q3_decode(q3_engine* e, int32_t max_frames, int32_t* codes_dev, int32_t codes_stride, void* stream_) {

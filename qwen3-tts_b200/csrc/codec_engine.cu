@@ -446,18 +446,6 @@ static RollTable hist_table(const q3_codec_stream* s) {
   return tb;
 }
 
-// the common position of all rows; -1 (q3_last_error says why) when rows differ
-extern "C" int q3_codec_stream_position(q3_codec_stream* s) {
-  if (!s) { q3_set_err("null stream"); return -1; }
-  for (int b = 1; b < s->B; ++b)
-    if (s->pos[b] != s->pos[0]) {
-      q3_set_err("rows are at different positions (row 0 at %d, row %d at %d): use q3_codec_stream_row_position", s->pos[0], b,
-                 s->pos[b]);
-      return -1;
-    }
-  return s->pos[0];
-}
-
 // frames pushed to `row` since its last reset; -1 for a bad row
 extern "C" int q3_codec_stream_row_position(q3_codec_stream* s, int32_t row) {
   if (!s || row < 0 || row >= s->B) { q3_set_err("row %d out of range [0, %d)", row, s ? s->B : 0); return -1; }
@@ -487,13 +475,6 @@ extern "C" int q3_codec_stream_step_rows(q3_codec_stream* s, const int32_t* code
   Q3_CUDA(cudaGetLastError());
   for (int b = 0; b < s->B; ++b) s->pos[b] += counts_host[b];
   return 0;
-}
-
-// next n frames of every row: codes_dev int32 [B][K][n] -> wav_dev fp32 [B][n * total_upsample]
-extern "C" int q3_codec_stream_step(q3_codec_stream* s, const int32_t* codes_dev, int32_t n, float* wav_dev, void* stream_) {
-  Q3_REQUIRE(s, "null argument");
-  const std::vector<int32_t> counts(s->B, n);
-  return q3_codec_stream_step_rows(s, codes_dev, n, counts.data(), wav_dev, stream_);
 }
 
 // forget the listed rows: their next packet starts a new utterance at position 0; the other rows are untouched
@@ -549,12 +530,4 @@ extern "C" int q3_codec_stream_copy_rows(q3_codec_stream* dst, const q3_codec_st
   Q3_CUDA(cudaGetLastError());
   for (int i = 0; i < n; ++i) dst->pos[dst_rows_host[i]] = src->pos[src_rows_host[i]];
   return 0;
-}
-
-// forget everything: the next packet starts a new utterance in every row
-extern "C" int q3_codec_stream_reset(q3_codec_stream* s, void* stream_) {
-  Q3_REQUIRE(s, "null stream");
-  std::vector<int32_t> rows(s->B);
-  for (int b = 0; b < s->B; ++b) rows[b] = b;
-  return q3_codec_stream_reset_rows(s, s->B, rows.data(), stream_);
 }

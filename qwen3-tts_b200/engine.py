@@ -6,7 +6,7 @@ tts_pad_embed, **talker_kwargs)` at core/models/modeling_qwen3_tts.py:2272-2278 
 PyTorch is used only for device memory and streams.
 """
 import ctypes as C
-from typing import Iterator, List, Optional, Sequence
+from typing import Optional, Sequence
 
 import torch
 
@@ -289,30 +289,3 @@ class AREngine:
         if return_hidden:
             return out, [hid[b, :o.shape[0]].clone() for b, o in enumerate(out)]
         return out
-
-    @torch.no_grad()
-    def stream(self, inputs_embeds, trailing_text, tts_pad_embed, sp: SamplingParams,
-               packet_frames: int = 4) -> Iterator[List[torch.Tensor]]:
-        """Streaming output (no counterpart in the reference, SURVEY F1): yields, per packet, the list of new
-        (n_i, G) code tensors per row (packet = 4 frames = 320 ms, Qwen3-TTS report §3.4)."""
-        B = len(inputs_embeds)
-        G = self.cfg.num_code_groups
-        max_frames = self._frame_budget(inputs_embeds, sp)
-        self.prefill(inputs_embeds, trailing_text, tts_pad_embed, sp)
-        codes = torch.zeros(B, max(max_frames, 1), G, dtype=torch.int32, device=self.device)
-        emitted = [0] * B
-        done = 0
-        while done < max_frames:
-            n = min(packet_frames, max_frames - done)
-            self.decode(n, codes)
-            torch.cuda.current_stream(self.device).synchronize()
-            fd, n_valid, fin = self.progress()
-            out = []
-            for b in range(B):
-                hi = min(n_valid[b], fd)
-                out.append(codes[b, emitted[b]:hi].to(torch.int64))
-                emitted[b] = max(emitted[b], hi)
-            yield out
-            if all(fin) or fd == done:
-                break
-            done = fd

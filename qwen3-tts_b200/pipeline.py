@@ -11,6 +11,7 @@ import torch
 from .codec import CodecDecoder, check_ref_codes
 from .config import CodecConfig, SamplingParams, TTSConfig
 from .engine import AREngine
+from .scheduler import ContinuousBatcher
 
 
 class TTSEngine:
@@ -58,14 +59,15 @@ class TTSEngine:
                           left_context="stateful", ref_codes=None):
         """Streaming OUTPUT (new surface: the reference returns audio whole, SURVEY F1).  Yields, per packet of
         `packet_frames` frames (4 frames = 320 ms, Qwen3-TTS report §3.4), a list with one fp32 numpy waveform chunk per
-        row.  Default: the STATEFUL codec stream (q3_codec_stream_*) — each packet costs its own frames only and the
-        concatenated chunks equal the one-shot causal decode.  `left_context=25` decodes every packet together with 25
+        row (empty for a row without new frames).  The rows run as one ContinuousBatcher session.  Default: the
+        STATEFUL codec stream (q3_codec_stream_*) — each packet costs its own frames only and the concatenated chunks
+        equal the one-shot causal decode.  `left_context=25` decodes every packet together with 25
         already-emitted frames, exactly like the reference's chunked_decode does between chunks (…v2.py:886-896);
         `left_context=None` re-decodes the whole prefix.
         `ref_codes`: one entry per row, the (L, K) reference codes of a voice-clone row (VoiceClonePromptItem.ref_code)
         or None.  A row's audio is then decoded as cat(ref_codes, generated codes) is (qwen3_tts_model.py:612-631):
-        the stateful stream seeds the row with its reference, the windowed modes start its history with it.  The
-        chunks hold the generated audio only."""
+        the stateful stream seeds the row with its reference (and caps its horizon at the codec's max_frames minus the
+        reference's length), the windowed modes start its history with it.  The chunks hold the generated audio only."""
         dev = self.device
         emb = [e.to(dev, non_blocking=True) for e in inputs_embeds]
         tr = [t.to(dev, non_blocking=True) for t in trailing_text]
@@ -81,7 +83,10 @@ class TTSEngine:
                 if r is not None:
                     check_ref_codes(self.codec_cfg, r, self.codec.max_frames, f"row {b}: ref_codes")
                     refs[b] = r.to(dev, torch.int64)
-        if left_context == "stateful":
+        budget = self.ar._frame_budget(emb, sp)
+        stateful = left_context == "stateful"
+        cs = None
+        if stateful:
             key = (B, int(packet_frames))
             if getattr(self, "_cstream_key", None) != key:
                 if getattr(self, "_cstream", None) is not None:
@@ -89,47 +94,36 @@ class TTSEngine:
                 self._cstream = self.codec.open_stream(B, max_packet_frames=int(packet_frames))
                 self._cstream_key = key
             cs = self._cstream
-            cs.reset()
-            seeded = [b for b in range(B) if refs[b] is not None]
-            if seeded:
-                cs.seed(seeded, [refs[b] for b in seeded])
-            for pkt in self.ar.stream(emb, tr, pad, sp, packet_frames=packet_frames):
-                n_new = [int(p.shape[0]) for p in pkt]
-                n = max(n_new) if n_new else 0
-                if n == 0:
-                    yield [np.zeros(0, dtype=np.float32) for _ in pkt]
-                    continue
-                # rows that already finished (or got fewer frames) are padded with code 0: their state no longer matters
-                codes = torch.zeros(B, n, K, dtype=torch.int64, device=dev)
-                for b, p in enumerate(pkt):
-                    if p.shape[0]:
-                        codes[b, :p.shape[0]] = p
-                # a seeded row starts past position 0: it takes its own frames only, so that padding never walks it
-                # past the RoPE table
-                wav = cs.push(codes.transpose(1, 2).contiguous(), n_new if seeded else None)[:, 0].to(torch.float32).cpu().numpy()
-                yield [wav[b, :n_new[b] * up] for b in range(B)]
+        # the static batch is a session of B slots whose rows are all admitted in the first step, row b with Philox key b
+        H = self.ar.cfg.talker.hidden_size
+        cb = ContinuousBatcher(self.ar, pad, sp, n_slots=B, packet_frames=packet_frames,
+                               max_trailing=max(int(t.reshape(-1, H).shape[0]) for t in tr), codec=cs)
+        for b in range(B):
+            cb.submit(emb[b], tr[b], key=b, max_frames=budget, ref_codes=refs[b] if stateful else None)
+        if budget == 0:
+            return
+        if stateful:
+            for chunks, _ in cb.stream():
+                yield [chunks.get(b, np.zeros(0, dtype=np.float32)) for b in range(B)]
             return
         hist = [torch.zeros(0, K, dtype=torch.int64, device=dev) if r is None else r for r in refs]
-        for pkt in self.ar.stream(emb, tr, pad, sp, packet_frames=packet_frames):
-            out = [np.zeros(0, dtype=np.float32) for _ in pkt]
+        for new, _ in cb.packets():
+            out = [np.zeros(0, dtype=np.float32) for _ in range(B)]
             # rows whose window has the same shape (the normal case: every live row got `packet_frames` new frames on top
             # of the same history) go through ONE batched codec call — rows are independent in the decoder, so this is
             # bit-identical to decoding them one by one, at 1/B of the launches
             groups = {}
-            for b, new in enumerate(pkt):
-                if new.shape[0] == 0:
-                    continue
+            for b, codes in new.items():
                 ctx = hist[b].shape[0] if left_context is None else min(left_context, hist[b].shape[0])
-                groups.setdefault((ctx, int(new.shape[0])), []).append(b)
+                groups.setdefault((ctx, int(codes.shape[0])), []).append(b)
             for (ctx, n_new), rows in groups.items():
-                windows = torch.stack([torch.cat([hist[b][hist[b].shape[0] - ctx:], pkt[b]], 0) for b in rows], 0)  # (n, T, K)
+                windows = torch.stack([torch.cat([hist[b][hist[b].shape[0] - ctx:], new[b]], 0) for b in rows], 0)  # (n, T, K)
                 wav = self.codec.forward(windows.transpose(1, 2).contiguous())[:, 0, ctx * up:]
                 wav = wav.to(torch.float32).cpu().numpy()
                 for i, b in enumerate(rows):
                     out[b] = wav[i]
-            for b, new in enumerate(pkt):
-                if new.shape[0]:
-                    hist[b] = torch.cat([hist[b], new], 0)
+            for b, codes in new.items():
+                hist[b] = torch.cat([hist[b], codes], 0)
             yield out
 
     def close(self):

@@ -17,7 +17,9 @@ sample with the session's parameters.
 With a codec the batcher also streams audio: one codec stream of `n_slots` rows follows the session, a slot's row is
 reset when a request enters it, and after every decode each running slot pushes its new frames as its own count (idle
 slots push none).  A request's concatenated chunks equal the one-shot decode of its codes alone
-(tests/test_gpu_scheduler_audio.py).
+(tests/test_gpu_scheduler_audio.py).  `packets()` hands out the new codes instead, for callers that decode them
+themselves.  TTSEngine.stream_synthesize runs its static batch as such a session: B requests submitted together are
+admitted in one call, in slots and with Philox keys 0..B-1, which is what q3_prefill does.
 
 A request may carry reference codes (voice cloning, `ref_codes` of submit): the reference decodes cat(ref_code,
 generated codes) and cuts the reference's audio off (qwen3_tts_model.py:612-631), so the generated frames are decoded
@@ -27,12 +29,12 @@ the generated part only (tests/test_gpu_scheduler_voice_clone.py).
 """
 from collections import deque
 from dataclasses import dataclass, field
-from typing import Deque, Dict, Iterator, List, Optional, Tuple
+from typing import Deque, Dict, Iterator, List, Optional, Tuple, Union
 
 import numpy as np
 import torch
 
-from .codec import CodecDecoder, check_ref_codes
+from .codec import CodecDecoder, CodecStream, check_ref_codes
 from .config import SamplingParams
 from .engine import AREngine
 
@@ -52,7 +54,9 @@ class _Request:
 
 class ContinuousBatcher:
     def __init__(self, engine: AREngine, tts_pad_embed: torch.Tensor, sp: SamplingParams, n_slots: int = 8, packet_frames: int = 4,
-                 max_trailing: int = 256, codec: Optional[CodecDecoder] = None):
+                 max_trailing: int = 256, codec: Union[CodecDecoder, CodecStream, None] = None):
+        """`codec`: a CodecDecoder, whose stream of `n_slots` rows the batcher opens, or an open CodecStream of
+        `n_slots` rows taking packets of at least `packet_frames` frames."""
         self.eng, self.sp = engine, sp
         self.n_slots, self.packet = int(n_slots), int(packet_frames)
         self.G = engine.cfg.num_code_groups
@@ -65,8 +69,16 @@ class ContinuousBatcher:
         self.max_trailing = int(max_trailing)
         engine.session_begin(self.n_slots, tts_pad_embed, sp, max_trailing=self.max_trailing)
         self.frames_total = 0
-        self.codec = codec
-        self.cstream = codec.open_stream(self.n_slots, max_packet_frames=self.packet) if codec is not None else None
+        if isinstance(codec, CodecStream):
+            if codec.B != self.n_slots or codec.nmax < self.packet:
+                raise ValueError(f"a codec stream of {codec.B} rows and packets of up to {codec.nmax} frames cannot "
+                                 f"serve {self.n_slots} slots with packets of {self.packet} frames")
+            self.codec, self.cstream = codec.dec, codec
+        elif codec is None or hasattr(codec, "open_stream"):   # a CodecDecoder (or a test's stand-in for one)
+            self.codec = codec
+            self.cstream = codec.open_stream(self.n_slots, max_packet_frames=self.packet) if codec is not None else None
+        else:
+            raise ValueError(f"codec must be a CodecDecoder or a CodecStream, got {type(codec).__name__}")
 
     # ------------------------------------------------------------------ API
     def submit(self, inputs_embeds: torch.Tensor, trailing_text: Optional[torch.Tensor] = None, key: Optional[int] = None,
@@ -100,7 +112,7 @@ class ContinuousBatcher:
         room = self.eng.max_ctx - L
         if room < 1:
             raise ValueError(f"prompt of {L} positions does not fit max_ctx={self.eng.max_ctx}")
-        horizon = min(max_frames or limit, limit, room)
+        horizon = min(limit if max_frames is None else max_frames, limit, room)
         if self.codec is not None:
             horizon = min(horizon, self.codec.max_frames - L_ref)  # a codec row's position may not pass its RoPE table
         self.pending.append(_Request(rid, inputs_embeds, tr, horizon, sampling, ref_codes))
@@ -108,7 +120,9 @@ class ContinuousBatcher:
 
     def step(self) -> List[int]:
         """Admit what fits, decode one packet, collect what finished.  Returns the ids that completed in this step."""
-        return self._advance()[1]
+        new, finished = self._advance()
+        self._push_audio(new)
+        return finished
 
     def stream(self) -> Iterator[Tuple[Dict[int, np.ndarray], List[int]]]:
         """Run the session with audio out: yields per step ({request id: float32 waveform of its new frames},
@@ -117,10 +131,19 @@ class ContinuousBatcher:
         if self.cstream is None:
             raise ValueError("stream() needs a ContinuousBatcher built with a codec")
         while self.pending or self.running:
-            chunks, finished = self._advance()
-            yield chunks, finished
+            new, finished = self._advance()
+            yield self._push_audio(new), finished
 
-    def _advance(self) -> Tuple[Dict[int, np.ndarray], List[int]]:
+    def packets(self) -> Iterator[Tuple[Dict[int, torch.Tensor], List[int]]]:
+        """Run the session with codes out: yields per step ({request id: (k, G) int64 codes of its k new frames},
+        [ids that finished in the step]) while requests are pending or running.  The codec stream, if any, is not
+        pushed."""
+        while self.pending or self.running:
+            new, finished = self._advance()
+            yield {r.rid: self.codes[slot, e0:e0 + k].to(torch.int64) for slot, (r, e0, k) in new.items() if k > 0}, finished
+
+    def _advance(self):
+        """One step of the session: ({slot: (request, first new frame, new frames)}, [ids that finished])."""
         free = [s for s in range(self.n_slots) if s not in self.running]
         batch = []
         while free and self.pending:
@@ -162,7 +185,7 @@ class ContinuousBatcher:
                 del self.running[slot]
         if give_up:
             self.eng.release_slots(give_up)
-        return self._push_audio(new), finished
+        return new, finished
 
     def _push_audio(self, new) -> Dict[int, np.ndarray]:
         """One codec step over all slots: slot s takes its new frames codes[s, e0:e0+k] as its count k, idle slots 0."""

@@ -13,7 +13,7 @@ def _declared_symbols():
     return sorted(set(re.findall(r"\b(q3_[a-z0-9_]+)\s*\(", hdr)))
 
 
-def test_library_builds_and_exports_header_symbols():
+def test_library_builds_and_exports_the_abi_2_header_symbols():
     from qwen3_tts_b200 import _lib, build
     path = build.build()
     assert os.path.exists(path)
@@ -24,7 +24,7 @@ def test_library_builds_and_exports_header_symbols():
     assert not missing, f"symbols declared in the header but not exported: {missing}"
     assert sorted(_lib.AR_SYMBOLS + _lib.CODEC_SYMBOLS) == syms
     lib.q3_abi_version.restype = ctypes.c_int
-    assert lib.q3_abi_version() == 1
+    assert lib.q3_abi_version() == 2
 
 
 def test_engine_fails_loudly_without_gpu():

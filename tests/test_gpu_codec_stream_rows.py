@@ -119,7 +119,7 @@ def test_full_config_rows_staggered_past_the_window():
     dec.close()
 
 
-def test_push_without_counts_equals_full_counts():
+def test_push_without_counts_equals_every_count_n():
     from qwen3_tts_b200.codec import CodecDecoder
     cfg = _small_cfg()
     Wb, _ = _bf16_round(OC.random_weights(cfg, seed=2))
@@ -131,12 +131,12 @@ def test_push_without_counts_equals_full_counts():
         wa = a.push(codes[:, :, s0:s0 + n]).cpu()
         wb = b.push(codes[:, :, s0:s0 + n], counts=[n, n]).cpu()
         assert torch.equal(wa, wb)
-    assert a.position == b.position == 19 and a.positions == b.positions == [19, 19]
+    assert a.positions == b.positions == [19, 19]
     a.close(), b.close()
     dec.close()
 
 
-def test_row_parked_at_the_table_end_with_count_zero():
+def test_row_parked_at_the_table_end_takes_count_zero():
     """A row at position max_frames takes count 0 while the other rows step: accepted, and the others stay exact."""
     from qwen3_tts_b200.codec import CodecDecoder
     cfg = _small_cfg()
@@ -151,7 +151,7 @@ def test_row_parked_at_the_table_end_with_count_zero():
         pkt[0], k1 = u0[:, s0:s0 + 4], min(4, max(0, 6 - s0))
         pkt[1, :, :k1] = u1[:, s0:s0 + k1]
         w1.append(st.push(pkt.to(DEV), [4, k1])[1, 0, :k1 * UP].cpu())
-    assert st.positions == [16, 6] and st.position == -1
+    assert st.positions == [16, 6]
     for s0 in range(6, 14, 4):                       # row 0 is parked at max_frames = 16
         pkt = _garbage((2, cfg.num_quantizers, 4), g)
         pkt[1] = u1[:, s0:s0 + 4]
@@ -165,7 +165,7 @@ def test_row_parked_at_the_table_end_with_count_zero():
     dec.close()
 
 
-def test_argument_checks_name_the_row_and_change_nothing():
+def test_argument_checks_name_the_row_and_change_no_position():
     """Every check fires before any device work.  Each bad case is paired with n = 0 (step) or more rows than the
     stream has (reset), so that a later check would refuse the call anyway and nothing is launched without it."""
     from qwen3_tts_b200.codec import CodecDecoder
@@ -205,7 +205,6 @@ def test_argument_checks_name_the_row_and_change_nothing():
         assert re.search(msg, lib.q3_last_error().decode()), (msg, lib.q3_last_error())
         assert st.positions == [8, 2, 1]
     assert lib.q3_codec_stream_row_position(st.h, 3) == -1 and "row 3 out of range" in lib.q3_last_error().decode()
-    assert st.position == -1 and "different positions" in lib.q3_last_error().decode()
     with pytest.raises(ValueError, match="row 1: count 5 outside"):
         st.push(codes, [0, 5, 0])
     # the stream still works: reset one row, the others keep their positions

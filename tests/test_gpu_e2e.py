@@ -46,16 +46,20 @@ def test_custom_voice_end_to_end_and_determinism():
     assert np.array_equal(solo[0], wavs[0])
 
 
-def test_streaming_packets_equal_one_shot():
+def test_batcher_packets_equal_one_shot():
     import qwen3_tts_b200 as q
+    from qwen3_tts_b200.scheduler import ContinuousBatcher
     cfg, core, m = _build()
     ids = [_proc(text=f"<|im_start|>assistant\n{t}<|im_end|>\n<|im_start|>assistant\n")["input_ids"] for t in ("abc def", "ghi")]
     emb, trail, pad = core.build_prefill(ids, None, None, None, ["english", "english"], ["alice", "bob"], False)
     sp = q.SamplingParams(max_new_tokens=14, suppress_eos=True, seed=3)
     one = core.engine.generate(emb, trail, pad, sp)
+    cb = ContinuousBatcher(core.engine, pad, sp, n_slots=len(emb), packet_frames=4)
+    for b in range(len(emb)):
+        cb.submit(emb[b], trail[b], key=b)
     parts = [[] for _ in emb]
-    for pkt in core.engine.stream(emb, trail, pad, sp, packet_frames=4):
-        for b, p in enumerate(pkt):
+    for new, _ in cb.packets():
+        for b, p in new.items():
             parts[b].append(p)
     for b in range(len(emb)):
         assert torch.equal(torch.cat(parts[b]), one[b]) and one[b].shape == (13, 16)

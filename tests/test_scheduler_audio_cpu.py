@@ -113,3 +113,30 @@ def test_without_a_codec_stream_is_refused_and_step_is_unchanged(monkeypatch):
     with pytest.raises(ValueError, match="codec"):
         next(cb.stream())
     assert cb.step() == [0]
+
+
+def test_an_open_stream_must_fit_the_session(monkeypatch):
+    """A CodecStream is taken as the session's stream when it has n_slots rows and room for a packet; anything that is
+    neither a stream nor a decoder is refused."""
+    import pytest
+    from qwen3_tts_b200.codec import CodecStream
+    from qwen3_tts_b200.scheduler import ContinuousBatcher
+    _mock_sync(monkeypatch)
+
+    class OpenStream(FakeStream, CodecStream):
+        def __init__(self, B, nmax, dec):
+            super().__init__(B, nmax, dec.log)
+            self.dec = dec
+
+    codec = FakeCodec()
+    make = lambda c: ContinuousBatcher(FakeEngine(), torch.zeros(8), SamplingParams(max_new_tokens=11), n_slots=2,  # noqa: E731
+                                       packet_frames=4, codec=c)
+    for bad, msg in ((OpenStream(3, 4, codec), "3 rows"), (OpenStream(2, 3, codec), "up to 3 frames"),
+                     (object(), "CodecDecoder or a CodecStream")):
+        with pytest.raises(ValueError, match=msg):
+            make(bad)
+    st = OpenStream(2, 8, codec)
+    cb = make(st)
+    assert cb.cstream is st and cb.codec is codec
+    cb.submit(torch.zeros(4, 8), key=0, max_frames=3)
+    assert [sorted(c) for c, _ in cb.stream()] == [[0]] and st.pos == [3, 0]

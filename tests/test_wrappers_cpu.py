@@ -167,53 +167,87 @@ def test_public_names_match_the_reference_package():
                                        "get_output_sample_rate", "get_encode_downsample_rate", "get_decode_upsample_rate"))
 
 
-def test_stream_synthesize_batches_rows_like_per_row_decoding():
-    """pipeline.TTSEngine.stream_synthesize groups rows with equal window shapes into one codec call; the packets must
-    equal what per-row decoding with the same left context yields (stub engines: a causal fake codec, ragged finish)."""
-    from types import SimpleNamespace
+def _stream_engine(monkeypatch, codec_max=64, eos_at=None):
+    """A TTSEngine over the fake engine of test_scheduler_cpu.py (row b's frame t has every code b * 100 + t) and the
+    seeding codec of test_scheduler_voice_clone_cpu.py, given a causal forward: the running sum of the codes."""
+    from qwen3_tts_b200.engine import AREngine
     from qwen3_tts_b200.pipeline import TTSEngine
-    K, up = 16, 3
-    calls = []
+    from tests.test_scheduler_cpu import FakeEngine, _mock_sync
+    from tests.test_scheduler_voice_clone_cpu import SeedingCodec, SeedingStream
+    from qwen3_tts_b200.codec import CodecStream
+    _mock_sync(monkeypatch)
 
-    class _Codec:
-        total_upsample = up
+    class _AR(FakeEngine):
+        _frame_budget = AREngine._frame_budget
 
-        def forward(self, codes):                       # (B, K, T) -> (B, 1, T*up): causal running sum, repeated `up` times
-            calls.append(tuple(codes.shape))
-            s = codes.sum(1).cumsum(-1).float()
-            return s.repeat_interleave(up, dim=-1)[:, None, :]
+    class _Stream(SeedingStream, CodecStream):
+        pass
 
-    g = torch.Generator().manual_seed(0)
-    full = [torch.randint(0, 50, (n, K), generator=g) for n in (10, 7, 10)]   # row 1 finishes early
+    class _Codec(SeedingCodec):
+        def open_stream(self, batch, max_packet_frames=8):
+            self.stream = _Stream(batch, max_packet_frames, self.log)
+            self.stream.dec = self
+            return self.stream
 
-    class _AR:
-        def stream(self, emb, tr, pad, sp, packet_frames=4):
-            for s0 in range(0, 10, packet_frames):
-                yield [f[s0:s0 + packet_frames] for f in full]
+        def forward(self, codes):                       # (B, K, T) -> (B, 1, T*up), repeated `up` times
+            self.log.append(("forward", tuple(codes.shape)))
+            return codes.sum(1).cumsum(-1).float().repeat_interleave(self.total_upsample, dim=-1)[:, None, :]
 
     eng = object.__new__(TTSEngine)
-    eng.device, eng.codec, eng.ar = torch.device("cpu"), _Codec(), _AR()
-    eng.codec_cfg = SimpleNamespace(num_quantizers=K)
-    z = [torch.zeros(1, 4)] * 3
-    for lc in (None, 2):
-        calls.clear()
+    eng.device, eng.ar, eng.codec = torch.device("cpu"), _AR(eos_at), _Codec(codec_max)
+    eng.codec_cfg = eng.codec.cfg
+    return eng
+
+
+def test_stream_synthesize_on_the_batcher_equals_per_row_decoding(monkeypatch):
+    """pipeline.TTSEngine.stream_synthesize runs the rows as one ContinuousBatcher session.  The windowed modes group
+    rows with equal window shapes into one codec call, and their packets must equal what per-row decoding with the same
+    left context yields; the stateful mode hands out each row's own frames of the codec stream (ragged finish)."""
+    from qwen3_tts_b200.config import SamplingParams
+    eng = _stream_engine(monkeypatch, eos_at={1: 7})                            # row 1 finishes early
+    up, K = eng.codec.total_upsample, eng.codec_cfg.num_quantizers
+    full = [(b * 100 + torch.arange(n))[:, None].expand(n, K) for b, n in enumerate((10, 7, 10))]
+    z = [torch.zeros(1, 8)] * 3
+    sp = SamplingParams(max_new_tokens=11)
+    for lc in (None, 2, "stateful"):
+        eng.codec.log.clear()
         parts = [[] for _ in full]
-        for pkt in eng.stream_synthesize(z, z, torch.zeros(4), None, packet_frames=4, left_context=lc):
-            assert len(pkt) == 3
+        for pkt in eng.stream_synthesize(z, z, torch.zeros(8), sp, packet_frames=4, left_context=lc):
+            assert len(pkt) == 3 and all(w.dtype == np.float32 for w in pkt)
             for b, w in enumerate(pkt):
                 parts[b].append(w)
         for b, f in enumerate(full):
             want, hist = [], 0
             for s0 in range(0, f.shape[0], 4):
                 new = f[s0:s0 + 4]
-                ctx = hist if lc is None else min(lc, hist)
-                win = torch.cat([f[hist - ctx:hist], new], 0)
-                want.append(_Codec().forward(win.t()[None])[0, 0, ctx * up:].numpy())
+                if lc == "stateful":
+                    want.append(new[:, 0].float().repeat_interleave(up).numpy())
+                else:
+                    ctx = hist if lc is None else min(lc, hist)
+                    win = torch.cat([f[hist - ctx:hist], new], 0)
+                    want.append(eng.codec.forward(win.t()[None])[0, 0, ctx * up:].numpy())
                 hist += new.shape[0]
             assert np.array_equal(np.concatenate(parts[b]), np.concatenate(want))
             assert np.concatenate(parts[b]).shape[0] == f.shape[0] * up
-    # packet 0: all three rows in one call; packet 1: rows 0 and 2 (4 new frames) + row 1 (3 new frames) = 2 calls; packet 2: 1 call
-    assert [c[0] for c in calls[:4 + 0] if True][:1] == [3]
+        if lc != "stateful":   # packet 0: all three rows in one codec call
+            assert next(e for e in eng.codec.log if e[0] == "forward")[1][0] == 3
+
+
+def test_stream_synthesize_zero_budget_and_seeded_horizon(monkeypatch):
+    """A zero-frame budget yields no packet in any mode; a seeded row's horizon leaves the codec's RoPE table room for
+    its reference (codec max_frames 12, reference of 7 frames: 5 frames), the other row runs to its budget."""
+    from qwen3_tts_b200.config import SamplingParams
+    from tests.test_scheduler_voice_clone_cpu import _ref
+    eng = _stream_engine(monkeypatch, codec_max=12)
+    z = [torch.zeros(1, 8)] * 2
+    for lc in (None, 2, "stateful"):
+        assert list(eng.stream_synthesize(z, z, torch.zeros(8), SamplingParams(max_new_tokens=1), left_context=lc)) == []
+    pkts = list(eng.stream_synthesize(z, z, torch.zeros(8), SamplingParams(max_new_tokens=11), packet_frames=4,
+                                      ref_codes=[_ref(7, 1), None]))
+    up = eng.codec.total_upsample
+    assert [sum(p[b].shape[0] for p in pkts) for b in range(2)] == [5 * up, 10 * up]
+    assert [e[0] for e in eng.codec.log[:2]] == ["reset", "seed"]
+    assert max(max(e[2]) for e in eng.codec.log if e[0] == "push") <= 12
 
 
 def test_batched_prefill_assembly_equals_per_sample_restatement():
