@@ -1,6 +1,6 @@
 // Attention phase: per-head q/k RMSNorm + RoPE, KV append, single-query GQA with cross-CTA split-K combine.
 // Part of the ar_engine.cu translation unit (include order: ar_program, ar_gemv, ar_attention, ar_sampler,
-// the persistent kernel in ar_engine.cu, ar_prefill).
+// the persistent kernel in ar_step, ar_prefill).
 #pragma once
 
 namespace {

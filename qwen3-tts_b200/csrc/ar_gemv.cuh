@@ -1,7 +1,7 @@
 // Grid barrier, mbarrier / TMA helpers, the per-warp weight ring and the GEMV phase (RMSNorm-fused activation staging,
 // batch-in-N mma.sync fed from shared memory, fused epilogues).
 // Part of the ar_engine.cu translation unit (include order: ar_program, ar_gemv, ar_attention, ar_sampler,
-// the persistent kernel in ar_engine.cu, ar_prefill).
+// the persistent kernel in ar_step, ar_prefill).
 #pragma once
 
 namespace {

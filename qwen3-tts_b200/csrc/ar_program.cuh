@@ -1,6 +1,6 @@
 // Data model of the fused frame-step kernel: tile constants, the phase descriptor, device-side state and launch parameters.
 // Part of the ar_engine.cu translation unit (include order: ar_program, ar_gemv, ar_attention, ar_sampler,
-// the persistent kernel in ar_engine.cu, ar_prefill).
+// the persistent kernel in ar_step, ar_prefill).
 #pragma once
 
 namespace {

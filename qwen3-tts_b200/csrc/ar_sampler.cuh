@@ -1,6 +1,6 @@
 // Sample phase: HF logits processors, argmax / inverse-CDF sampling with Philox uniforms, next-input embedding.
 // Part of the ar_engine.cu translation unit (include order: ar_program, ar_gemv, ar_attention, ar_sampler,
-// the persistent kernel in ar_engine.cu, ar_prefill).
+// the persistent kernel in ar_step, ar_prefill).
 #pragma once
 
 namespace {
