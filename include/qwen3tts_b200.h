@@ -142,11 +142,19 @@ int q3_sampling_check(const q3_sampling* sp);
  * frame t adds trailing[t] while t < the row's trailing length and tts_pad afterwards (modeling_qwen3_tts.py:1689-1692).
  * The capacity is the trailing stride given at q3_prefill / max_trailing of q3_session_begin. */
 int q3_append_trailing(q3_engine* e, int32_t slot, const void* rows_dev, int32_t n, void* stream);
+/* Live text: open = 1 marks a running row (admitted, not released, of a static batch or a session) whose text may
+ * still grow.  A step of an open row whose text row has not arrived (row frame >= trailing length) is HELD instead of
+ * reading tts_pad: it commits nothing, and q3_decode moves the row back onto its committed steps before it returns, so
+ * the next decode runs that step again.  An open row therefore generates exactly what it generates with the whole text
+ * given up front, however its rows arrive.  open = 0 closes the row: past its text it reads tts_pad again.  Every
+ * admission starts closed.  Refused while hidden-state capture is set (q3_decode refuses the combination too). */
+int q3_set_trailing_open(q3_engine* e, int32_t slot, int32_t open);
 /* give up rows that reached their frame horizon without EOS (their slots become free) */
 int q3_release_slots(q3_engine* e, int32_t n, const int32_t* slots_host, void* stream);
 
 /* After synchronising `stream`: frames_done = frames whose 16 codes are complete (same for all rows);
- * n_valid[b] = frames of row b before its first EOS (== modeling_qwen3_tts.py:2283-2290 trim);
+ * n_valid[b] = frames of row b before its first EOS (== modeling_qwen3_tts.py:2283-2290 trim); for a row the last
+ * decode left held, its committed frames + 1 (the held step's 16 codes are final: they do not depend on its text);
  * finished[b] = 1 once row b sampled EOS.  Host pointers (may be NULL). */
 int q3_get_progress(q3_engine* e, int32_t* frames_done, int32_t* n_valid, int32_t* finished);
 

@@ -88,7 +88,7 @@ struct q3_engine {
   // device buffers
   DevState* st = nullptr;
   StackDev talker{}, cp{};
-  bf16 *x_cp = nullptr, *past_hidden = nullptr, *h_last = nullptr;
+  bf16 *x_cp = nullptr, *past_hidden = nullptr, *past_keep = nullptr, *h_last = nullptr;
   bf16 *trailing = nullptr, *tts_pad = nullptr;
   int trailing_cap = 0;
   size_t trailing_alloc = 0;
@@ -97,6 +97,9 @@ struct q3_engine {
   int frame0[MAXB] = {0};
   unsigned int row_key[MAXB] = {0};
   bool active[MAXB] = {false};
+  // live text (q3_set_trailing_open): rows whose text may still grow, and rows whose last decode ended held at a step
+  // whose text row had not arrived (that step's code-predictor half, i.e. one more frame of codes, is done)
+  bool text_open[MAXB] = {false}, held[MAXB] = {false};
   bool session = false;       // continuous-batching session (q3_session_begin / q3_admit_with_sampling)
   unsigned int admit_mask = 0xffffffffu;
   unsigned char* seen = nullptr;
@@ -186,6 +189,7 @@ extern "C" int q3_engine_create(const q3_engine_cfg* cfg, q3_engine** out) {
   const int H = cfg->talker.hidden_size;
   if (store.alloc(&e->x_cp, (size_t)2 * MAXB * H, true)) return 1;
   if (store.alloc(&e->past_hidden, (size_t)MAXB * H, true)) return 1;
+  if (store.alloc(&e->past_keep, (size_t)MAXB * H, true)) return 1;
   if (store.alloc(&e->h_last, (size_t)MAXB * H, true)) return 1;
   if (store.alloc(&e->tts_pad, (size_t)H, true)) return 1;
   if (store.alloc(&e->seen, (size_t)MAXB * cfg->talker.vocab_size, true)) return 1;
@@ -493,8 +497,10 @@ static int launch_program(q3_engine* e, int off, int n, int mode, int max_iters,
   P.max_len0 = e->max_len0;
   for (int b = 0; b < MAXB; ++b) { P.frame0[b] = e->frame0[b]; P.row_key[b] = e->row_key[b]; }
   P.admit_mask = e->admit_mask;
+  for (int b = 0; b < e->B; ++b)
+    if (e->active[b] && e->text_open[b]) P.text_open |= 1u << b;
   P.emb_t = e->emb_t; P.emb_cp = e->emb_cp;
-  P.x_cp = e->cfg.has_cp_projection ? e->x_cp : e->cp.h; P.past_hidden = e->past_hidden; P.trailing = e->trailing; P.trailing_stride = e->trailing_cap;
+  P.x_cp = e->cfg.has_cp_projection ? e->x_cp : e->cp.h; P.past_hidden = e->past_hidden; P.past_keep = e->past_keep; P.trailing = e->trailing; P.trailing_stride = e->trailing_cap;
   if (e->proj_tab) { P.cp_next = e->proj_tab; P.cp_next_dst = e->cp.h; P.cp_next_w = e->cfg.cp.hidden_size; }
   else { P.cp_next = P.emb_cp; P.cp_next_dst = P.x_cp; P.cp_next_w = e->cfg.talker.hidden_size; }
   P.tts_pad = e->tts_pad; P.seen = e->seen; P.codes_out = codes_dev; P.codes_stride = e->codes_stride;
@@ -648,6 +654,7 @@ static int reset_rows(q3_engine* e, int B, int max_trailing, const void* tts_pad
   for (int b = 0; b < MAXB; ++b) {
     hs.finished[b] = 1; hs.len0[b] = 1;
     e->len0[b] = 1; e->frame0[b] = 0; e->row_key[b] = (unsigned int)b; e->trailing_len[b] = 0; e->active[b] = false;
+    e->text_open[b] = false; e->held[b] = false;
   }
   e->max_len0 = 1;
   Q3_CUDA(cudaMemcpyAsync(e->st, &hs, sizeof(hs), cudaMemcpyHostToDevice, stream));
@@ -667,6 +674,7 @@ static int admit_rows(q3_engine* e, const Admission& A, int F, unsigned int runn
     const int b = A.slots[r];
     e->len0[b] = A.lens[r] - F; e->frame0[b] = F; e->row_key[b] = A.keys[r]; e->trailing_len[b] = A.tl ? A.tl[r] : 0;
     e->row_sp[b] = A.sp ? A.sp[r] : e->sp;
+    e->text_open[b] = false; e->held[b] = false;  // every admission starts closed: q3_set_trailing_open opens it
     admitted |= 1u << b;
   }
   e->frames_issued = F;
@@ -751,8 +759,33 @@ extern "C" int q3_decode(q3_engine* e, int32_t max_frames, int32_t* codes_dev, i
     if (e->active[b])
       Q3_REQUIRE(e->len0[b] + e->frames_issued + max_frames <= e->cfg.max_ctx,
                  "KV capacity exceeded: row %d would reach position %d > max_ctx %d", b, e->len0[b] + e->frames_issued + max_frames, e->cfg.max_ctx);
+  for (int b = 0; b < e->B; ++b)
+    Q3_REQUIRE(!(e->active[b] && e->text_open[b] && e->hid_out), "row %d is open for live text while hidden-state capture is set", b);
+  const int F = e->frames_issued;
   e->frames_issued += max_frames;
-  return launch_program(e, e->off_frame, (int)e->prog_frame.size(), 1, max_frames, e->nt_frame, e->plan_frame, e->pt_frame, codes_dev, stream);
+  if (launch_program(e, e->off_frame, (int)e->prog_frame.size(), 1, max_frames, e->nt_frame, e->plan_frame, e->pt_frame, codes_dev, stream))
+    return 1;
+  // Live text: an open row held at step f (its row frame f >= trailing_len) stays held for the rest of the launch, so
+  // of the n steps only the first `avail` committed.  Moving its admission frame by the held steps makes its row frame
+  // (frame - frame0) and its position (len0 + frame) those of its committed steps again: the next launch runs step f
+  // anew.  A held row is not finished, so the launch ran all n steps whenever this applies.  No device state changes.
+  bool rebased = false;
+  for (int b = 0; b < e->B; ++b) {
+    e->held[b] = false;
+    if (!e->active[b] || !e->text_open[b]) continue;
+    const int avail = std::max(0, e->trailing_len[b] - (F - e->frame0[b]));
+    const int held = max_frames - std::min(max_frames, avail);
+    e->frame0[b] += held;
+    e->len0[b] -= held;
+    e->held[b] = held > 0;
+    rebased = rebased || held > 0;
+  }
+  if (rebased) {  // still the largest (prompt - frame0) of the running rows: the attention split count of the batch
+    e->max_len0 = 1;
+    for (int b = 0; b < e->B; ++b)
+      if (e->active[b]) e->max_len0 = std::max(e->max_len0, e->len0[b]);
+  }
+  return 0;
 }
 
 // Streaming TEXT input (SURVEY §8f-2): more trailing_text_hidden rows for a row that is already generating.  Frame t of a
@@ -771,6 +804,17 @@ extern "C" int q3_append_trailing(q3_engine* e, int32_t slot, const void* rows_d
   return 0;
 }
 
+// Live text (SURVEY §8f-2): while a row is open its text may still grow, and a step whose text row has not arrived is
+// held instead of reading tts_pad (see q3_decode).  Closing puts the row back on the reference's semantics.
+extern "C" int q3_set_trailing_open(q3_engine* e, int32_t slot, int32_t open) {
+  Q3_REQUIRE(e && e->B > 0, "prefill or q3_session_begin first");
+  Q3_REQUIRE(slot >= 0 && slot < e->B, "slot %d out of range", slot);
+  Q3_REQUIRE(e->active[slot], "slot %d has no running request", slot);
+  Q3_REQUIRE(!open || !e->hid_out, "live text is not available while hidden-state capture is set");
+  e->text_open[slot] = open != 0;
+  return 0;
+}
+
 extern "C" int q3_release_slots(q3_engine* e, int32_t n, const int32_t* slots_host, void* stream_) {
   Q3_REQUIRE(e && e->session && slots_host && n >= 0 && n <= MAXB, "bad argument");
   Q3_CUDA(cudaSetDevice(e->cfg.device));
@@ -780,6 +824,8 @@ extern "C" int q3_release_slots(q3_engine* e, int32_t n, const int32_t* slots_ho
     Q3_REQUIRE(slots_host[r] >= 0 && slots_host[r] < e->B, "slot %d out of range", slots_host[r]);
     A.slot[r] = slots_host[r];
     e->active[slots_host[r]] = false;
+    e->text_open[slots_host[r]] = false;
+    e->held[slots_host[r]] = false;
   }
   if (n > 0) release_state_kernel<<<1, 32, 0, (cudaStream_t)stream_>>>(e->st, A);
   return 0;
@@ -793,8 +839,9 @@ extern "C" int q3_get_progress(q3_engine* e, int32_t* frames_done, int32_t* n_va
   Q3_REQUIRE(hs.error == 0, "device-side error %d (grid barrier timeout)", hs.error);
   if (frames_done) *frames_done = hs.step;
   for (int b = 0; b < e->B; ++b) {
-    if (n_valid) n_valid[b] = hs.finished[b] ? hs.n_valid[b] : hs.step - e->frame0[b];  // the row's own frame count
-    if (hs.finished[b]) e->active[b] = false;
+    // the row's own frame count; a held row has one frame more: its held step's code-predictor half is done
+    if (n_valid) n_valid[b] = hs.finished[b] ? hs.n_valid[b] : hs.step - e->frame0[b] + (e->held[b] ? 1 : 0);
+    if (hs.finished[b]) e->active[b] = e->text_open[b] = e->held[b] = false;
     if (finished) finished[b] = hs.finished[b];
   }
   return 0;

@@ -111,6 +111,8 @@ struct KParams {
                             // the row's own frame counter is frame - frame0[b]; len0[b] is stored as prompt_len - frame0[b]
   unsigned int row_key[MAXB];  // Philox row key (the request's identity, not its slot: an admitted row samples what it would alone)
   unsigned int admit_mask;  // prefill-head program only: rows whose first token is sampled / whose hidden state is saved
+  unsigned int text_open;   // rows whose text may still grow: such a row is HELD at a step whose text row has not
+                            // arrived (row frame >= trailing_len[b]) and its talker sample commits nothing (live text)
   int trailing_len[MAXB];
   q3_sampling sp;           // sampling parameters of every row, unless row_sampling is set
   int row_sampling;         // 1: row b samples with row_sp[b] (continuous batching: per-request parameters); 0: with sp
@@ -123,6 +125,8 @@ struct KParams {
   bf16* cp_next_dst;        // where they go: cp.h (table / Identity projection) or x_cp (projection phase follows)
   int cp_next_w;            // row width of cp_next / cp_next_dst
   bf16* past_hidden;        // [B][H]
+  bf16* past_keep;          // [B][H] past_hidden as the row's last committed talker sample copied it into x_cp: a held
+                            // step puts x_cp back from it (the code predictor's passes may overwrite x_cp in place)
   const bf16* trailing;     // [B][stride][H]
   int trailing_stride;
   const bf16* tts_pad;      // [H]

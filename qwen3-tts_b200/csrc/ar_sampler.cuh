@@ -209,6 +209,19 @@ __device__ __forceinline__ void sample_phase(const Phase& ph, const KParams& P, 
   const StackDev& S = talker ? P.talker : P.cp;
   const int V = S.vocab;
   const int H = P.talker.hidden;
+  if (talker && !in_prefill && ((P.text_open >> b) & 1u) && frame >= P.trailing_len[b]) {
+    // held step (live text): this step's talker input needed trailing[frame], which has not arrived.  Nothing of the
+    // sample is committed; the code predictor's input is put back to what the last committed sample left (its passes
+    // may have run in place on it), so the step can run again, bit for bit, once the text is there.
+    const bf16* e = P.emb_t + (size_t)ldcgi(&st->c0[b]) * H;
+    const bf16* k = P.past_keep + (size_t)b * H;
+#pragma unroll 1
+    for (int i = tid * 8; i < H; i += NTHREADS * 8) {
+      *reinterpret_cast<uint4*>(P.x_cp + ((size_t)B + b) * H + i) = *reinterpret_cast<const uint4*>(e + i);
+      *reinterpret_cast<uint4*>(P.x_cp + (size_t)b * H + i) = ldcg16(k + i);
+    }
+    return;
+  }
   float* sv = reinterpret_cast<float*>(smem);       // [MAXV]
   float* pv = sv + MAXV;                            // [MAXV]
   float* red = pv + MAXV;                           // [32]
@@ -373,10 +386,13 @@ __device__ __forceinline__ void sample_phase(const Phase& ph, const KParams& P, 
     bf16* x0 = P.x_cp + (size_t)b * H;
     const bf16* e = P.emb_t + (size_t)tok * H;
     const bf16* ph_ = P.past_hidden + (size_t)b * H;
+    bf16* keep = P.past_keep ? P.past_keep + (size_t)b * H : nullptr;  // (a caller that never opens a row may leave it unset)
 #pragma unroll 1
     for (int i = tid * 8; i < H; i += NTHREADS * 8) {
       *reinterpret_cast<uint4*>(x1 + i) = *reinterpret_cast<const uint4*>(e + i);
-      *reinterpret_cast<uint4*>(x0 + i) = ldcg16(ph_ + i);
+      const uint4 v = ldcg16(ph_ + i);
+      *reinterpret_cast<uint4*>(x0 + i) = v;
+      if (keep) *reinterpret_cast<uint4*>(keep + i) = v;
     }
   } else {
     const int j = group;  // codebook index 1..G-1

@@ -194,6 +194,12 @@ class AREngine:
         stream = torch.cuda.current_stream(self.device).cuda_stream
         _lib.check(self.lib.q3_append_trailing(self.h, int(slot), r.data_ptr(), int(r.shape[0]), C.c_void_p(stream)))
 
+    def set_text_open(self, slot: int, open: bool):
+        """Live text (q3_set_trailing_open): while `slot` is open its text may still grow, and a step whose text row
+        has not arrived is held (the row waits) instead of reading tts_pad.  Closing returns the row to reading tts_pad
+        past its text.  Every admission starts closed."""
+        _lib.check(self.lib.q3_set_trailing_open(self.h, int(slot), int(bool(open))))
+
     def release_slots(self, slots: Sequence[int]):
         n = len(slots)
         stream = torch.cuda.current_stream(self.device).cuda_stream

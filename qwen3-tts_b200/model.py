@@ -257,6 +257,34 @@ class Qwen3TTSForConditionalGenerationB200:
         return embeds, trailing, tts_pad_embed.reshape(-1)
 
     @torch.no_grad()
+    def build_live_prefill(self, input_ids, instruct_ids=None, voice_clone_prompt=None, languages=None, speakers=None):
+        """Live text: the streaming-layout prefill (build_prefill with non_streaming_mode=False, :2199-2202 / :2229-2232)
+        of the text known so far.  The prefill holds the first text token; the trailing rows are the rest of the ids
+        (`ids[4:-5]`) WITHOUT the final tts_eos row, which is appended (tts_eos_row) when the text ends.  A request
+        whose later ids arrive through text_rows() and end with tts_eos_row() has exactly the prefill and trailing rows
+        of build_prefill(non_streaming_mode=False) over all its ids.  ICL voice-clone prompts are refused: their prefill
+        consumes the target text.  A text without tokens yet is refused too."""
+        vcp = voice_clone_prompt
+        for i, ids in enumerate(input_ids):
+            if int(ids.reshape(-1).shape[0]) < 9:   # 3 role tokens, >= 1 text token, 5 closing tokens
+                raise ValueError(f"request {i}: live text needs at least one text token in the prefill")
+            if vcp is not None and vcp["ref_code"] is not None and vcp["icl_mode"][i]:
+                raise ValueError(f"request {i}: an ICL voice-clone prompt cannot take live text (its prefill consumes the "
+                                 f"target text); use an x-vector-only prompt")
+        embeds, trailing, pad = self.build_prefill(input_ids, instruct_ids, None, vcp, languages, speakers, non_streaming_mode=False)
+        return embeds, [t[:-1] for t in trailing], pad
+
+    @torch.no_grad()
+    def text_rows(self, ids) -> torch.Tensor:
+        """Trailing rows (n, H) of n more text ids of a live request: text_projection(text_embedding(ids))."""
+        return self._tp(torch.as_tensor(ids, dtype=torch.long).reshape(1, -1))[0]
+
+    @torch.no_grad()
+    def tts_eos_row(self) -> torch.Tensor:
+        """The (1, H) trailing row that ends a live request's text (the last trailing row of the streaming layout)."""
+        return self.text_rows([self.cfg.tts_eos_token_id])
+
+    @torch.no_grad()
     def build_prefill_per_sample(self, input_ids, instruct_ids=None, ref_ids=None, voice_clone_prompt=None, languages=None,
                       speakers=None, non_streaming_mode=False):
         """:2068-2237 restated statement by statement (one small embedding / MLP launch per piece and per sample, as
@@ -711,6 +739,42 @@ class Qwen3TTSModel:
                                        speakers=speakers, non_streaming_mode=non_streaming_mode,
                                        **self._merge_generate_kwargs(**kwargs))
         return self._decode(codes)
+
+    # ---- live text (speaking a text while it is still being written)
+    def build_live_request(self, text, speaker=None, language=None, instruct=None, voice_clone_prompt=None):
+        """One live request for ContinuousBatcher.submit(..., text_open=True): (inputs_embeds, trailing_text,
+        tts_pad_embed) of the streaming layout for the text known so far (`text`, at least one token).  Custom voice
+        (`speaker`, optional `instruct`), voice design (`instruct`) and x-vector-only voice-clone prompts are supported;
+        an ICL prompt raises ValueError.  Feed later pieces with append_text(rid, live_text_rows(piece)) and end with
+        append_text(rid, live_text_end()) and close_text(rid).  The request then generates what the whole text's ids
+        generate up front (non_streaming_mode=False).  The guarantee is in ids: a string split into pieces may tokenise
+        differently from the whole string."""
+        if isinstance(text, list):
+            raise ValueError("build_live_request takes one text")
+        if voice_clone_prompt is not None:
+            input_ids, _, vcp, languages = self._voice_clone_inputs(text, language, None, None, False, voice_clone_prompt,
+                                                                    "build_live_request")
+            embeds, trailing, pad = self.model.build_live_prefill(input_ids, voice_clone_prompt=vcp, languages=languages)
+            return embeds[0], trailing[0], pad
+        language = "Auto" if language is None else language
+        self._validate_languages([language])
+        self._validate_speakers([speaker])
+        if self.model.tts_model_type == "custom_voice" and self.model.tts_model_size in "0b6":
+            instruct = None
+        input_ids = self._tokenize_texts([self._build_assistant_text(text)])
+        instruct_ids = [None if (instruct is None or instruct == "") else self._tokenize_texts([self._build_instruct_text(instruct)])[0]]
+        embeds, trailing, pad = self.model.build_live_prefill(input_ids, instruct_ids=instruct_ids, languages=[language],
+                                                              speakers=[speaker])
+        return embeds[0], trailing[0], pad
+
+    def live_text_rows(self, text: str) -> torch.Tensor:
+        """Trailing rows (n, H) of one more piece of a live request's text: its token ids with no chat wrapper."""
+        ids = self.processor(text=text, return_tensors="pt", padding=True)["input_ids"]
+        return self.model.text_rows(ids.reshape(-1))
+
+    def live_text_end(self) -> torch.Tensor:
+        """The (1, H) tts_eos row to append_text before close_text: it tells the model the text is over."""
+        return self.model.tts_eos_row()
 
     # ---- :636-728
     def generate_voice_design(self, text, instruct, language=None, non_streaming_mode=True, **kwargs):

@@ -26,6 +26,15 @@ generated codes) and cuts the reference's audio off (qwen3_tts_model.py:612-631)
 with the reference as their causal left context.  At admission such a slot's codec row is seeded with its reference
 (CodecStream.seed, one call for all seeded slots of the admission) instead of reset; its chunks and `done` entry hold
 the generated part only (tests/test_gpu_scheduler_voice_clone.py).
+
+Live text (`submit(text_open=True)`, `append_text`, `close_text`): a request's text may keep arriving after submit, as
+when speaking an LLM's answer while it is being written.  Its slot is open in the engine (AREngine.set_text_open): a
+frame-step whose text row has not arrived holds the row instead of reading tts_pad, so the request generates exactly
+what it generates with the whole text given up front (tests/test_gpu_live_text.py).  A step launches only when it
+admits a request or some running row can produce a frame: a closed row always can, an open row when its text reaches
+the frames it has reported.  Otherwise the step launches nothing and returns no frames, and `stream()` / `packets()`
+yield empty results, so a single-threaded caller feeds text between iterations.  `cancel` drops a request, pending or
+running (a client that disconnected).
 """
 from collections import deque
 from dataclasses import dataclass, field
@@ -47,6 +56,9 @@ class _Request:
     max_frames: int
     sampling: Optional[SamplingParams] = None
     ref_codes: Optional[torch.Tensor] = None
+    text_open: bool = False    # submitted with text that may still grow
+    closed: bool = False       # close_text() was called
+    n_text: int = 0            # trailing rows given so far
     slot: int = -1
     emitted: int = 0
     chunks: List[torch.Tensor] = field(default_factory=list)
@@ -66,6 +78,7 @@ class ContinuousBatcher:
         self.running: Dict[int, _Request] = {}     # slot -> request
         self.done: Dict[int, torch.Tensor] = {}
         self._next_id = 0
+        self._cancelled = set()
         self.max_trailing = int(max_trailing)
         engine.session_begin(self.n_slots, tts_pad_embed, sp, max_trailing=self.max_trailing)
         self.frames_total = 0
@@ -83,12 +96,14 @@ class ContinuousBatcher:
     # ------------------------------------------------------------------ API
     def submit(self, inputs_embeds: torch.Tensor, trailing_text: Optional[torch.Tensor] = None, key: Optional[int] = None,
                max_frames: Optional[int] = None, sampling: Optional[SamplingParams] = None,
-               ref_codes: Optional[torch.Tensor] = None) -> int:
+               ref_codes: Optional[torch.Tensor] = None, text_open: bool = False) -> int:
         """Queue one request; returns its id (also its Philox row key unless `key` is given).  `sampling`: the
         request's own generation parameters (default: the session's); its max_new_tokens bounds the request's horizon
         and may not exceed the session's.  `ref_codes`: (L, num_quantizers) reference codes of a voice-clone request
         (VoiceClonePromptItem.ref_code); its audio is decoded after them, and the horizon leaves the codec's RoPE
-        table room for them.  Bad parameters raise ValueError here, never in a later step()."""
+        table room for them.  `text_open`: the request's text may grow after submit (append_text, then close_text);
+        until it is closed the request waits for text instead of reading tts_pad past its end.  Bad parameters raise
+        ValueError here, never in a later step()."""
         H = self.eng.cfg.talker.hidden_size
         L_ref = 0
         if ref_codes is not None:
@@ -115,8 +130,64 @@ class ContinuousBatcher:
         horizon = min(limit if max_frames is None else max_frames, limit, room)
         if self.codec is not None:
             horizon = min(horizon, self.codec.max_frames - L_ref)  # a codec row's position may not pass its RoPE table
-        self.pending.append(_Request(rid, inputs_embeds, tr, horizon, sampling, ref_codes))
+        self.pending.append(_Request(rid, inputs_embeds, tr, horizon, sampling, ref_codes, text_open=bool(text_open),
+                                     n_text=int(tr.reshape(-1, H).shape[0])))
         return rid
+
+    def _live(self, rid: int, what: str) -> _Request:
+        """The pending or running request `rid` whose text is still open, else ValueError."""
+        r = next((q for q in self.pending if q.rid == rid), None) or next((q for q in self.running.values() if q.rid == rid), None)
+        if r is None:
+            state = "was cancelled" if rid in self._cancelled else "has finished" if rid in self.done else "is unknown"
+            raise ValueError(f"{what}: request {rid} {state}")
+        if not r.text_open:
+            raise ValueError(f"{what}: request {rid} was not submitted with text_open=True")
+        if r.closed:
+            raise ValueError(f"{what}: the text of request {rid} is already closed")
+        return r
+
+    def append_text(self, rid: int, rows: torch.Tensor):
+        """More trailing text rows (n, H) for an open request, pending or running (Qwen3TTSModel.live_text_rows makes
+        them from a piece of text).  ValueError for an unknown, finished or cancelled request, one that was not
+        submitted open or is already closed, or text beyond max_trailing."""
+        r = self._live(rid, "append_text")
+        H = self.eng.cfg.talker.hidden_size
+        rows = rows.reshape(-1, H)
+        if r.n_text + rows.shape[0] > self.max_trailing:
+            raise ValueError(f"append_text: request {rid} would have {r.n_text + rows.shape[0]} trailing rows, more than "
+                             f"max_trailing={self.max_trailing}")
+        if rows.shape[0] == 0:
+            return
+        if r.slot >= 0:
+            self.eng.append_trailing(r.slot, rows)
+        else:
+            r.trailing = torch.cat([r.trailing.reshape(-1, H).to(rows.device, rows.dtype), rows], 0)
+        r.n_text += int(rows.shape[0])
+
+    def close_text(self, rid: int):
+        """No more text is coming for `rid` (append Qwen3TTSModel.live_text_end() first): past its text the request
+        reads tts_pad and ends.  ValueError as for append_text."""
+        r = self._live(rid, "close_text")
+        r.closed = True
+        if r.slot >= 0:
+            self.eng.set_text_open(r.slot, False)
+
+    def cancel(self, rid: int) -> bool:
+        """Drop request `rid`: a pending one leaves the queue, a running one's slot is released (its codec row is reset
+        at the slot's next admission).  It gets no `done` entry.  False when there is no such pending or running
+        request."""
+        for r in self.pending:
+            if r.rid == rid:
+                self.pending.remove(r)
+                self._cancelled.add(rid)
+                return True
+        for slot, r in self.running.items():
+            if r.rid == rid:
+                self.eng.release_slots([slot])
+                del self.running[slot]
+                self._cancelled.add(rid)
+                return True
+        return False
 
     def step(self) -> List[int]:
         """Admit what fits, decode one packet, collect what finished.  Returns the ids that completed in this step."""
@@ -142,6 +213,12 @@ class ContinuousBatcher:
             new, finished = self._advance()
             yield {r.rid: self.codes[slot, e0:e0 + k].to(torch.int64) for slot, (r, e0, k) in new.items() if k > 0}, finished
 
+    def _runnable(self) -> bool:
+        """Some running row can produce a frame in the next launch: a closed row always can; an open row when its
+        text covers the frames it has reported (the step after them has its text row, or is the one held step that
+        completes one more frame)."""
+        return any(not r.text_open or r.closed or r.n_text >= r.emitted for r in self.running.values())
+
     def _advance(self):
         """One step of the session: ({slot: (request, first new frame, new frames)}, [ids that finished])."""
         free = [s for s in range(self.n_slots) if s not in self.running]
@@ -158,14 +235,16 @@ class ContinuousBatcher:
                 self.eng.admit(*args)
             for r in batch:
                 self.running[r.slot] = r
+                if r.text_open and not r.closed:
+                    self.eng.set_text_open(r.slot, True)
             if self.cstream is not None:
                 seeded = [r for r in batch if r.ref_codes is not None]
                 if len(seeded) < len(batch):
                     self.cstream.reset([r.slot for r in batch if r.ref_codes is None])
                 if seeded:
                     self.cstream.seed([r.slot for r in seeded], [r.ref_codes for r in seeded])
-        if not self.running:
-            return {}, []
+        if not batch and not self._runnable():
+            return {}, []   # every running row is open and waiting for text: launch nothing
         n = min([self.packet] + [r.max_frames - r.emitted for r in self.running.values()])
         self.eng.decode(max(n, 1), self.codes)
         torch.cuda.current_stream(self.eng.device).synchronize()
@@ -205,7 +284,11 @@ class ContinuousBatcher:
         return {r.rid: wav[slot, :k * up] for slot, (r, _, k) in new.items() if k > 0}
 
     def run(self) -> Dict[int, torch.Tensor]:
-        """Drain the queue; returns {request id: (N_i, G) codes}."""
+        """Drain the queue; returns {request id: (N_i, G) codes}.  Requests with open text must be closed first (or
+        be fed through step() / stream() / packets()): run() raises ValueError when every running request waits for
+        text."""
         while self.pending or self.running:
+            if not self._runnable() and not (self.pending and len(self.running) < self.n_slots):
+                raise ValueError("every running request waits for text: close_text() them, or feed them between step()s")
             self.step()
         return self.done

@@ -12,8 +12,13 @@ by those frames, as an ICL voice-clone prompt is: its codec row is seeded with t
 (CodecStream.seed).  The probe then also reports the seed time per admission, the first-chunk times of voice-clone and
 plain requests apart, and, for comparison in the same run, the time to push one reference through an n_slots-row
 stream of the session's packet size, which is what seeding through the session's own stream would stall it for.
+With --live-text TOKENS_PER_S every request is live (submit(text_open=True)): its prompt holds the first text token,
+and its other text rows (horizon // 3 of them, then tts_eos) are appended between steps at that rate from its submit
+time, after which it is closed.  The probe then also reports the share of row-steps held (the host's count of the
+engine's hold rule); first_chunk_ms is then the time from the first text token to the first audio chunk.
 
     python tools/serve_probe.py [--slots 8 32] [--requests-per-slot 3] [--packet 4] [--mix] [--voice-clone]
+                                [--live-text TOKENS_PER_S]
 
 Prints one JSON line.  Writes nothing.
 """
@@ -56,9 +61,10 @@ def mixed_sampling(sp, i):
     return None
 
 
-def run_session(eng, codec, pad, sp, prompts, n_slots, packet, horizons, timed, mix=False, refs=None):
+def run_session(eng, codec, pad, sp, prompts, n_slots, packet, horizons, timed, mix=False, refs=None, live=None, texts=None):
     """One session: n_slots requests at once, then one more per step until all are in.  refs[i]: request i's
-    reference codes or None.  Returns the measurements."""
+    reference codes or None.  live: text rows per second (texts[i]: request i's rows after the first token, tts_eos
+    last), or None.  Returns the measurements."""
     from qwen3_tts_b200.scheduler import ContinuousBatcher
     cb = ContinuousBatcher(eng, pad, sp, n_slots=n_slots, packet_frames=packet, codec=codec)
     t_ar, t_codec, t_seed = [], [], []
@@ -74,17 +80,52 @@ def run_session(eng, codec, pad, sp, prompts, n_slots, packet, horizons, timed, 
             return r
         return call
 
+    held = [0, 0]     # row-steps held, row-steps run (live text)
+    committed = {}    # request id -> steps committed, by the engine's hold rule
+
+    def count_holds(fn):
+        def call(n, codes):
+            for r in cb.running.values():
+                c = committed.get(r.rid, 0)
+                k = n if r.closed else min(n, max(0, r.n_text - c))
+                committed[r.rid] = c + k
+                held[0] += n - k
+                held[1] += n
+            return fn(n, codes)
+        return call
+
+    decode = type(eng).decode.__get__(eng)
     if timed:
-        eng.decode = clocked(type(eng).decode.__get__(eng), t_ar)
+        decode = clocked(decode, t_ar)
+    if live:
+        decode = count_holds(decode)
+    if timed or live:
+        eng.decode = decode
         cb.cstream.push = clocked(cb.cstream.push, t_codec)
         cb.cstream.seed = clocked(cb.cstream.seed, t_seed)
     submitted, first, samples = {}, {}, 0
     todo = list(range(len(prompts)))
+    fed = {}
 
     def submit(i):
-        rid = cb.submit(prompts[i], None, key=i, max_frames=horizons[i % len(horizons)],
-                        sampling=mixed_sampling(sp, i) if mix else None, ref_codes=refs[i])
+        rid = cb.submit(prompts[i], texts[i][:0] if live else None, key=i, max_frames=horizons[i % len(horizons)],
+                        sampling=mixed_sampling(sp, i) if mix else None, ref_codes=refs[i], text_open=bool(live))
         submitted[rid] = time.perf_counter()
+        if live:
+            fed[rid] = 0
+
+    def feed(now):
+        for rid in list(fed):
+            if rid in cb.done:
+                del fed[rid]
+                continue
+            due = min(int((now - submitted[rid]) * live), texts[rid].shape[0])
+            if due > fed[rid]:
+                cb.append_text(rid, texts[rid][fed[rid]:due])
+                fed[rid] = due
+            if fed[rid] == texts[rid].shape[0]:
+                cb.close_text(rid)
+                del fed[rid]
 
     for i in todo[:n_slots]:
         submit(i)
@@ -98,8 +139,10 @@ def run_session(eng, codec, pad, sp, prompts, n_slots, packet, horizons, timed, 
                 samples += a.shape[0]
             if todo:
                 submit(todo.pop(0))
+            if live:
+                feed(time.perf_counter())
     finally:
-        if timed:
+        if timed or live:
             del eng.decode
         cb.cstream.close()
     wall = time.perf_counter() - t0
@@ -107,6 +150,8 @@ def run_session(eng, codec, pad, sp, prompts, n_slots, packet, horizons, timed, 
     out = {"requests": len(prompts), "steps": len(t_ar), "ar_ms_per_step": ms(t_ar), "codec_ms_per_step": ms(t_codec),
            "first_chunk_ms": ms(list(first.values())), "audio_s": samples / SAMPLE_RATE, "wall_s": wall,
            "audio_s_per_wall_s": samples / SAMPLE_RATE / wall}
+    if live:
+        out["held_row_step_share"] = held[0] / max(held[1], 1)
     if any(r is not None for r in refs):
         out["first_chunk_ms_voice_clone"] = ms([t for rid, t in first.items() if refs[rid] is not None])
         out["first_chunk_ms_plain"] = ms([t for rid, t in first.items() if refs[rid] is None])
@@ -148,6 +193,8 @@ def main():
     ap.add_argument("--mix", action="store_true", help="per-request parameters: 1/4 top-p 0.8, 1/4 greedy, the rest the session's")
     ap.add_argument("--voice-clone", action="store_true",
                     help=f"every second request carries a {REF_FRAMES}-frame reference and a prompt longer by it")
+    ap.add_argument("--live-text", type=float, default=None, metavar="TOKENS_PER_S",
+                    help="every request is live: its text rows arrive at this rate after submit")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("serve_probe needs a CUDA device")
@@ -171,6 +218,9 @@ def main():
                    f"{args.packet}-frame packets, horizons {list(HORIZONS)} frames, n_slots requests at once then one "
                    "more per step", "sampling": "mixed: 1/4 top-p 0.8, 1/4 greedy, 1/2 session (top-k 50, T 0.9)" if args.mix
            else "uniform: top-k 50, T 0.9", "card": card(), "results": {}}
+    if args.live_text:
+        out["live_text"] = (f"every request live: {args.live_text:g} text tokens/s from submit, horizon // 3 tokens "
+                            "after the first, then tts_eos and close")
     if args.voice_clone:
         out["voice_clone"] = (f"every second request: {REF_FRAMES}-frame reference of random valid codes, prompt "
                               f"{args.prompt_len + REF_FRAMES} positions instead of {args.prompt_len}")
@@ -180,9 +230,12 @@ def main():
                 if args.voice_clone and i % 2 == 1 else None for i in range(n_req)]
         prompts = [(torch.randn(args.prompt_len + (0 if r is None else REF_FRAMES), H, generator=g) * 0.5).bfloat16()
                    for r in refs]
+        texts = [torch.cat([(torch.randn(HORIZONS[i % len(HORIZONS)] // 3, H, generator=g) * 0.1).bfloat16(),
+                            (torch.randn(1, H, generator=g) * 0.1).bfloat16()]) for i in range(n_req)] if args.live_text else None
         run_session(eng, codec, pad, sp, prompts[:S], S, args.packet, (8,), timed=False, mix=args.mix,
-                    refs=refs[:S])   # warm-up: every shape
-        res = run_session(eng, codec, pad, sp, prompts, S, args.packet, HORIZONS, timed=True, mix=args.mix, refs=refs)
+                    refs=refs[:S], live=args.live_text, texts=texts)   # warm-up: every shape
+        res = run_session(eng, codec, pad, sp, prompts, S, args.packet, HORIZONS, timed=True, mix=args.mix, refs=refs,
+                          live=args.live_text, texts=texts)
         if args.voice_clone:
             res["naive_push_ms_per_admission"] = naive_seed_ms(codec, S, args.packet, refs[1])
         out["results"][f"n_slots={S}"] = res
