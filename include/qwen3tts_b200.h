@@ -294,6 +294,36 @@ int q3_codec_enc_last_launch_count(q3_codec_enc* e);
  * transformer layer, downsample) of the next encode into dst; stage < 0 clears all captures. */
 int q3_codec_enc_debug_capture(q3_codec_enc* e, int32_t stage, float* dst_dev, int64_t capacity);
 
+/* ---- stateful streaming encoder.  The encoder is causal (causal convolutions, a causal sliding-window transformer,
+ * a causal stride-2 downsample), so whole 1920-sample frames can be encoded as they arrive: this handle carries each
+ * row's causal state (the conv tails, the transformer's residual stream tail for the downsample, window - 1 columns of
+ * rotated K and V per transformer layer) and runs the one-shot's kernels over only the new frames.  The codes of a clip
+ * pushed in packets of any sizes and ended with finish_rows equal q3_codec_enc_encode of that clip alone (B = 1) bit
+ * for bit.  Only the clip's final partial frame needs the clip's end: the one-shot pads every layer on the right, which
+ * is not the same as encoding zero audio, so finish_rows encodes it on its own path.
+ * open: B rows (<= Q3_MAX_BATCH), packets of <= max_packet_frames frames.  A row's 25 Hz position (2 x its 12.5 Hz
+ * frames since reset) may not pass the encoder's max_frames (RoPE table), as in the one-shot.
+ * step_rows: wav_dev fp32 [B][n * hop]; row b takes its first counts_host[b] frames (0..n, host int32 [B]);
+ *   codes_dev int32 [B][num_quantizers][n], row b's codes past counts_host[b] are -1.  Samples past a row's count are
+ *   never read.  A row with count 0 keeps its state and position.  Asynchronous on `stream`, no host sync.
+ * finish_rows: for i < n, row rows_host[i] ends its clip with tail_host[i] (0..hop-1) samples at wav_dev[i][0..tail)
+ *   (wav_dev fp32 [n][hop]); codes_dev int32 [n][num_quantizers] = its last frame (-1 when the tail is 0).  The row is
+ *   then reset.  Asynchronous.
+ * reset_rows: the n rows in rows_host (host int32, each in [0, B), no repeats) start new clips at position 0.
+ * row_position: 12.5 Hz frames encoded for one row since its reset (-1 for a bad row).
+ * Bad arguments (a count outside [0, n], n > max_packet_frames, a tail outside [0, hop), a row out of range or listed
+ * twice, null pointers, a row whose 25 Hz position would pass max_frames) are rejected with an error naming the row
+ * before any device work, and leave every position unchanged. */
+typedef struct q3_codec_enc_stream q3_codec_enc_stream;
+int q3_codec_enc_stream_open(q3_codec_enc* e, int32_t B, int32_t max_packet_frames, q3_codec_enc_stream** out);
+int q3_codec_enc_stream_step_rows(q3_codec_enc_stream* s, const float* wav_dev, int32_t n, const int32_t* counts_host,
+                                  int32_t* codes_dev, void* stream);
+int q3_codec_enc_stream_finish_rows(q3_codec_enc_stream* s, int32_t n, const int32_t* rows_host, const int32_t* tail_host,
+                                    const float* wav_dev, int32_t* codes_dev, void* stream);
+int q3_codec_enc_stream_reset_rows(q3_codec_enc_stream* s, int32_t n, const int32_t* rows_host, void* stream);
+int q3_codec_enc_stream_row_position(q3_codec_enc_stream* s, int32_t row);
+void q3_codec_enc_stream_close(q3_codec_enc_stream* s);
+
 /* ---------------------------------------------------------------- speaker x-vector (voice cloning)
  * Replaces Qwen3TTSForConditionalGeneration.extract_speaker_embedding (core/models/modeling_qwen3_tts.py:1941-1954):
  * mel_spectrogram (:396-448) + Qwen3TTSSpeakerEncoder.forward (:371-393).  fp32. */

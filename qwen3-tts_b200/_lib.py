@@ -71,6 +71,8 @@ CODEC_SYMBOLS = ["q3_codec_create", "q3_codec_destroy", "q3_codec_load_tensor", 
                  "q3_codec_enc_create", "q3_codec_enc_destroy", "q3_codec_enc_load_tensor", "q3_codec_enc_finalize",
                  "q3_codec_enc_encode", "q3_codec_enc_frames", "q3_codec_enc_hop", "q3_codec_enc_last_launch_count",
                  "q3_codec_enc_debug_capture",
+                 "q3_codec_enc_stream_open", "q3_codec_enc_stream_step_rows", "q3_codec_enc_stream_finish_rows",
+                 "q3_codec_enc_stream_reset_rows", "q3_codec_enc_stream_row_position", "q3_codec_enc_stream_close",
                  "q3_spk_create", "q3_spk_destroy", "q3_spk_load_tensor", "q3_spk_finalize", "q3_spk_frames", "q3_spk_mel",
                  "q3_spk_embed", "q3_spk_last_launch_count"]
 
@@ -150,6 +152,13 @@ def load():
         lib.q3_codec_enc_hop.argtypes = [vp]
         lib.q3_codec_enc_last_launch_count.argtypes = [vp]
         lib.q3_codec_enc_debug_capture.argtypes = [vp, i32, vp, i64]
+        lib.q3_codec_enc_stream_open.argtypes = [vp, i32, i32, C.POINTER(vp)]
+        lib.q3_codec_enc_stream_step_rows.argtypes = [vp, vp, i32, C.POINTER(i32), vp, vp]
+        lib.q3_codec_enc_stream_finish_rows.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(i32), vp, vp, vp]
+        lib.q3_codec_enc_stream_reset_rows.argtypes = [vp, i32, C.POINTER(i32), vp]
+        lib.q3_codec_enc_stream_row_position.argtypes = [vp, i32]
+        lib.q3_codec_enc_stream_close.argtypes = [vp]
+        lib.q3_codec_enc_stream_close.restype = None
         lib.q3_spk_create.argtypes = [C.POINTER(SpkCfg), C.POINTER(vp)]
         lib.q3_spk_destroy.argtypes = [vp]
         lib.q3_spk_destroy.restype = None

@@ -12,8 +12,9 @@ encoder's output is discrete, see csrc/codec_encoder.cu.  Engine-native tensors 
   rvq.<q>.e = embed_sum / clamp(cluster_usage, 1e-5) [K][D], .et = its transpose, .e2 = squared norms
 """
 import ctypes as C
-from typing import Dict, List
+from typing import Dict, List, Tuple
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -144,6 +145,11 @@ class CodecEncoder:
     def last_launches(self) -> int:
         return self.lib.q3_codec_enc_last_launch_count(self.h)
 
+    def open_stream(self, batch: int, max_packet_frames: int = 8) -> "EncoderStream":
+        """A streaming encoder of `batch` rows (see EncoderStream): codes come back as each 1920-sample frame completes,
+        and a clip ended with end() has exactly the codes of forward() on that clip alone."""
+        return EncoderStream(self, batch, max_packet_frames)
+
     def forward_with_stages(self, wav: torch.Tensor):
         """Test helper: one forward that also returns every stage activation (name -> (B, C, T) fp32)."""
         wav = wav.to(self.device, torch.float32).contiguous()
@@ -167,3 +173,145 @@ class CodecEncoder:
         torch.cuda.current_stream(self.device).synchronize()
         _lib.check(self.lib.q3_codec_enc_debug_capture(self.h, -1, None, 0))
         return codes, dict(zip(self.stage_names, bufs))
+
+
+# ---------------------------------------------------------------------------------------------- streaming encoder
+def split_frames(buffered: int, new: int, hop: int) -> Tuple[int, int]:
+    """`buffered` samples held back plus `new` ones -> (whole frames ready to encode, samples left over, < hop)."""
+    total = int(buffered) + int(new)
+    return total // hop, total % hop
+
+
+def check_chunks(chunks: Dict, batch: int) -> Dict[int, torch.Tensor]:
+    """Validate push() input before any native call: {row: 1-D finite samples} with rows in [0, batch).  Returns the
+    chunks as fp32 CPU-or-device tensors (numpy arrays are converted)."""
+    if not isinstance(chunks, dict):
+        raise ValueError("push expects a dict {row: 1-D samples}")
+    out = {}
+    for row, x in chunks.items():
+        if isinstance(row, bool) or not isinstance(row, (int, np.integer)) or not 0 <= int(row) < batch:
+            raise ValueError(f"row {row!r} is not a row of this stream (0..{batch - 1})")
+        t = torch.from_numpy(np.ascontiguousarray(x)) if isinstance(x, np.ndarray) else x
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f"row {row}: samples must be a numpy array or a torch tensor, got {type(x).__name__}")
+        if t.dim() != 1:
+            raise ValueError(f"row {row}: expected 1-D samples, got shape {tuple(t.shape)}")
+        if not (t.is_floating_point() or t.numel() == 0):
+            raise ValueError(f"row {row}: expected floating-point samples, got {t.dtype}")
+        t = t.to(torch.float32)
+        if not bool(torch.isfinite(t).all()):
+            raise ValueError(f"row {row}: samples are not all finite")
+        out[int(row)] = t
+    return out
+
+
+def check_rows(rows, batch: int) -> List[int]:
+    rows = [rows] if isinstance(rows, (int, np.integer)) else list(rows)
+    for r in rows:
+        if isinstance(r, bool) or not isinstance(r, (int, np.integer)) or not 0 <= int(r) < batch:
+            raise ValueError(f"row {r!r} is not a row of this stream (0..{batch - 1})")
+    if len(set(int(r) for r in rows)) != len(rows):
+        raise ValueError(f"rows listed twice: {rows}")
+    return [int(r) for r in rows]
+
+
+class EncoderStream:
+    """Stateful streaming encoder over `batch` rows (q3_codec_enc_stream_*).  push({row: samples}) takes chunks of any
+    length at the encoder's input rate, holds back each row's partial frame, encodes every completed frame in packets of
+    at most `max_packet_frames` and returns {row: LongTensor (n_i, nq)} for the frames this push completed.  end(rows)
+    encodes each row's held-back partial frame exactly as the one-shot encoder pads a clip's end and returns its
+    (0 or 1, nq) codes; the rows then start new clips.  The concatenation of a clip's pushes and its end equals
+    CodecEncoder.forward of the whole clip alone, bit for bit."""
+
+    def __init__(self, enc: CodecEncoder, batch: int, max_packet_frames: int = 8):
+        self.enc, self.lib = enc, enc.lib
+        self.batch, self.max_packet_frames = int(batch), int(max_packet_frames)
+        self.hop, self.nq = enc.hop, enc.cfg.valid_num_quantizers
+        self.device = enc.device
+        h = C.c_void_p()
+        _lib.check(self.lib.q3_codec_enc_stream_open(enc.h, self.batch, self.max_packet_frames, C.byref(h)))
+        self.h = h
+        self._pending = [torch.zeros(0, dtype=torch.float32, device=self.device) for _ in range(self.batch)]
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.q3_codec_enc_stream_close(self.h)
+            self.h = None
+
+    def _stream(self):
+        if not self.h:
+            raise RuntimeError("encoder stream is closed")
+        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    @property
+    def positions(self) -> List[int]:
+        """12.5 Hz frames encoded per row since its reset (held-back samples not counted)."""
+        return [self.lib.q3_codec_enc_stream_row_position(self.h, b) for b in range(self.batch)]
+
+    def push(self, chunks: Dict) -> Dict[int, torch.Tensor]:
+        chunks = check_chunks(chunks, self.batch)
+        st = self._stream()
+        todo, frames = {}, {}
+        for b, x in chunks.items():
+            n, _ = split_frames(self._pending[b].numel(), x.numel(), self.hop)
+            todo[b] = torch.cat([self._pending[b], x.to(self.device)])
+            frames[b] = n
+        pos, ds = self.positions, self.enc.cfg.downsample_stride
+        for b, n in frames.items():
+            if (pos[b] + n) * ds > self.enc.max_frames:
+                raise ValueError(f"row {b}: 25 Hz position {pos[b] * ds} + {n * ds} frames exceeds the encoder's "
+                                 f"max_frames {self.enc.max_frames}")
+        out = {b: [] for b in chunks}
+        done = {b: 0 for b in chunks}
+        while any(done[b] < frames[b] for b in chunks):
+            n = min(self.max_packet_frames, max(frames[b] - done[b] for b in chunks))
+            counts = (C.c_int32 * self.batch)()
+            wav = torch.zeros(self.batch, n * self.hop, dtype=torch.float32, device=self.device)
+            for b in chunks:
+                k = min(n, frames[b] - done[b])
+                counts[b] = k
+                wav[b, : k * self.hop] = todo[b][done[b] * self.hop: (done[b] + k) * self.hop]
+            codes = torch.empty(self.batch, self.nq, n, dtype=torch.int32, device=self.device)
+            _lib.check(self.lib.q3_codec_enc_stream_step_rows(self.h, wav.data_ptr(), n, counts, codes.data_ptr(), st))
+            for b in chunks:
+                if counts[b]:
+                    out[b].append(codes[b, :, : counts[b]].transpose(0, 1))
+                done[b] += counts[b]
+        for b in chunks:
+            self._pending[b] = todo[b][frames[b] * self.hop:].clone()
+        return {b: (torch.cat(v).long() if v else torch.zeros(0, self.nq, dtype=torch.long, device=self.device))
+                for b, v in out.items()}
+
+    def end(self, rows) -> Dict[int, torch.Tensor]:
+        """Encode each row's held-back partial frame (the clip's last frame) and start new clips on these rows."""
+        rows = check_rows(rows, self.batch)
+        if not rows:
+            return {}
+        st = self._stream()
+        n = len(rows)
+        wav = torch.zeros(n, self.hop, dtype=torch.float32, device=self.device)
+        tails = (C.c_int32 * n)()
+        for i, b in enumerate(rows):
+            tails[i] = self._pending[b].numel()
+            wav[i, : tails[i]] = self._pending[b]
+        codes = torch.empty(n, self.nq, dtype=torch.int32, device=self.device)
+        _lib.check(self.lib.q3_codec_enc_stream_finish_rows(self.h, n, (C.c_int32 * n)(*rows), tails, wav.data_ptr(),
+                                                            codes.data_ptr(), st))
+        for b in rows:
+            self._pending[b] = self._pending[b][:0]
+        return {b: codes[i: i + 1].long() if tails[i] else codes[i: i].long() for i, b in enumerate(rows)}
+
+    def reset(self, rows):
+        """Drop the rows' clips (state and held-back samples); they start new clips at position 0."""
+        rows = check_rows(rows, self.batch)
+        if not rows:
+            return
+        _lib.check(self.lib.q3_codec_enc_stream_reset_rows(self.h, len(rows), (C.c_int32 * len(rows))(*rows), self._stream()))
+        for b in rows:
+            self._pending[b] = self._pending[b][:0]

@@ -12,7 +12,7 @@ __device__ __forceinline__ float elu1(float v) { return v > 0.f ? v : expm1f(v);
 __device__ __forceinline__ float gelu_erf(float v) { return 0.5f * v * (1.f + erff(v * 0.70710678118654752440f)); }
 
 // block = 256 threads = 16 (channel groups of 4) x 16 (time lanes; each owns t = lane + 16*i, i < 4)
-__global__ void __launch_bounds__(256) conv_f32_kernel(const ConvF32Args a) {
+__global__ void __launch_bounds__(256) conv_f32_kernel(const ConvF32Args a, const int xT, const int yT) {
   extern __shared__ float sm[];
   const int XW = (TT - 1) * a.stride + (a.k - 1) * a.dil + 1;
   float* xs = sm;                 // [CI][XW]
@@ -20,8 +20,8 @@ __global__ void __launch_bounds__(256) conv_f32_kernel(const ConvF32Args a) {
   const int b = blockIdx.z, co0 = blockIdx.y * CT, t0 = blockIdx.x * TT;
   const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
   const int in0 = t0 * a.stride - a.pad_left;  // input index of xs[.][0]
-  const float* xb = a.x + ((size_t)b * a.xC + a.x_off) * a.Tin;
-  const float* x2b = a.x2 ? a.x2 + ((size_t)b * a.x2C + a.x2_off) * a.Tin : nullptr;
+  const float* xb = a.x + ((size_t)b * a.xC + a.x_off) * xT;
+  const float* x2b = a.x2 ? a.x2 + ((size_t)b * a.x2C + a.x2_off) * xT : nullptr;
   float acc[4][4];
 #pragma unroll
   for (int i = 0; i < 4; ++i)
@@ -39,8 +39,8 @@ __global__ void __launch_bounds__(256) conv_f32_kernel(const ConvF32Args a) {
         if (a.pad == PAD_REPLICATE) ti = min(max(ti, 0), a.Tin - 1);
         else if (a.pad == PAD_REFLECT) ti = reflect_idx(ti, a.Tin);
         if (ti >= 0 && ti < a.Tin) {
-          v = xb[(size_t)(c0 + ci) * a.Tin + ti];
-          if (x2b) v += x2b[(size_t)(c0 + ci) * a.Tin + ti];
+          v = xb[(size_t)(c0 + ci) * xT + ti];
+          if (x2b) v += x2b[(size_t)(c0 + ci) * xT + ti];
           if (a.act_in == IN_ELU) v = elu1(v);
           else if (a.act_in == IN_TANH) v = tanhf(v);
         }
@@ -85,7 +85,7 @@ __global__ void __launch_bounds__(256) conv_f32_kernel(const ConvF32Args a) {
       if (a.act_out == OUT_GELU) v = gelu_erf(v);
       else if (a.act_out == OUT_RELU) v = fmaxf(v, 0.f);
       else if (a.act_out == OUT_SIGMOID) v = 1.f / (1.f + expf(-v));
-      const size_t o = ((size_t)b * a.yC + a.y_off + co) * a.Tout + t;
+      const size_t o = ((size_t)b * a.yC + a.y_off + co) * yT + t;
       if (a.scale) v = sc * v;
       if (a.res) v = a.res[o] + v;
       a.y[o] = v;
@@ -100,11 +100,11 @@ int conv_f32_init() {
   return 0;
 }
 
-int conv_f32_launch(const ConvF32Args& a, int B, cudaStream_t stream) {
+int conv_f32_launch(const ConvF32Args& a, int B, cudaStream_t stream, int xT, int yT) {
   const int XW = (TT - 1) * a.stride + (a.k - 1) * a.dil + 1;
   const size_t smem = (size_t)(CI * XW + CT * CI * a.k) * sizeof(float);
   Q3_REQUIRE(smem <= kMaxSmem, "conv tile needs %zu B of shared memory", smem);
   dim3 grid((a.Tout + TT - 1) / TT, (a.Cout + CT - 1) / CT, B);
-  conv_f32_kernel<<<grid, 256, smem, stream>>>(a);
+  conv_f32_kernel<<<grid, 256, smem, stream>>>(a, xT ? xT : a.Tin, yT ? yT : a.Tout);
   return 0;
 }

@@ -3,6 +3,9 @@
 //   y[b][y_off + co][t] = epi( bias[co] + sum_{ci,j} w[co][ci][j] * X[b][ci][t*stride + j*dil - pad_left] )
 //   X = act_in(x[b][x_off + ci] (+ x2[b][x2_off + ci])), out-of-range time indices padded by `pad`
 //   epi(v) = res + scale * act_out(v)   (scale and res optional; res is read in y's view)
+// x (and x2) step xT floats per channel and y (and res) yT; 0 means Tin and Tout.  A larger step views the columns of a
+// wider buffer, e.g. a streaming encoder's history-prefixed activations.  The steps are kernel arguments of their own
+// rather than fields: a larger parameter struct costs the kernel its register allocation (48 instead of 64, ~4 % slower).
 #pragma once
 #include "common.cuh"
 
@@ -35,4 +38,4 @@ __device__ __forceinline__ int reflect_idx(int i, int T) {
 #endif
 
 int conv_f32_init();  // sets the kernel's 96 KB dynamic shared-memory limit on the current device
-int conv_f32_launch(const ConvF32Args& a, int B, cudaStream_t stream);
+int conv_f32_launch(const ConvF32Args& a, int B, cudaStream_t stream, int xT = 0, int yT = 0);

@@ -553,6 +553,15 @@ class Qwen3TTSTokenizer:
         from types import SimpleNamespace
         return SimpleNamespace(audio_codes=codes)
 
+    def open_encode_stream(self, batch: int = 1, max_packet_frames: int = 8):
+        """A streaming encoder of `batch` rows (codec_encoder.EncoderStream): push({row: samples}) returns the (n_i, 16)
+        codes of the frames each push completes, end(rows) the clip's last frame, in the layout of encode().audio_codes;
+        a clip's pushes plus its end equal encode() of the whole clip.  Audio must already be at
+        get_input_sample_rate(): resampling chunk by chunk would not match encode()'s whole-clip resampling."""
+        if self.encoder is None:
+            raise RuntimeError("this tokenizer was built without encoder weights (decode-only)")
+        return self.encoder.open_stream(batch, max_packet_frames)
+
     def decode(self, encoded) -> Tuple[List[np.ndarray], int]:
         """:259-365 — accepts an encode()-style output (has .audio_codes), a dict or a list of dicts whose
         "audio_codes" is a (T,K) tensor / ndarray; pads with -1, decodes, trims to T_i*1920, returns float32 numpy."""
