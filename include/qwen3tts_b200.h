@@ -135,6 +135,28 @@ int q3_admit_with_sampling(q3_engine* e, int32_t n, const int32_t* slots_host, c
                            const q3_sampling* sp_host, const void* embeds_dev, const int32_t* lens_host,
                            const void* trailing_dev, const int32_t* trailing_lens_host, int32_t trailing_stride,
                            void* stream);
+/* ---- registered prompt prefixes: rows that many requests' prompts begin with (a voice's instruct, role and codec
+ * prefix rows, an ICL clone's reference).  q3_prefix_create runs the talker layers over `len` rows embeds_dev bf16
+ * [len][H] on `stream` and keeps their K and V ([2][layers][nkv][len][128] bf16, 114,688 B per row at the 1.7B shape) in
+ * a device block of the engine; *id_out receives its id.  1 <= len < max_ctx - 1.  It writes no slot's K/V and no
+ * row's state, so it may run between two decodes of a session.  Prefixes survive q3_session_begin and q3_prefill, and
+ * live until q3_prefix_free or q3_engine_destroy.  q3_prefix_free synchronises `stream` (an admission's copy of the
+ * block may be queued on it) and releases the block; the id is never reused.  q3_prefix_length: the prefix's rows, or
+ * -1 when no such prefix exists. */
+int q3_prefix_create(q3_engine* e, const void* embeds_dev, int32_t len, void* stream, int32_t* id_out);
+int q3_prefix_free(q3_engine* e, int32_t id, void* stream);
+int q3_prefix_length(q3_engine* e, int32_t id);
+/* q3_admit_with_sampling where request r's prompt is the prefix prefix_ids_host[r] (-1: none; prefix_ids_host == NULL:
+ * none for all) followed by lens_host[r] rows of its own (at least 1).  The prefix's K/V are copied into the slot's
+ * cache at positions [0, P) (P its length) and only the request's own rows are prefilled, at positions P.., so the
+ * request generates exactly what q3_admit_with_sampling of cat(prefix rows, own rows) generates: every prefill stage is
+ * row-wise or causal within one sequence.  Besides the checks of q3_admit_with_sampling, each request's prefix must
+ * exist and P + lens_host[r] < max_ctx; a rejected call admits no row.  Errors name the request index.
+ * q3_admit_with_sampling is this call with prefix_ids_host == NULL. */
+int q3_admit_with_prefix(q3_engine* e, int32_t n, const int32_t* slots_host, const uint32_t* keys_host,
+                         const q3_sampling* sp_host, const int32_t* prefix_ids_host, const void* embeds_dev,
+                         const int32_t* lens_host, const void* trailing_dev, const int32_t* trailing_lens_host,
+                         int32_t trailing_stride, void* stream);
 /* The range check q3_prefill, q3_session_begin and q3_admit_with_sampling apply (see q3_sampling): 0 if sp is
  * accepted, else non-zero with q3_last_error() naming the field.  Host only: needs no engine and no GPU. */
 int q3_sampling_check(const q3_sampling* sp);

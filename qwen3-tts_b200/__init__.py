@@ -5,9 +5,9 @@ Importable as `qwen3_tts_b200` (see the shim module at the repo root; the direct
 from .config import CodecConfig, SamplingParams, StackConfig, TTSConfig  # noqa: F401
 
 __all__ = ["TTSConfig", "StackConfig", "SamplingParams", "CodecConfig",
-           "Qwen3TTSModel", "Qwen3TTSTokenizer", "VoiceClonePromptItem"]
+           "Qwen3TTSModel", "Qwen3TTSTokenizer", "VoiceClonePromptItem", "Voice"]
 
-_PUBLIC = {"Qwen3TTSModel", "Qwen3TTSTokenizer", "VoiceClonePromptItem"}
+_PUBLIC = {"Qwen3TTSModel", "Qwen3TTSTokenizer", "VoiceClonePromptItem", "Voice"}
 
 
 def __getattr__(name):

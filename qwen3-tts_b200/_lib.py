@@ -62,7 +62,8 @@ AR_SYMBOLS = ["q3_abi_version", "q3_last_error", "q3_engine_create", "q3_engine_
               "q3_engine_finalize", "q3_prefill", "q3_decode", "q3_get_progress", "q3_set_debug",
               "q3_algorithmic_bytes", "q3_set_profile", "q3_describe_frame_program",
               "q3_session_begin", "q3_release_slots", "q3_append_trailing", "q3_set_hidden_capture",
-              "q3_admit_with_sampling", "q3_sampling_check", "q3_set_trailing_open"]
+              "q3_admit_with_sampling", "q3_sampling_check", "q3_set_trailing_open",
+              "q3_prefix_create", "q3_prefix_free", "q3_prefix_length", "q3_admit_with_prefix"]
 CODEC_SYMBOLS = ["q3_codec_create", "q3_codec_destroy", "q3_codec_load_tensor", "q3_codec_finalize",
                  "q3_codec_forward", "q3_codec_total_upsample", "q3_codec_last_launch_count", "q3_codec_debug_capture",
                  "q3_codec_stream_open", "q3_codec_stream_close",
@@ -119,6 +120,11 @@ def load():
     lib.q3_set_trailing_open.argtypes = [vp, i32, i32]
     lib.q3_admit_with_sampling.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(C.c_uint32), C.POINTER(Sampling), vp,
                                            C.POINTER(i32), vp, C.POINTER(i32), i32, vp]
+    lib.q3_admit_with_prefix.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(C.c_uint32), C.POINTER(Sampling), C.POINTER(i32),
+                                         vp, C.POINTER(i32), vp, C.POINTER(i32), i32, vp]
+    lib.q3_prefix_create.argtypes = [vp, vp, i32, vp, C.POINTER(i32)]
+    lib.q3_prefix_free.argtypes = [vp, i32, vp]
+    lib.q3_prefix_length.argtypes = [vp, i32]
     lib.q3_sampling_check.argtypes = [C.POINTER(Sampling)]
     lib.q3_get_progress.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
     lib.q3_set_debug.argtypes = [vp, vp, i32, vp, vp]

@@ -10,7 +10,7 @@ on libqwen3tts_b200.so.  The reference state_dict is re-laid-out here into the e
 """
 import ctypes as C
 import math
-from typing import List, Optional, Sequence
+from typing import List, Optional, Sequence, Tuple
 
 import torch
 
@@ -72,6 +72,8 @@ class CodecDecoder:
         _lib.check(self.lib.q3_codec_finalize(self.h))
         self.total_upsample = self.lib.q3_codec_total_upsample(self.h)
         assert self.total_upsample == cfg.total_upsample
+        self._banks: List[Optional["CodecStream"]] = []   # bank_reference's streams and their rows in use
+        self._bank_used: List[set] = []
 
     # ------------------------------------------------------------------ weight conversion
     def _put(self, name, x, bf16):
@@ -199,6 +201,10 @@ class CodecDecoder:
         return int(self.lib.q3_codec_last_launch_count(self.h))
 
     def close(self):
+        for st in getattr(self, "_banks", []):
+            if st is not None:
+                st.close()
+        self._banks = []
         if getattr(self, "h", None):
             self.lib.q3_codec_destroy(self.h)
             self.h = None
@@ -259,6 +265,43 @@ class CodecDecoder:
         """Stateful streaming decoder over `batch` rows (q3_codec_stream_*): push packets, get exactly the waveform of
         the full causal forward over everything pushed, for the cost of the new frames only."""
         return CodecStream(self, batch, max_packet_frames)
+
+    # ------------------------------------------------------------------ reference state bank (registered voices)
+    def bank_reference(self, codes: torch.Tensor) -> Tuple[int, int]:
+        """Decode reference codes ((L, K), the layout of VoiceClonePromptItem.ref_code) once into a row of a bank
+        stream of this decoder and return (bank, row).  A row copied from it (CodecStream.copy_from(bank_stream(bank),
+        [row], [slot])) has exactly the state CodecStream.seed with these codes leaves.  A bank holds up to max_batch
+        rows; it grows by opening a larger stream and copying its rows over, so (bank, row) stays valid until
+        bank_release.  Bank streams take no packets: they are opened with packets of one frame."""
+        check_ref_codes(self.cfg, codes, self.max_frames, "reference codes")
+        bank = next((i for i, used in enumerate(self._bank_used) if len(used) < self.max_batch), None)
+        if bank is None:
+            self._banks.append(None)
+            self._bank_used.append(set())
+            bank = len(self._banks) - 1
+        used, old = self._bank_used[bank], self._banks[bank]
+        if old is None or len(used) == old.B:
+            grown = CodecStream(self, min(max(2 * len(used), 1), self.max_batch), 1)
+            if used:
+                grown.copy_from(old, sorted(used), sorted(used))
+            if old is not None:
+                torch.cuda.current_stream(self.device).synchronize()   # the copy reads the old stream
+                old.close()
+            self._banks[bank] = grown
+        st = self._banks[bank]
+        row = min(set(range(st.B)) - used)
+        st.seed([row], [codes])
+        st._seeder.close()      # registration is rare: the private seed stream is not kept
+        st._seeder = None
+        used.add(row)
+        return bank, row
+
+    def bank_stream(self, bank: int) -> "CodecStream":
+        return self._banks[bank]
+
+    def bank_release(self, bank: int, row: int):
+        """Free a row of bank_reference; the bank's stream stays open for later references."""
+        self._bank_used[bank].discard(int(row))
 
     @torch.no_grad()
     def chunked_decode(self, codes, chunk_size=300, left_context_size=25):
@@ -365,8 +408,18 @@ class CodecStream:
             pkt[i, :, :lens[i]] = c.to(dec.device, torch.int32).T
         sd.reset()
         sd.push(pkt, lens + [0] * (sd.B - n))   # the prefixes' audio is discarded
-        stream = C.c_void_p(torch.cuda.current_stream(dec.device).cuda_stream)
-        _lib.check(dec.lib.q3_codec_stream_copy_rows(self.h, sd.h, n, (C.c_int32 * n)(*range(n)), (C.c_int32 * n)(*rows), stream))
+        self.copy_from(sd, range(n), rows)
+
+    def copy_from(self, src: "CodecStream", src_rows: Sequence[int], rows: Sequence[int]):
+        """Row rows[i] of this stream becomes row src_rows[i] of `src`, a stream of the same decoder of any size
+        (q3_codec_stream_copy_rows): its whole causal state and its position.  The other rows are untouched."""
+        src_rows, rows = [int(r) for r in src_rows], [int(r) for r in rows]
+        if len(src_rows) != len(rows):
+            raise ValueError(f"{len(src_rows)} source rows for {len(rows)} rows")
+        n = len(rows)
+        stream = C.c_void_p(torch.cuda.current_stream(self.dec.device).cuda_stream)
+        _lib.check(self.dec.lib.q3_codec_stream_copy_rows(self.h, src.h, n, (C.c_int32 * max(n, 1))(*src_rows),
+                                                          (C.c_int32 * max(n, 1))(*rows), stream))
 
     def close(self):
         if getattr(self, "_seeder", None) is not None:

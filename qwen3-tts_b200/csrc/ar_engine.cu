@@ -130,6 +130,10 @@ struct q3_engine {
   unsigned long long* prof = nullptr;
   size_t smem_bytes = 0;
   double w_talker_bytes = 0, w_cp_unique_bytes = 0, w_cp_stream_bytes = 0;
+  // registered prompt prefixes (q3_prefix_create): their talker K/V, [2 (K, V)][layers][nkv][len][HD]
+  struct Prefix { bf16* kv; int len; };
+  std::map<int, Prefix> prefixes;
+  int next_prefix = 0;
 
   ~q3_engine() {
     if (copy_stream) cudaStreamDestroy(copy_stream);
@@ -519,13 +523,15 @@ static int launch_program(q3_engine* e, int off, int n, int mode, int max_iters,
 }
 
 // One admission of n requests: request r enters engine slot slots[r] with the Philox row key keys[r] and the sampling
-// parameters sp[r] (sp == nullptr: the default e->sp); its prompt is lens[r] rows of embeds (packed back to back), its
-// trailing text the first tl[r] rows of trailing[r] ([n][stride][H]; tl == nullptr: none).
+// parameters sp[r] (sp == nullptr: the default e->sp); its prompt is the prefix prefix[r] (prefix == nullptr or an id
+// of -1: none) followed by lens[r] rows of embeds (packed back to back), its trailing text the first tl[r] rows of
+// trailing[r] ([n][stride][H]; tl == nullptr: none).
 struct Admission {
   int n;
   const int32_t* slots;
   const uint32_t* keys;
   const q3_sampling* sp;
+  const int32_t* prefix;
   const void* embeds;
   const int32_t* lens;
   const void* trailing;
@@ -533,39 +539,37 @@ struct Admission {
   int stride;
 };
 
-// Prefill of an admission into its slots: the index kernel resets the rows' device state and gathers their trailing
-// text, wgmma GEMMs run over all their tokens at once, K/V go into the slots' cache rows, then the head GEMV + the first
-// codebook-0 sample of exactly those rows (`mask`: the admitted slots).
-static int prefill_rows(q3_engine* e, const Admission& A, unsigned int mask, cudaStream_t stream) {
-  const int n = A.n, H = e->cfg.talker.hidden_size;
-  PfLens pl{};
-  PfRows pr{};
-  pl.B = n;
-  pr.src = reinterpret_cast<const bf16*>(A.trailing); pr.dst = e->trailing; pr.stride = A.stride; pr.cap = e->trailing_cap; pr.H = H;
-  const int V = e->cfg.talker.vocab_size;
-  int row_work = V;  // index-kernel threads per row: its seen bytes or its trailing elements
-  for (int r = 0; r < n; ++r) {
-    pl.start[r + 1] = pl.start[r] + A.lens[r]; pl.slot[r] = A.slots[r];
-    pr.trailing_len[r] = A.tl ? A.tl[r] : 0;
-    row_work = std::max(row_work, pr.trailing_len[r] * H);
-  }
-  const int ntok = pl.start[n];
+// the prefix of request r of A (checked by check_admission), or null
+static const q3_engine::Prefix* admission_prefix(const q3_engine* e, const Admission& A, int r) {
+  if (!A.prefix || A.prefix[r] < 0) return nullptr;
+  const auto it = e->prefixes.find(A.prefix[r]);
+  return it == e->prefixes.end() ? nullptr : &it->second;
+}
+
+// room in the prefill scratch for ntok packed rows
+static int ensure_prefill_rows(q3_engine* e, int ntok, cudaStream_t stream) {
+  if (ntok <= e->pf_cap) return 0;
   const q3_stack_cfg& tc = e->cfg.talker;
-  const int nh = tc.num_heads, nkv = tc.num_kv_heads, I = tc.intermediate_size, QKV = (nh + 2 * nkv) * HD;
-  if (ntok > e->pf_cap) {
-    const size_t cap = std::max(ntok + ntok / 4, 1024);
-    DevStore& store = e->store;
-    e->pf_cap = 0;  // until every block has grown: a failed growth leaves a freed block behind
-    if (store.grow(&e->pf_x, cap * H * sizeof(bf16), stream, true) || store.grow(&e->pf_xn, cap * H * sizeof(bf16), stream, true) ||
-        store.grow(&e->pf_qkv, cap * QKV * sizeof(bf16), stream, true) ||
-        store.grow(&e->pf_attn, cap * nh * HD * sizeof(bf16), stream, true) ||
-        store.grow(&e->pf_act, cap * I * sizeof(bf16), stream, true) || store.grow(&e->pf_seq, cap * sizeof(int), stream, true) ||
-        store.grow(&e->pf_pos, cap * sizeof(int), stream, true))
-      return 1;
-    e->pf_cap = (int)cap;
-  }
-  pf_index_kernel<<<dim3((std::max(ntok, row_work) + 255) / 256, n), 256, 0, stream>>>(pl, pr, e->st, e->seen, V, e->pf_seq, e->pf_pos);
-  Q3_CUDA(cudaMemcpyAsync(e->pf_x, A.embeds, (size_t)ntok * H * 2, cudaMemcpyDeviceToDevice, stream));
+  const int H = tc.hidden_size, nh = tc.num_heads, I = tc.intermediate_size, QKV = (nh + 2 * tc.num_kv_heads) * HD;
+  const size_t cap = std::max(ntok + ntok / 4, 1024);
+  DevStore& store = e->store;
+  e->pf_cap = 0;  // until every block has grown: a failed growth leaves a freed block behind
+  if (store.grow(&e->pf_x, cap * H * sizeof(bf16), stream, true) || store.grow(&e->pf_xn, cap * H * sizeof(bf16), stream, true) ||
+      store.grow(&e->pf_qkv, cap * QKV * sizeof(bf16), stream, true) ||
+      store.grow(&e->pf_attn, cap * nh * HD * sizeof(bf16), stream, true) ||
+      store.grow(&e->pf_act, cap * I * sizeof(bf16), stream, true) || store.grow(&e->pf_seq, cap * sizeof(int), stream, true) ||
+      store.grow(&e->pf_pos, cap * sizeof(int), stream, true))
+    return 1;
+  e->pf_cap = (int)cap;
+  return 0;
+}
+
+// The talker layers over the ntok packed rows of pf_x, whose sequence and position are in pf_seq / pf_pos: wgmma GEMMs
+// over all rows at once, K/V of every row into kc / vc ([seq][layers][nkv][cap][HD]), attention over each sequence's
+// keys up to the row's position.  Every stage is row-wise or causal within one sequence.
+static int prefill_layers(q3_engine* e, int ntok, bf16* kc, bf16* vc, int cap, cudaStream_t stream) {
+  const q3_stack_cfg& tc = e->cfg.talker;
+  const int H = tc.hidden_size, nh = tc.num_heads, nkv = tc.num_kv_heads, I = tc.intermediate_size, QKV = (nh + 2 * nkv) * HD;
   const int mt = (ntok + 127) / 128;
   const int zero = 0;
   auto gemm = [&](const bf16* a, int K, const bf16* w, int N, GemmEpilogue ep) -> int {
@@ -580,16 +584,50 @@ static int prefill_rows(q3_engine* e, const Admission& A, unsigned int mask, cud
     pf_rmsnorm_kernel<<<(ntok + rows_per_blk - 1) / rows_per_blk, 256, 0, stream>>>(e->pf_x, L.ln1, e->pf_xn, ntok, H, tc.rms_eps);
     { GemmEpilogue ep{}; ep.out_raw = e->pf_qkv; if (gemm(e->pf_xn, H, L.qkv, QKV, ep)) return 1; }
     pf_qkv_post_kernel<<<(ntok * (nh + 2 * nkv) + 7) / 8, 256, 0, stream>>>(e->pf_qkv, ntok, e->pf_seq, e->pf_pos, nh, nkv, L.qn, L.kn, tc.rms_eps,
-                                                                         e->talker.rope_cos, e->talker.rope_sin, e->talker.kc,
-                                                                         e->talker.vc, l, tc.num_layers, e->talker.cap);
-    pf_attention_kernel<<<(ntok * nh + 7) / 8, 256, 0, stream>>>(e->pf_qkv, e->pf_attn, ntok, e->pf_seq, e->pf_pos, nh, nkv, e->talker.kc,
-                                                                 e->talker.vc, l, tc.num_layers, e->talker.cap);
+                                                                         e->talker.rope_cos, e->talker.rope_sin, kc, vc, l,
+                                                                         tc.num_layers, cap);
+    pf_attention_kernel<<<(ntok * nh + 7) / 8, 256, 0, stream>>>(e->pf_qkv, e->pf_attn, ntok, e->pf_seq, e->pf_pos, nh, nkv, kc, vc, l,
+                                                                 tc.num_layers, cap);
     { GemmEpilogue ep{}; ep.resid = e->pf_x; ep.out_raw = e->pf_x; if (gemm(e->pf_attn, nh * HD, L.o, H, ep)) return 1; }
     pf_rmsnorm_kernel<<<(ntok + rows_per_blk - 1) / rows_per_blk, 256, 0, stream>>>(e->pf_x, L.ln2, e->pf_xn, ntok, H, tc.rms_eps);
     { GemmEpilogue ep{}; ep.act = ACT_SWIGLU_BLK8; ep.out_act = e->pf_act; if (gemm(e->pf_xn, H, L.gate_up, 2 * I, ep)) return 1; }
     { GemmEpilogue ep{}; ep.resid = e->pf_x; ep.out_raw = e->pf_x; if (gemm(e->pf_act, I, L.down, H, ep)) return 1; }
   }
   Q3_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// Prefill of an admission into its slots: the index kernel resets the rows' device state, gathers their trailing text
+// and copies their prefixes' K/V into the slots' caches; the layers run over the rows' own (suffix) tokens, whose K/V
+// go into the slots' cache rows behind the prefix; then the head GEMV + the first codebook-0 sample of exactly those
+// rows (`mask`: the admitted slots).
+static int prefill_rows(q3_engine* e, const Admission& A, unsigned int mask, cudaStream_t stream) {
+  const int n = A.n, H = e->cfg.talker.hidden_size;
+  const q3_stack_cfg& tc = e->cfg.talker;
+  PfLens pl{};
+  PfRows pr{};
+  PfPrefix px{};
+  pl.B = n;
+  pr.src = reinterpret_cast<const bf16*>(A.trailing); pr.dst = e->trailing; pr.stride = A.stride; pr.cap = e->trailing_cap; pr.H = H;
+  px.kc = reinterpret_cast<uint4*>(e->talker.kc); px.vc = reinterpret_cast<uint4*>(e->talker.vc);
+  px.lh = tc.num_layers * tc.num_kv_heads; px.cap = e->talker.cap;
+  const int V = tc.vocab_size;
+  int row_work = V;  // index-kernel threads per row: its seen bytes, its trailing elements or its prefix K chunks
+  for (int r = 0; r < n; ++r) {
+    pl.start[r + 1] = pl.start[r] + A.lens[r]; pl.slot[r] = A.slots[r];
+    pr.trailing_len[r] = A.tl ? A.tl[r] : 0;
+    row_work = std::max(row_work, pr.trailing_len[r] * H);
+    if (const q3_engine::Prefix* p = admission_prefix(e, A, r)) {
+      pl.p0[r] = p->len;
+      px.kv[r] = reinterpret_cast<const uint4*>(p->kv);
+      row_work = std::max(row_work, px.lh * p->len * (HD / 8));
+    }
+  }
+  const int ntok = pl.start[n];
+  if (ensure_prefill_rows(e, ntok, stream)) return 1;
+  pf_index_kernel<<<dim3((std::max(ntok, row_work) + 255) / 256, n), 256, 0, stream>>>(pl, pr, px, e->st, e->seen, V, e->pf_seq, e->pf_pos);
+  Q3_CUDA(cudaMemcpyAsync(e->pf_x, A.embeds, (size_t)ntok * H * 2, cudaMemcpyDeviceToDevice, stream));
+  if (prefill_layers(e, ntok, e->talker.kc, e->talker.vc, e->talker.cap, stream)) return 1;
   pf_gather_last_kernel<<<n, 128, 0, stream>>>(pl, e->pf_x, e->h_last, H);
   // head + sample codebook-0 of the rows' first frame (codes are materialised by the following q3_decode via st->c0)
   e->admit_mask = mask;
@@ -635,7 +673,12 @@ static int check_admission(const q3_engine* e, const Admission& A, int B, int ca
     Q3_REQUIRE(b >= 0 && b < B, "slot %d out of range", b);
     Q3_REQUIRE(!((running >> b) & 1u), "slot %d is still running (q3_release_slots it first)", b);
     for (int q = 0; q < r; ++q) Q3_REQUIRE(A.slots[q] != b, "slot %d admitted twice", b);
-    Q3_REQUIRE(A.lens[r] >= 1 && A.lens[r] < e->cfg.max_ctx, "prompt length %d out of range", A.lens[r]);
+    const int id = A.prefix ? A.prefix[r] : -1;
+    Q3_REQUIRE(id == -1 || e->prefixes.count(id), "request %d: prefix %d does not exist (never created, or freed)", r, id);
+    const int P = id == -1 ? 0 : e->prefixes.at(id).len, S = A.lens[r];
+    Q3_REQUIRE(S >= 1 && P + S < e->cfg.max_ctx,
+               "request %d: prompt length %d out of range (a prefix of %d rows and %d rows of its own, at least 1, below max_ctx %d)",
+               r, P + S, P, S, e->cfg.max_ctx);
     Q3_REQUIRE(tl >= 0 && tl <= A.stride && tl <= cap, "trailing length %d exceeds the stride %d or the capacity %d", tl, A.stride, cap);
     Q3_REQUIRE(tl == 0 || A.trailing, "request %d has a trailing length of %d but no trailing text", r, tl);
   }
@@ -672,7 +715,8 @@ static int admit_rows(q3_engine* e, const Admission& A, int F, unsigned int runn
   unsigned int admitted = 0;
   for (int r = 0; r < A.n; ++r) {
     const int b = A.slots[r];
-    e->len0[b] = A.lens[r] - F; e->frame0[b] = F; e->row_key[b] = A.keys[r]; e->trailing_len[b] = A.tl ? A.tl[r] : 0;
+    const q3_engine::Prefix* p = admission_prefix(e, A, r);
+    e->len0[b] = (p ? p->len : 0) + A.lens[r] - F; e->frame0[b] = F; e->row_key[b] = A.keys[r]; e->trailing_len[b] = A.tl ? A.tl[r] : 0;
     e->row_sp[b] = A.sp ? A.sp[r] : e->sp;
     e->text_open[b] = false; e->held[b] = false;  // every admission starts closed: q3_set_trailing_open opens it
     admitted |= 1u << b;
@@ -697,7 +741,7 @@ extern "C" int q3_prefill(q3_engine* e, int32_t B, const void* embeds_dev, const
   Q3_REQUIRE(embeds_dev && lens_host && tts_pad_dev, "null argument");
   int32_t slots[MAXB]; uint32_t keys[MAXB];
   for (int b = 0; b < B; ++b) { slots[b] = b; keys[b] = (uint32_t)b; }
-  const Admission A{B, slots, keys, nullptr, embeds_dev, lens_host, trailing_dev, trailing_lens_host, trailing_stride};
+  const Admission A{B, slots, keys, nullptr, nullptr, embeds_dev, lens_host, trailing_dev, trailing_lens_host, trailing_stride};
   if (check_admission(e, A, B, trailing_stride, 0)) return 1;
   Q3_CUDA(cudaSetDevice(e->cfg.device));
   cudaStream_t stream = (cudaStream_t)stream_;
@@ -722,11 +766,11 @@ extern "C" int q3_sampling_check(const q3_sampling* sp) {
   return check_sampling(*sp);
 }
 
-// sp_host == nullptr: every request samples with the session's parameters
-extern "C" int q3_admit_with_sampling(q3_engine* e, int32_t n, const int32_t* slots_host, const uint32_t* keys_host,
-                                      const q3_sampling* sp_host, const void* embeds_dev, const int32_t* lens_host,
-                                      const void* trailing_dev, const int32_t* trailing_lens_host, int32_t trailing_stride,
-                                      void* stream_) {
+// sp_host == nullptr: every request samples with the session's parameters; prefix_ids_host == nullptr: no prefixes
+extern "C" int q3_admit_with_prefix(q3_engine* e, int32_t n, const int32_t* slots_host, const uint32_t* keys_host,
+                                    const q3_sampling* sp_host, const int32_t* prefix_ids_host, const void* embeds_dev,
+                                    const int32_t* lens_host, const void* trailing_dev, const int32_t* trailing_lens_host,
+                                    int32_t trailing_stride, void* stream_) {
   Q3_REQUIRE(e && e->finalized && e->session, "q3_session_begin first");
   Q3_REQUIRE(n >= 1 && n <= e->B && slots_host && keys_host && embeds_dev && lens_host, "bad argument");
   // every request's parameters before anything else: one bad entry fails the whole admission before any device work
@@ -745,8 +789,65 @@ extern "C" int q3_admit_with_sampling(q3_engine* e, int32_t n, const int32_t* sl
   unsigned int running = 0;
   for (int b = 0; b < e->B; ++b)
     if (e->active[b] && !hs.finished[b]) running |= 1u << b;
-  const Admission A{n, slots_host, keys_host, sp_host, embeds_dev, lens_host, trailing_dev, trailing_lens_host, trailing_stride};
+  const Admission A{n, slots_host, keys_host, sp_host, prefix_ids_host, embeds_dev, lens_host, trailing_dev, trailing_lens_host,
+                    trailing_stride};
   return admit_rows(e, A, hs.step, running, stream);
+}
+
+extern "C" int q3_admit_with_sampling(q3_engine* e, int32_t n, const int32_t* slots_host, const uint32_t* keys_host,
+                                      const q3_sampling* sp_host, const void* embeds_dev, const int32_t* lens_host,
+                                      const void* trailing_dev, const int32_t* trailing_lens_host, int32_t trailing_stride,
+                                      void* stream_) {
+  return q3_admit_with_prefix(e, n, slots_host, keys_host, sp_host, nullptr, embeds_dev, lens_host, trailing_dev,
+                              trailing_lens_host, trailing_stride, stream_);
+}
+
+// ---- registered prompt prefixes: the talker K/V of rows that many requests' prompts begin with ---------------------
+extern "C" int q3_prefix_create(q3_engine* e, const void* embeds_dev, int32_t len, void* stream_, int32_t* id_out) {
+  Q3_REQUIRE(e && e->finalized, "engine not finalized");
+  Q3_REQUIRE(len >= 1 && len < e->cfg.max_ctx - 1, "prefix length %d out of range [1, %d)", len, e->cfg.max_ctx - 1);
+  Q3_REQUIRE(embeds_dev && id_out, "null argument");
+  Q3_CUDA(cudaSetDevice(e->cfg.device));
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const q3_stack_cfg& tc = e->cfg.talker;
+  const size_t half = (size_t)tc.num_layers * tc.num_kv_heads * len * HD;
+  bf16* kv = nullptr;
+  if (e->store.alloc(&kv, 2 * half, false)) return 1;  // the layers write every element
+  int rc = ensure_prefill_rows(e, len, stream);
+  if (!rc) {
+    pf_prefix_index_kernel<<<(len + 255) / 256, 256, 0, stream>>>(len, e->pf_seq, e->pf_pos);
+    Q3_CUDA(cudaMemcpyAsync(e->pf_x, embeds_dev, (size_t)len * tc.hidden_size * 2, cudaMemcpyDeviceToDevice, stream));
+    rc = prefill_layers(e, len, kv, kv + half, len, stream);
+  }
+  if (rc) {  // the error stays the one recorded; launches already queued may still write the block
+    cudaStreamSynchronize(stream);
+    e->store.release(kv);
+    return 1;
+  }
+  const int id = e->next_prefix++;
+  e->prefixes[id] = q3_engine::Prefix{kv, len};
+  *id_out = id;
+  return 0;
+}
+
+extern "C" int q3_prefix_free(q3_engine* e, int32_t id, void* stream_) {
+  Q3_REQUIRE(e, "null engine");
+  const auto it = e->prefixes.find(id);
+  Q3_REQUIRE(it != e->prefixes.end(), "prefix %d does not exist (never created, or freed)", id);
+  Q3_CUDA(cudaSetDevice(e->cfg.device));
+  Q3_CUDA(cudaStreamSynchronize((cudaStream_t)stream_));  // an admission's copy of the block may still be queued
+  bf16* kv = it->second.kv;
+  e->prefixes.erase(it);
+  return e->store.release(kv);
+}
+
+extern "C" int q3_prefix_length(q3_engine* e, int32_t id) {
+  if (e) {
+    const auto it = e->prefixes.find(id);
+    if (it != e->prefixes.end()) return it->second.len;
+  }
+  q3_set_err("prefix %d does not exist", id);
+  return -1;
 }
 
 extern "C" int q3_decode(q3_engine* e, int32_t max_frames, int32_t* codes_dev, int32_t codes_stride, void* stream_) {

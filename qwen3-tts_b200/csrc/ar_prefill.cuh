@@ -41,28 +41,51 @@ __global__ void pf_rmsnorm_kernel(const bf16* __restrict__ x, const bf16* __rest
 
 // packed-token index (row, position) of all prompt tokens, built on the device from the prompt lengths (passed by
 // value: no host staging buffer, no synchronisation), and the gather of every row's last hidden state
-struct PfLens { int B; int start[MAXB + 1]; int slot[MAXB]; };  // row r of the packed prompt batch lives in engine slot slot[r]
+// row r of the packed prompt batch lives in engine slot slot[r]; its packed rows are the suffix of a prompt whose first
+// p0[r] positions (a prefix, 0: none) are already in the slot's K/V cache
+struct PfLens { int B; int start[MAXB + 1]; int slot[MAXB]; int p0[MAXB]; };
 // the admitted rows' trailing lengths and text [r][stride][H], gathered into the engine's copy [slot][cap][H]
 struct PfRows {
   int trailing_len[MAXB];
   const bf16* src; bf16* dst; int stride, cap, H;
 };
-// grid (x, row r): slice r resets row r's device state and seen bytes and gathers its trailing text (element-wise: the
-// source may be any bf16 pointer); slice 0 also writes the token index
-__global__ void pf_index_kernel(PfLens L, PfRows R, DevState* st, unsigned char* seen, int V, int* tok_seq, int* tok_pos) {
+// the prefix K/V of the admitted rows (null: none), each [lh = layers * nkv][p0[r]][HD] for K and then for V, copied
+// into the slots' caches [slot][lh][cap][HD] at positions [0, p0[r])
+struct PfPrefix {
+  const uint4* kv[MAXB];
+  uint4 *kc, *vc;
+  int lh, cap;
+};
+// grid (x, row r): slice r resets row r's device state and seen bytes, gathers its trailing text (element-wise: the
+// source may be any bf16 pointer) and copies its prefix K/V; slice 0 also writes the token index
+__global__ void pf_index_kernel(PfLens L, PfRows R, PfPrefix X, DevState* st, unsigned char* seen, int V, int* tok_seq, int* tok_pos) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x, r = blockIdx.y, b = L.slot[r];
   if (r == 0 && i < L.start[L.B]) {
     int s = 0;
     while (i >= L.start[s + 1]) ++s;
     tok_seq[i] = L.slot[s];
-    tok_pos[i] = i - L.start[s];
+    tok_pos[i] = L.p0[s] + i - L.start[s];
   }
   if (i == 0) {
     st->finished[b] = 0; st->n_valid[b] = 0; st->n_gen[b] = 0; st->c0[b] = 0;
-    st->len0[b] = L.start[r + 1] - L.start[r]; st->trailing_len[b] = R.trailing_len[r];
+    st->len0[b] = L.p0[r] + L.start[r + 1] - L.start[r]; st->trailing_len[b] = R.trailing_len[r];
   }
   if (i < V) seen[(size_t)b * V + i] = 0;
   if (i < R.trailing_len[r] * R.H) R.dst[(size_t)b * R.cap * R.H + i] = R.src[(size_t)r * R.stride * R.H + i];
+  if (X.kv[r]) {  // one 16-byte chunk of K and one of V per thread and step; a position is HD / 8 chunks
+    const int row = L.p0[r] * (HD / 8);
+    const size_t n = (size_t)X.lh * row;
+    for (size_t j = i; j < n; j += (size_t)gridDim.x * blockDim.x) {
+      const size_t lh = j / row, c = j - lh * row, d = ((size_t)b * X.lh + lh) * X.cap * (HD / 8) + c;
+      X.kc[d] = X.kv[r][j];
+      X.vc[d] = X.kv[r][n + j];
+    }
+  }
+}
+// token index of a prefix computed alone: its n rows are positions 0..n-1 of sequence 0 of the prefix's K/V block
+__global__ void pf_prefix_index_kernel(int n, int* tok_seq, int* tok_pos) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) { tok_seq[i] = 0; tok_pos[i] = i; }
 }
 __global__ void pf_gather_last_kernel(PfLens L, const bf16* __restrict__ x, bf16* __restrict__ h_last, int H) {
   const int b = blockIdx.x;

@@ -47,15 +47,24 @@ class DevStore {
   int grow(T** p, size_t bytes, cudaStream_t stream, bool zero = false) {
     if (*p) {
       Q3_CUDA(cudaStreamSynchronize(stream));
-      for (size_t i = 0; i < blocks_.size(); ++i)
-        if (blocks_[i] == *p) { blocks_.erase(blocks_.begin() + i); break; }
-      Q3_CUDA(cudaFree(*p));
+      if (release(*p)) return 1;
       *p = nullptr;
     }
     void* q = nullptr;
     if (alloc(&q, bytes, zero)) return 1;
     *p = static_cast<T*>(q);
     return 0;
+  }
+
+  // free the block p of this store before the store ends.  The caller has drained every stream that may still use it.
+  int release(void* p) {
+    for (size_t i = 0; i < blocks_.size(); ++i)
+      if (blocks_[i] == p) {
+        blocks_.erase(blocks_.begin() + i);
+        Q3_CUDA(cudaFree(p));
+        return 0;
+      }
+    return q3_set_err("%s: block %p is not one of this store's", engine_, p);
   }
 
   // copy the device tensor `dev` (shape[ndim], elements of `dtype`) in as `name`.  `dev` may still be being produced on

@@ -170,11 +170,14 @@ class AREngine:
         _lib.check(self.lib.q3_session_begin(self.h, int(n_slots), int(max_trailing), pad.data_ptr(), C.byref(s), C.c_void_p(stream)))
 
     def admit(self, slots: Sequence[int], keys: Sequence[int], inputs_embeds: Sequence[torch.Tensor],
-              trailing_text: Sequence[torch.Tensor], sampling: Optional[Sequence[Optional[SamplingParams]]] = None):
+              trailing_text: Sequence[torch.Tensor], sampling: Optional[Sequence[Optional[SamplingParams]]] = None,
+              prefixes: Optional[Sequence[Optional[int]]] = None):
         """Prefill new requests into free slots of the running session (q3_admit_with_sampling).  `sampling`: None
         (every request samples with the session's parameters) or one entry per request, a SamplingParams or None for
         the session's; a bad entry fails the whole admission before anything changes.  Of each entry the fields of
-        q3_sampling are used, max_new_tokens is the caller's horizon."""
+        q3_sampling are used, max_new_tokens is the caller's horizon.  `prefixes`: None, or one entry per request, a
+        prefix id of create_prefix or None; request r's prompt is then that prefix followed by inputs_embeds[r]
+        (q3_admit_with_prefix), and it generates what the admission of the whole prompt generates."""
         n = len(slots)
         sps = None
         if sampling is not None:
@@ -183,9 +186,36 @@ class AREngine:
             sps = (_lib.Sampling * n)(*[self._sampling(self._session_sp if s is None else s) for s in sampling])
         emb, lens, tr, tl, stride = self._pack(inputs_embeds, trailing_text)
         stream = torch.cuda.current_stream(self.device).cuda_stream
-        _lib.check(self.lib.q3_admit_with_sampling(self.h, n, (C.c_int32 * n)(*[int(x) for x in slots]),
-                                                   (C.c_uint32 * n)(*[int(k) & 0xffffffff for k in keys]), sps,
-                                                   emb.data_ptr(), lens, tr.data_ptr(), tl, stride, C.c_void_p(stream)))
+        sl, ks = (C.c_int32 * n)(*[int(x) for x in slots]), (C.c_uint32 * n)(*[int(k) & 0xffffffff for k in keys])
+        if prefixes is None:
+            _lib.check(self.lib.q3_admit_with_sampling(self.h, n, sl, ks, sps, emb.data_ptr(), lens, tr.data_ptr(), tl, stride,
+                                                       C.c_void_p(stream)))
+            return
+        if len(prefixes) != n:
+            raise ValueError(f"prefixes has {len(prefixes)} entries for {n} requests")
+        ids = (C.c_int32 * n)(*[-1 if p is None else int(p) for p in prefixes])
+        _lib.check(self.lib.q3_admit_with_prefix(self.h, n, sl, ks, sps, ids, emb.data_ptr(), lens, tr.data_ptr(), tl, stride,
+                                                 C.c_void_p(stream)))
+
+    def create_prefix(self, embeds: torch.Tensor) -> int:
+        """Register prompt rows (n, H) that requests' prompts begin with (q3_prefix_create): their talker K/V are
+        computed once and kept on the device, and admit(..., prefixes=[id]) copies them into a request's slot instead of
+        prefilling them again.  May be called while a session runs: no running row changes.  Returns the prefix id."""
+        H = self.cfg.talker.hidden_size
+        e = embeds.reshape(-1, H).to(self.device, torch.bfloat16).contiguous()
+        out = C.c_int32()
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        _lib.check(self.lib.q3_prefix_create(self.h, e.data_ptr(), int(e.shape[0]), C.c_void_p(stream), C.byref(out)))
+        return out.value
+
+    def free_prefix(self, prefix_id: int):
+        """Release a prefix of create_prefix (q3_prefix_free).  Rows admitted with it keep their copy of its K/V."""
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        _lib.check(self.lib.q3_prefix_free(self.h, int(prefix_id), C.c_void_p(stream)))
+
+    def prefix_length(self, prefix_id: int) -> int:
+        """Rows of a live prefix, -1 when there is none of that id."""
+        return int(self.lib.q3_prefix_length(self.h, int(prefix_id)))
 
     def append_trailing(self, slot: int, rows: torch.Tensor):
         """Streaming text input: more trailing_text_hidden rows (n, H) for a row that is already generating."""

@@ -34,6 +34,45 @@ class VoiceClonePromptItem:
     ref_text: Optional[str] = None
 
 
+class Voice:
+    """A registered voice (Qwen3TTSModel.register_voice): `prefix`, the (P, H) prompt rows every request of the voice
+    begins with, whose talker K/V live in the AR engine as prefix `prefix_id`; for an ICL clone, the codec decoder's
+    state after its reference codes in row `bank` = (bank, row) of the decoder's reference bank.  `pending` counts its
+    requests a batcher has queued but not admitted; running requests hold their own copies."""
+
+    def __init__(self, owner, language, speaker, instruct_ids, vcp, ref_ids, non_streaming_mode, icl):
+        self.engine = owner.model.engine
+        self.language, self.speaker, self.instruct_ids = language, speaker, instruct_ids
+        self.vcp, self.ref_ids, self.non_streaming_mode, self.icl = vcp, ref_ids, non_streaming_mode, icl
+        self.prefix: Optional[torch.Tensor] = None
+        self.prefix_id: Optional[int] = None
+        self.codec = None
+        self.ref_codes: Optional[torch.Tensor] = None
+        self.bank: Optional[Tuple[int, int]] = None
+        self.pending = 0
+        self.closed = False
+
+    @property
+    def prefix_len(self) -> int:
+        return int(self.prefix.shape[0])
+
+    @property
+    def ref_len(self) -> int:
+        """Frames of the reference the voice's audio continues (0 without one)."""
+        return 0 if self.ref_codes is None else int(self.ref_codes.shape[0])
+
+    def close(self):
+        """Free the voice's prefix and reference-bank row.  ValueError while a batcher holds pending requests of it."""
+        if self.closed:
+            return
+        if self.pending:
+            raise ValueError(f"the voice has {self.pending} pending requests")
+        self.engine.free_prefix(self.prefix_id)
+        if self.bank is not None:
+            self.codec.bank_release(*self.bank)
+        self.closed = True
+
+
 class Qwen3TTSForConditionalGenerationB200:
     def __init__(self, cfg: TTSConfig, weights: Dict[str, torch.Tensor], device="cuda:0", spk_id=None,
                  spk_is_dialect=None, codec_language_id=None, tts_model_type="custom_voice", tts_model_size="1b7",
@@ -886,6 +925,101 @@ class Qwen3TTSModel:
             ref_ids = [None if (rt is None or rt == "") else self._tokenize_texts([self._build_ref_text(rt)])[0]
                        for rt in ref_texts]
         return input_ids, ref_ids, vcp, languages
+
+    # ---- registered voices: a voice's prompt prefix and reference state are computed once and kept on the device
+    def register_voice(self, speaker=None, language=None, instruct=None, voice_clone_prompt=None,
+                       non_streaming_mode=False) -> "Voice":
+        """Register a voice for ContinuousBatcher.submit(..., voice=): the rows of its prompt that do not depend on a
+        request's text (the instruct, the role rows, the codec-prefix overlay and, for an ICL clone, the reference
+        positions before the target text) are prefilled once into a prefix of the AR engine, and an ICL clone's
+        reference codes are decoded once into a row of the codec's reference bank.  The arguments and their checks are
+        those of generate_custom_voice (speaker, instruct), generate_voice_design (instruct) and generate_voice_clone
+        (one voice_clone_prompt item), by model type.  An ICL prefix depends on the layout, so the voice fixes
+        `non_streaming_mode`.  Build its requests with build_voice_request; Voice.close() releases it."""
+        mt = self.model.tts_model_type
+        language = "Auto" if language is None else language
+        if isinstance(language, list) or isinstance(speaker, list) or isinstance(instruct, list):
+            raise ValueError("register_voice takes one voice")
+        vcp, ref_ids, icl = None, None, False
+        if mt == "base":
+            if voice_clone_prompt is None:
+                raise ValueError("a base model's voice needs a voice_clone_prompt")
+            items = voice_clone_prompt if isinstance(voice_clone_prompt, list) else [voice_clone_prompt]
+            if len(items) != 1:
+                raise ValueError(f"register_voice takes one voice_clone_prompt item, got {len(items)}")
+            self._validate_languages([language])
+            vcp = self._prompt_items_to_voice_clone_prompt(items)
+            icl = items[0].ref_code is not None and bool(items[0].icl_mode)
+            if icl:
+                ref_ids = [self._tokenize_texts([self._build_ref_text(items[0].ref_text)])[0]]
+            speaker, instruct = None, None
+        elif mt == "custom_voice":
+            self._validate_languages([language])
+            self._validate_speakers([speaker])
+            if self.model.tts_model_size in "0b6":
+                instruct = None
+        elif mt == "voice_design":
+            self._validate_languages([language])
+            speaker = None
+        else:
+            raise ValueError(f"model type {mt} does not support register_voice")
+        if voice_clone_prompt is not None and mt != "base":
+            raise ValueError(f"model type {mt} takes no voice_clone_prompt")
+        instruct_ids = [None if (instruct is None or instruct == "") else self._tokenize_texts([self._build_instruct_text(instruct)])[0]]
+        voice = Voice(self, language, speaker, instruct_ids, vcp, ref_ids, bool(non_streaming_mode), icl)
+        # the prompt of any text: its first rows are the voice's, computed here once
+        embeds, _, _, T = self._voice_rows(voice, "a")
+        voice.prefix = embeds[:self._voice_prefix_len(voice, embeds.shape[0], T)].clone()
+        eng = self.model.engine
+        voice.prefix_id = eng.create_prefix(voice.prefix)
+        if icl:
+            tok = self.model.speech_tokenizer
+            dec = getattr(tok, "decoder", None) if tok is not None else None
+            if dec is None:
+                eng.free_prefix(voice.prefix_id)
+                raise ValueError("an ICL voice needs the model's speech tokenizer to keep its reference state")
+            voice.codec, voice.ref_codes = dec, vcp["ref_code"][0]
+            voice.bank = dec.bank_reference(voice.ref_codes)
+        return voice
+
+    def _voice_rows(self, voice: "Voice", text, live=False):
+        """build_prefill (or build_live_prefill) of one request of `voice` speaking `text`, and the text's tokens."""
+        input_ids = self._tokenize_texts([self._build_assistant_text(text)])
+        T = int(input_ids[0].reshape(-1).shape[0]) - 8                 # 3 role and 5 closing tokens around the text
+        if live:
+            e, t, p = self.model.build_live_prefill(input_ids, instruct_ids=voice.instruct_ids, voice_clone_prompt=voice.vcp,
+                                                    languages=[voice.language], speakers=[voice.speaker])
+        else:
+            e, t, p = self.model.build_prefill(input_ids, voice.instruct_ids, voice.ref_ids, voice.vcp, [voice.language],
+                                               [voice.speaker], voice.non_streaming_mode)
+        return e[0], t[0], p, T
+
+    def _voice_prefix_len(self, voice: "Voice", n_rows: int, T: int) -> int:
+        """Rows of the prompt layout (_plan_sample) that do not depend on the text, never the prompt's last row: the
+        instruct, 3 role and |C|-1 overlay rows, and for an ICL clone the first min(R, Lc) (streaming) or R
+        (non-streaming) ICL positions, R the reference text's tokens and Lc = L + 1 the codec stream.  `n_rows`: the
+        prompt length of a request whose text has T tokens."""
+        if not voice.icl:
+            return n_rows - (T + 2 if voice.non_streaming_mode else 1)    # the text rows: T + 2, or the first token
+        R = int(voice.ref_ids[0].reshape(-1).shape[0]) - 5              # ref_id[3:-2]
+        Lc = int(voice.vcp["ref_code"][0].shape[0]) + 1
+        if voice.non_streaming_mode:
+            return n_rows - (R + T + 1) - Lc + R                          # text stream R + T + 1 rows, then Lc
+        return min(n_rows - Lc + min(R, Lc), n_rows - 1)
+
+    def build_voice_request(self, text, voice: "Voice", live: bool = False):
+        """One request of a registered voice for ContinuousBatcher.submit(suffix_embeds, trailing, voice=voice):
+        (suffix_embeds, trailing_text, tts_pad_embed), where cat(voice.prefix, suffix_embeds) and trailing_text are
+        the rows build_prefill makes for the same request.  With `live=True` the trailing rows end without tts_eos,
+        as in build_live_request (submit with text_open=True); ICL voices refuse it."""
+        if voice.closed:
+            raise ValueError("the voice is closed")
+        if isinstance(text, list):
+            raise ValueError("build_voice_request takes one text")
+        if live and voice.non_streaming_mode:
+            raise ValueError("live text needs a voice registered with non_streaming_mode=False")
+        embeds, trailing, pad, _ = self._voice_rows(voice, text, live)
+        return embeds[voice.prefix_len:], trailing, pad
 
     def build_voice_clone_requests(self, text, language=None, ref_audio=None, ref_text=None, x_vector_only_mode=False,
                                    voice_clone_prompt=None, non_streaming_mode=False):

@@ -27,6 +27,13 @@ with the reference as their causal left context.  At admission such a slot's cod
 (CodecStream.seed, one call for all seeded slots of the admission) instead of reset; its chunks and `done` entry hold
 the generated part only (tests/test_gpu_scheduler_voice_clone.py).
 
+A request of a registered voice (`submit(suffix, trailing, voice=voice)`, Qwen3TTSModel.register_voice) is admitted
+with the voice's prompt prefix: its K/V are copied into the slot (AREngine.admit(..., prefixes=)) and only the
+request's own rows are prefilled, and an ICL voice's codec row is copied from the decoder's reference bank
+(CodecStream.copy_from, one call per bank) instead of decoding the reference.  It generates and streams exactly what
+the request submitted with its whole prompt and ref_codes does (tests/test_gpu_voice_prefix.py).  A batch without
+voices makes the same calls as before.
+
 Live text (`submit(text_open=True)`, `append_text`, `close_text`): a request's text may keep arriving after submit, as
 when speaking an LLM's answer while it is being written.  Its slot is open in the engine (AREngine.set_text_open): a
 frame-step whose text row has not arrived holds the row instead of reading tts_pad, so the request generates exactly
@@ -38,7 +45,7 @@ running (a client that disconnected).
 """
 from collections import deque
 from dataclasses import dataclass, field
-from typing import Deque, Dict, Iterator, List, Optional, Tuple, Union
+from typing import Any, Deque, Dict, Iterator, List, Optional, Tuple, Union
 
 import numpy as np
 import torch
@@ -56,6 +63,7 @@ class _Request:
     max_frames: int
     sampling: Optional[SamplingParams] = None
     ref_codes: Optional[torch.Tensor] = None
+    voice: Optional[Any] = None   # a registered voice (model.Voice): its prompt prefix and reference state
     text_open: bool = False    # submitted with text that may still grow
     closed: bool = False       # close_text() was called
     n_text: int = 0            # trailing rows given so far
@@ -96,16 +104,31 @@ class ContinuousBatcher:
     # ------------------------------------------------------------------ API
     def submit(self, inputs_embeds: torch.Tensor, trailing_text: Optional[torch.Tensor] = None, key: Optional[int] = None,
                max_frames: Optional[int] = None, sampling: Optional[SamplingParams] = None,
-               ref_codes: Optional[torch.Tensor] = None, text_open: bool = False) -> int:
+               ref_codes: Optional[torch.Tensor] = None, text_open: bool = False, voice=None) -> int:
         """Queue one request; returns its id (also its Philox row key unless `key` is given).  `sampling`: the
         request's own generation parameters (default: the session's); its max_new_tokens bounds the request's horizon
         and may not exceed the session's.  `ref_codes`: (L, num_quantizers) reference codes of a voice-clone request
         (VoiceClonePromptItem.ref_code); its audio is decoded after them, and the horizon leaves the codec's RoPE
         table room for them.  `text_open`: the request's text may grow after submit (append_text, then close_text);
-        until it is closed the request waits for text instead of reading tts_pad past its end.  Bad parameters raise
-        ValueError here, never in a later step()."""
+        until it is closed the request waits for text instead of reading tts_pad past its end.  `voice`: a registered
+        voice (Qwen3TTSModel.register_voice) of this engine, and of this codec if it clones with a reference; the prompt
+        is then the voice's prefix followed by `inputs_embeds` (the suffix of Qwen3TTSModel.build_voice_request), the
+        prefix's K/V are copied at admission instead of prefilled, and an ICL voice's codec row is copied from its
+        reference state instead of decoding the reference.  It takes no `ref_codes`.  Bad parameters raise ValueError
+        here, never in a later step()."""
         H = self.eng.cfg.talker.hidden_size
-        L_ref = 0
+        L_ref, P = 0, 0
+        if voice is not None:
+            if ref_codes is not None:
+                raise ValueError("a registered voice carries its own reference: submit it without ref_codes")
+            if voice.closed:
+                raise ValueError("the voice is closed")
+            if voice.engine is not self.eng:
+                raise ValueError("the voice was registered on another engine")
+            if voice.bank is not None and (self.codec is None or voice.codec is not self.codec):
+                raise ValueError("the voice's reference state belongs to another codec")
+            P = voice.prefix_len
+            L_ref = voice.ref_len if self.codec is not None else 0
         if ref_codes is not None:
             if self.codec is None:
                 raise ValueError("ref_codes need a ContinuousBatcher built with a codec")
@@ -123,15 +146,20 @@ class ContinuousBatcher:
         tr = trailing_text if trailing_text is not None else torch.zeros(0, H)
         if tr.reshape(-1, H).shape[0] > self.max_trailing:
             raise ValueError(f"trailing text of {tr.shape[0]} positions exceeds max_trailing={self.max_trailing}")
-        L = int(inputs_embeds.reshape(-1, H).shape[0])
+        S = int(inputs_embeds.reshape(-1, H).shape[0])
+        if voice is not None and S < 1:
+            raise ValueError("a request of a registered voice needs at least one row of its own")
+        L = P + S
         room = self.eng.max_ctx - L
         if room < 1:
             raise ValueError(f"prompt of {L} positions does not fit max_ctx={self.eng.max_ctx}")
         horizon = min(limit if max_frames is None else max_frames, limit, room)
         if self.codec is not None:
             horizon = min(horizon, self.codec.max_frames - L_ref)  # a codec row's position may not pass its RoPE table
-        self.pending.append(_Request(rid, inputs_embeds, tr, horizon, sampling, ref_codes, text_open=bool(text_open),
+        self.pending.append(_Request(rid, inputs_embeds, tr, horizon, sampling, ref_codes, voice, text_open=bool(text_open),
                                      n_text=int(tr.reshape(-1, H).shape[0])))
+        if voice is not None:
+            voice.pending += 1
         return rid
 
     def _live(self, rid: int, what: str) -> _Request:
@@ -179,6 +207,8 @@ class ContinuousBatcher:
         for r in self.pending:
             if r.rid == rid:
                 self.pending.remove(r)
+                if r.voice is not None:
+                    r.voice.pending -= 1
                 self._cancelled.add(rid)
                 return True
         for slot, r in self.running.items():
@@ -229,20 +259,28 @@ class ContinuousBatcher:
             batch.append(r)
         if batch:
             args = ([r.slot for r in batch], [r.rid for r in batch], [r.embeds for r in batch], [r.trailing for r in batch])
+            kw = {}
             if any(r.sampling is not None for r in batch):
-                self.eng.admit(*args, sampling=[r.sampling for r in batch])   # None entries: the session's parameters
-            else:
-                self.eng.admit(*args)
+                kw["sampling"] = [r.sampling for r in batch]   # None entries: the session's parameters
+            if any(r.voice is not None for r in batch):
+                kw["prefixes"] = [r.voice.prefix_id if r.voice is not None else None for r in batch]
+            self.eng.admit(*args, **kw)
             for r in batch:
                 self.running[r.slot] = r
+                if r.voice is not None:
+                    r.voice.pending -= 1   # the slot has its own copy of the voice's K/V now
                 if r.text_open and not r.closed:
                     self.eng.set_text_open(r.slot, True)
             if self.cstream is not None:
                 seeded = [r for r in batch if r.ref_codes is not None]
-                if len(seeded) < len(batch):
-                    self.cstream.reset([r.slot for r in batch if r.ref_codes is None])
+                banked = [r for r in batch if r.voice is not None and r.voice.bank is not None]
+                if len(seeded) + len(banked) < len(batch):
+                    self.cstream.reset([r.slot for r in batch if r.ref_codes is None and not any(r is q for q in banked)])
                 if seeded:
                     self.cstream.seed([r.slot for r in seeded], [r.ref_codes for r in seeded])
+                for bank in sorted({r.voice.bank[0] for r in banked}):   # one copy per bank, no reference decode
+                    rs = [r for r in banked if r.voice.bank[0] == bank]
+                    self.cstream.copy_from(self.codec.bank_stream(bank), [r.voice.bank[1] for r in rs], [r.slot for r in rs])
         if not batch and not self._runnable():
             return {}, []   # every running row is open and waiting for text: launch nothing
         n = min([self.packet] + [r.max_frames - r.emitted for r in self.running.values()])

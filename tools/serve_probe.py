@@ -16,9 +16,16 @@ With --live-text TOKENS_PER_S every request is live (submit(text_open=True)): it
 and its other text rows (horizon // 3 of them, then tts_eos) are appended between steps at that rate from its submit
 time, after which it is closed.  The probe then also reports the share of row-steps held (the host's count of the
 engine's hold rule); first_chunk_ms is then the time from the first text token to the first audio chunk.
+With --voices K the requests are drawn from K registered voices, alternately ICL clones (a 38-frame reference and a
+24-token reference text: a 33-row prefix of 3 role, 6 codec-prefix and 24 reference rows, 15 rows of its own) and
+VoiceDesign voices (a 48-token instruct: a 56-row prefix, 1 row of its own), with the engine's random rows of those
+lengths.  Every request set runs registered (submit(voice=)) and unregistered (the whole prompt, and ref_codes for the
+clones), the two sessions alternated twice in one run.  The probe reports for each the median admission time (a host
+clock around the engine's admission and the codec-row setup of every step that admits, each ending in a device
+synchronise), the AR step and the first-chunk latency.
 
     python tools/serve_probe.py [--slots 8 32] [--requests-per-slot 3] [--packet 4] [--mix] [--voice-clone]
-                                [--live-text TOKENS_PER_S]
+                                [--live-text TOKENS_PER_S] [--voices K]
 
 Prints one JSON line.  Writes nothing.
 """
@@ -162,6 +169,100 @@ def run_session(eng, codec, pad, sp, prompts, n_slots, packet, horizons, timed, 
     return out
 
 
+VOICE_REF_TEXT, VOICE_INSTRUCT = 24, 48   # tokens
+VOICE_OVERLAY = 3 + 6                     # role rows and codec-prefix overlay rows (think, language, speaker, pad)
+
+
+def voice_session(eng, codec, pad, sp, reqs, n_slots, packet, horizons, registered):
+    """One session of `reqs` [(voice, own rows, full rows)]: registered requests submit their own rows with the voice,
+    unregistered ones the full rows and the reference codes.  Returns admission, AR-step and first-chunk times."""
+    from qwen3_tts_b200.scheduler import ContinuousBatcher
+    cb = ContinuousBatcher(eng, pad, sp, n_slots=n_slots, packet_frames=packet, codec=codec)
+    t_ar, t_admit = [], []
+    admitting = [0.0]
+
+    def clocked(fn, acc=None):
+        def call(*a, **k):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            r = fn(*a, **k)
+            torch.cuda.synchronize()
+            if acc is None:
+                admitting[0] += time.perf_counter() - t0
+            else:
+                acc.append(time.perf_counter() - t0)
+            return r
+        return call
+
+    eng.admit = clocked(type(eng).admit.__get__(eng))
+    eng.decode = clocked(type(eng).decode.__get__(eng), t_ar)
+    for name in ("seed", "copy_from", "reset"):
+        setattr(cb.cstream, name, clocked(getattr(cb.cstream, name)))
+    submitted, first = {}, {}
+
+    def submit(i):
+        v, own, full = reqs[i]
+        h = horizons[i % len(horizons)]
+        if registered:
+            cb.submit(own, None, key=i, max_frames=h, voice=v)
+        else:
+            cb.submit(full, None, key=i, max_frames=h, ref_codes=v.ref_codes)
+        submitted[i] = time.perf_counter()
+
+    todo = list(range(len(reqs)))
+    for i in todo[:n_slots]:
+        submit(i)
+    todo = todo[n_slots:]
+    try:
+        for chunks, _ in cb.stream():
+            now = time.perf_counter()
+            if admitting[0]:
+                t_admit.append(admitting[0])
+                admitting[0] = 0.0
+            for rid in chunks:
+                first.setdefault(rid, now - submitted[rid])
+            if todo:
+                submit(todo.pop(0))
+    finally:
+        del eng.admit, eng.decode
+        cb.cstream.close()
+    ms = lambda v: {"median": float(np.median(v)) * 1e3, "p90": float(np.percentile(v, 90)) * 1e3} if v else None  # noqa: E731
+    return {"admissions": len(t_admit), "admission_ms": ms(t_admit), "ar_ms_per_step": ms(t_ar),
+            "first_chunk_ms": ms(list(first.values()))}
+
+
+def voices_probe(eng, codec, pad, sp, S, K, n_req, packet, g):
+    """--voices K: K voices, requests i of voice i % K, registered and unregistered sessions alternated twice."""
+    from types import SimpleNamespace
+    H = eng.cfg.talker.hidden_size
+    voices = []
+    for k in range(K):
+        icl = k % 2 == 0
+        P = VOICE_OVERLAY + (VOICE_REF_TEXT if icl else VOICE_INSTRUCT)
+        prefix = (torch.randn(P, H, generator=g) * 0.5).bfloat16()
+        ref = torch.randint(0, codec.cfg.codebook_size, (REF_FRAMES, codec.cfg.num_quantizers), generator=g) if icl else None
+        v = SimpleNamespace(engine=eng, codec=codec, prefix=prefix, prefix_len=P, prefix_id=eng.create_prefix(prefix),
+                            ref_codes=ref, ref_len=REF_FRAMES if icl else 0, bank=codec.bank_reference(ref) if icl else None,
+                            own=REF_FRAMES + 1 - VOICE_REF_TEXT if icl else 1, pending=0, closed=False)
+        voices.append(v)
+    reqs = []
+    for i in range(n_req):
+        v = voices[i % K]
+        own = (torch.randn(v.own, H, generator=g) * 0.5).bfloat16()
+        reqs.append((v, own, torch.cat([v.prefix, own], 0)))
+    voice_session(eng, codec, pad, sp, reqs[:S], S, packet, (8,), True)      # warm-up: every shape
+    voice_session(eng, codec, pad, sp, reqs[:S], S, packet, (8,), False)
+    runs = {"registered": [], "unregistered": []}
+    for _ in range(2):
+        for mode in ("registered", "unregistered"):
+            runs[mode].append(voice_session(eng, codec, pad, sp, reqs, S, packet, HORIZONS, mode == "registered"))
+    for v in voices:
+        eng.free_prefix(v.prefix_id)
+        if v.bank is not None:
+            codec.bank_release(*v.bank)
+    return runs
+
+
 def naive_seed_ms(codec, n_slots, packet, ref, reps=5):
     """The path seeding avoids: one reference pushed through an n_slots-row stream of the session's packet size (every
     row computed each step, the other rows with count 0).  Sync-clocked; median over `reps` after one warm-up."""
@@ -195,6 +296,8 @@ def main():
                     help=f"every second request carries a {REF_FRAMES}-frame reference and a prompt longer by it")
     ap.add_argument("--live-text", type=float, default=None, metavar="TOKENS_PER_S",
                     help="every request is live: its text rows arrive at this rate after submit")
+    ap.add_argument("--voices", type=int, default=None, metavar="K",
+                    help="requests of K registered voices (ICL clones and VoiceDesign), run registered and unregistered")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("serve_probe needs a CUDA device")
@@ -205,7 +308,9 @@ def main():
     dev = "cuda:0"
     cfg, ccfg = synthetic.cfg_1p7b(), q.CodecConfig()
     max_b = max(args.slots)
-    extra = REF_FRAMES if args.voice_clone else 0   # the reference's frames in the prompt and in the codec row
+    extra = REF_FRAMES if (args.voice_clone or args.voices) else 0   # the reference's frames in the prompt and the codec row
+    if args.voices:
+        extra += VOICE_OVERLAY + VOICE_INSTRUCT
     eng = AREngine(cfg, synthetic.random_tts_weights(cfg, device="cpu", seed=0), device=dev, max_batch=max_b,
                    max_ctx=args.prompt_len + extra + max(HORIZONS) + 8)
     codec = CodecDecoder(ccfg, synthetic.random_codec_weights(ccfg, device="cpu", seed=0), device=dev,
@@ -224,6 +329,18 @@ def main():
     if args.voice_clone:
         out["voice_clone"] = (f"every second request: {REF_FRAMES}-frame reference of random valid codes, prompt "
                               f"{args.prompt_len + REF_FRAMES} positions instead of {args.prompt_len}")
+    if args.voices:
+        out["voices"] = (f"{args.voices} voices: ICL clones ({REF_FRAMES}-frame reference, {VOICE_REF_TEXT}-token reference "
+                         f"text) and VoiceDesign ({VOICE_INSTRUCT}-token instruct); registered and unregistered sessions "
+                         "alternated twice")
+        for S in args.slots:
+            out["results"][f"n_slots={S}"] = voices_probe(eng, codec, pad, sp, S, args.voices, S * args.requests_per_slot,
+                                                          args.packet, g)
+        out["card_after"] = card()
+        print(json.dumps(out))
+        codec.close()
+        eng.close()
+        return
     for S in args.slots:
         n_req = S * args.requests_per_slot
         refs = [torch.randint(0, ccfg.codebook_size, (REF_FRAMES, ccfg.num_quantizers), generator=g)
