@@ -58,7 +58,7 @@ __global__ void dwconv_ln_kernel(const bf16* __restrict__ x, const float* __rest
   const int bt = blockIdx.x;
   const int t = bt % T;
   const size_t xrow = (size_t)(bt / T) * x_bs_rows + hist + t;  // row of x that holds time step t of this batch row
-  float s1 = 0.f, s2 = 0.f;
+  float s1 = 0.f;
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     float acc = bias[c];
 #pragma unroll
@@ -69,16 +69,24 @@ __global__ void dwconv_ln_kernel(const bf16* __restrict__ x, const float* __rest
     acc = rbf(acc);
     sh[c] = acc;
     s1 += acc;
-    s2 += acc * acc;
   }
+  // two-pass variance, as F.layer_norm: a one-pass q / C - mean^2 loses about log2((mean / std)^2) bits of it
   float* red = sh + C;
-  s1 = warp_sum(s1); s2 = warp_sum(s2);
-  if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5] = s1; red[32 + (threadIdx.x >> 5)] = s2; }
+  const int nw = blockDim.x >> 5;
+  s1 = warp_sum(s1);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s1;
   __syncthreads();
-  float a = 0.f, q = 0.f;
-  for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { a += red[i]; q += red[32 + i]; }
+  float a = 0.f;
+  for (int i = 0; i < nw; ++i) a += red[i];
   const float mean = a / C;
-  const float var = fmaxf(q / C - mean * mean, 0.f);
+  float s2 = 0.f;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) { const float d = sh[c] - mean; s2 += d * d; }
+  s2 = warp_sum(s2);
+  if ((threadIdx.x & 31) == 0) red[32 + (threadIdx.x >> 5)] = s2;
+  __syncthreads();
+  float q = 0.f;
+  for (int i = 0; i < nw; ++i) q += red[32 + i];
+  const float var = q / C;
   const float inv = rsqrtf(var + 1e-6f);
   for (int c = threadIdx.x; c < C; c += blockDim.x) y[(size_t)bt * C + c] = f2bf((sh[c] - mean) * inv * lnw[c] + lnb[c]);
 }
