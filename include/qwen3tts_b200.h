@@ -173,6 +173,25 @@ int q3_append_trailing(q3_engine* e, int32_t slot, const void* rows_dev, int32_t
 int q3_set_trailing_open(q3_engine* e, int32_t slot, int32_t open);
 /* give up rows that reached their frame horizon without EOS (their slots become free) */
 int q3_release_slots(q3_engine* e, int32_t n, const int32_t* slots_host, void* stream);
+/* ---- parked rows (session only): a running request leaves its slot and later continues in any free slot.
+ * q3_row_park moves the request of `slot` (admitted, not finished, released or parked) into a record, a device block of
+ * the engine: its talker K/V at positions [0, pos) (pos = the position its next step writes) in the layout of a
+ * registered prefix, and every per-row state a frame-step reads before it writes it (the row's DevState fields, its
+ * repetition-penalty row, its code-predictor input rows, past_hidden / past_keep, its trailing text), plus on the host its
+ * committed frames, Philox key, sampling parameters and live-text flags.  One launch on `stream`, no host sync; the slot
+ * is then free as after q3_release_slots, and *id_out receives the record's id (never reused).  The caller's codes
+ * buffer is not saved.  q3_row_resume synchronises `stream` (it needs the frame counter, like an admission), puts record
+ * `id` into the free slot `slot` with one launch, synchronises again and frees the record: the request then generates
+ * exactly the frames it would have generated never parked, and q3_get_progress reports the same n_valid as before the
+ * park (committed frames + 1 for a row the last decode left held).  q3_row_discard frees a record without resuming it
+ * (after synchronising `stream`).  Records belong to their session: q3_session_begin, q3_prefill and q3_engine_destroy
+ * free them all.  Refused, before any device work and with every row, record and position unchanged, with an error
+ * naming the slot or id: not a session; a slot out of range or without a running request; hidden-state capture or
+ * teacher forcing set; resume into a running slot; an unknown, resumed or discarded id, or one of an earlier session;
+ * a record whose position would not fit max_ctx; a failed allocation (the row keeps running). */
+int q3_row_park(q3_engine* e, int32_t slot, void* stream, int32_t* id_out);
+int q3_row_resume(q3_engine* e, int32_t id, int32_t slot, void* stream);
+int q3_row_discard(q3_engine* e, int32_t id, void* stream);
 
 /* After synchronising `stream`: frames_done = frames whose 16 codes are complete (same for all rows);
  * n_valid[b] = frames of row b before its first EOS (== modeling_qwen3_tts.py:2283-2290 trim); for a row the last

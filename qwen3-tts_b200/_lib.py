@@ -63,7 +63,8 @@ AR_SYMBOLS = ["q3_abi_version", "q3_last_error", "q3_engine_create", "q3_engine_
               "q3_algorithmic_bytes", "q3_set_profile", "q3_describe_frame_program",
               "q3_session_begin", "q3_release_slots", "q3_append_trailing", "q3_set_hidden_capture",
               "q3_admit_with_sampling", "q3_sampling_check", "q3_set_trailing_open",
-              "q3_prefix_create", "q3_prefix_free", "q3_prefix_length", "q3_admit_with_prefix"]
+              "q3_prefix_create", "q3_prefix_free", "q3_prefix_length", "q3_admit_with_prefix",
+              "q3_row_park", "q3_row_resume", "q3_row_discard"]
 CODEC_SYMBOLS = ["q3_codec_create", "q3_codec_destroy", "q3_codec_load_tensor", "q3_codec_finalize",
                  "q3_codec_forward", "q3_codec_total_upsample", "q3_codec_last_launch_count", "q3_codec_debug_capture",
                  "q3_codec_stream_open", "q3_codec_stream_close",
@@ -125,6 +126,9 @@ def load():
     lib.q3_prefix_create.argtypes = [vp, vp, i32, vp, C.POINTER(i32)]
     lib.q3_prefix_free.argtypes = [vp, i32, vp]
     lib.q3_prefix_length.argtypes = [vp, i32]
+    lib.q3_row_park.argtypes = [vp, i32, vp, C.POINTER(i32)]
+    lib.q3_row_resume.argtypes = [vp, i32, i32, vp]
+    lib.q3_row_discard.argtypes = [vp, i32, vp]
     lib.q3_sampling_check.argtypes = [C.POINTER(Sampling)]
     lib.q3_get_progress.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
     lib.q3_set_debug.argtypes = [vp, vp, i32, vp, vp]

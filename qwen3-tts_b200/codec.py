@@ -266,7 +266,7 @@ class CodecDecoder:
         the full causal forward over everything pushed, for the cost of the new frames only."""
         return CodecStream(self, batch, max_packet_frames)
 
-    # ------------------------------------------------------------------ reference state bank (registered voices)
+    # ------------------------------------------------------------------ state bank (registered voices, parked requests)
     def bank_reference(self, codes: torch.Tensor) -> Tuple[int, int]:
         """Decode reference codes ((L, K), the layout of VoiceClonePromptItem.ref_code) once into a row of a bank
         stream of this decoder and return (bank, row).  A row copied from it (CodecStream.copy_from(bank_stream(bank),
@@ -274,6 +274,33 @@ class CodecDecoder:
         rows; it grows by opening a larger stream and copying its rows over, so (bank, row) stays valid until
         bank_release.  Bank streams take no packets: they are opened with packets of one frame."""
         check_ref_codes(self.cfg, codes, self.max_frames, "reference codes")
+        bank, row = self._bank_row()
+        st = self._banks[bank]
+        try:
+            st.seed([row], [codes])
+        except Exception:
+            self.bank_release(bank, row)
+            raise
+        st._seeder.close()      # registration is rare: the private seed stream is not kept
+        st._seeder = None
+        return bank, row
+
+    def bank_copy(self, src: "CodecStream", src_row: int) -> Tuple[int, int]:
+        """Copy row `src_row` of a stream of this decoder, its whole causal state and position, into a bank row and
+        return (bank, row), as bank_reference does for a reference (a parked request's codec row).  Copying it back with
+        CodecStream.copy_from(bank_stream(bank), [row], [slot]) restores exactly that state; bank_release frees it."""
+        if not 0 <= int(src_row) < src.B:
+            raise ValueError(f"source row {src_row} out of range [0, {src.B})")
+        bank, row = self._bank_row()
+        try:
+            self._banks[bank].copy_from(src, [int(src_row)], [row])
+        except Exception:
+            self.bank_release(bank, row)
+            raise
+        return bank, row
+
+    def _bank_row(self) -> Tuple[int, int]:
+        """A free row of a bank stream, growing a bank or adding one when every row is in use; marked used."""
         bank = next((i for i, used in enumerate(self._bank_used) if len(used) < self.max_batch), None)
         if bank is None:
             self._banks.append(None)
@@ -288,11 +315,7 @@ class CodecDecoder:
                 torch.cuda.current_stream(self.device).synchronize()   # the copy reads the old stream
                 old.close()
             self._banks[bank] = grown
-        st = self._banks[bank]
-        row = min(set(range(st.B)) - used)
-        st.seed([row], [codes])
-        st._seeder.close()      # registration is rare: the private seed stream is not kept
-        st._seeder = None
+        row = min(set(range(self._banks[bank].B)) - used)
         used.add(row)
         return bank, row
 

@@ -134,6 +134,17 @@ struct q3_engine {
   struct Prefix { bf16* kv; int len; };
   std::map<int, Prefix> prefixes;
   int next_prefix = 0;
+  // parked rows of the current session (q3_row_park): a device block each, laid out by record_layout, and the host state
+  // that resume restores.  Ids count on across sessions; first_record is the first id of the current one.
+  struct Record {
+    unsigned char* blk;
+    int pos, f, trailing_len;  // position of the row's next step, its committed frames, its trailing rows
+    unsigned int key;
+    q3_sampling sp;
+    bool text_open, held;
+  };
+  std::map<int, Record> records;
+  int next_record = 0, first_record = 0;
 
   ~q3_engine() {
     if (copy_stream) cudaStreamDestroy(copy_stream);
@@ -685,10 +696,22 @@ static int check_admission(const q3_engine* e, const Admission& A, int B, int ca
   return 0;
 }
 
+// Free every parked row's record: a park's gather may still be queued on `stream`
+static int free_records(q3_engine* e, cudaStream_t stream) {
+  if (!e->records.empty()) Q3_CUDA(cudaStreamSynchronize(stream));
+  for (auto& kv : e->records)
+    if (e->store.release(kv.second.blk)) return 1;
+  e->records.clear();
+  e->first_record = e->next_record;
+  return 0;
+}
+
 // A batch of B slots, every row finished (an empty slot is a finished row: it keeps stepping, like HF's padded rows, and
-// is ignored), sampling with the default sp, room for max_trailing rows of trailing text per slot.
+// is ignored), sampling with the default sp, room for max_trailing rows of trailing text per slot.  Records of parked
+// rows belong to the session they were parked in and are freed.
 static int reset_rows(q3_engine* e, int B, int max_trailing, const void* tts_pad_dev, const q3_sampling& sp, bool session,
                       cudaStream_t stream) {
+  if (free_records(e, stream)) return 1;
   if (build_programs(e, B)) return 1;
   e->B = B; e->sp = sp; e->session = session;
   DevState hs;
@@ -930,6 +953,128 @@ extern "C" int q3_release_slots(q3_engine* e, int32_t n, const int32_t* slots_ho
   }
   if (n > 0) release_state_kernel<<<1, 32, 0, (cudaStream_t)stream_>>>(e->st, A);
   return 0;
+}
+
+// ---- parked rows: a running request's state moves out of its slot into a record and back into any free slot --------
+// Record block: [2][layers * nkv][pos][HD] bf16 talker K/V (a registered prefix's layout), then the x_cp rows of blocks
+// 0 and 1, past_hidden and past_keep ([4][H] bf16), the trailing text [trailing_len][H] bf16, the seen bytes [V] and the
+// DevState ints.  Every piece starts on a 16-byte boundary (H % 32 == 0, V % 16 == 0).
+struct RecordLayout { size_t kv, rows, text, seen, ints, bytes; };
+static RecordLayout record_layout(const q3_engine* e, int pos, int trailing_len) {
+  const q3_stack_cfg& tc = e->cfg.talker;
+  const size_t H = tc.hidden_size;
+  RecordLayout L;
+  L.kv = 0;
+  L.rows = L.kv + (size_t)2 * tc.num_layers * tc.num_kv_heads * pos * HD * sizeof(bf16);
+  L.text = L.rows + 4 * H * sizeof(bf16);
+  L.seen = L.text + (size_t)trailing_len * H * sizeof(bf16);
+  L.ints = L.seen + (size_t)tc.vocab_size;
+  L.bytes = L.ints + kRowInts * sizeof(int);
+  return L;
+}
+
+// The one launch of a park (kResume false) or a resume of record R in slot b
+template <bool kResume>
+static int launch_row_move(q3_engine* e, const q3_engine::Record& R, int b, cudaStream_t stream) {
+  const q3_stack_cfg& tc = e->cfg.talker;
+  const int H = tc.hidden_size, V = tc.vocab_size;
+  const RecordLayout L = record_layout(e, R.pos, R.trailing_len);
+  bf16* xcp = e->cfg.has_cp_projection ? e->x_cp : e->cp.h;  // what KParams::x_cp points at: [2][B][H]
+  const bf16* rows[4] = {xcp + (size_t)b * H, xcp + ((size_t)e->B + b) * H, e->past_hidden + (size_t)b * H,
+                         e->past_keep + (size_t)b * H};
+  RowMove M{};
+  for (int k = 0; k < 4; ++k)
+    M.span[k] = RowSpan{(uint4*)rows[k], (uint4*)(R.blk + L.rows + (size_t)k * H * sizeof(bf16)), H / 8};
+  M.span[4] = RowSpan{(uint4*)(e->trailing + (size_t)b * e->trailing_cap * H), (uint4*)(R.blk + L.text), R.trailing_len * H / 8};
+  M.span[5] = RowSpan{(uint4*)(e->seen + (size_t)b * V), (uint4*)(R.blk + L.seen), V / 16};
+  M.kc = reinterpret_cast<uint4*>(e->talker.kc); M.vc = reinterpret_cast<uint4*>(e->talker.vc);
+  M.kv = reinterpret_cast<uint4*>(R.blk + L.kv);
+  M.lh = tc.num_layers * tc.num_kv_heads; M.cap = e->talker.cap; M.pos = R.pos; M.slot = b;
+  M.ints = reinterpret_cast<int*>(R.blk + L.ints);
+  const size_t work = std::max<size_t>((size_t)M.lh * R.pos * (HD / 8), (size_t)std::max(V / 16, R.trailing_len * H / 8));
+  const int grid = (int)std::min<size_t>((work + 255) / 256, (size_t)e->sm_count * 8);
+  row_move_kernel<kResume><<<std::max(grid, 1), 256, 0, stream>>>(M, e->st);
+  Q3_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// The rules park and resume share: a session without hidden-state capture or teacher forcing (the rules of live text)
+static int check_row_move(const q3_engine* e, const char* what) {
+  Q3_REQUIRE(e && e->finalized && e->session, "%s: q3_session_begin first (rows are parked only in a session)", what);
+  Q3_REQUIRE(!e->hid_out && !e->forced, "%s: not available while hidden-state capture or teacher forcing is set", what);
+  return 0;
+}
+
+static int record_missing(const q3_engine* e, int id) {
+  if (id >= 0 && id < e->first_record) return q3_set_err("record %d belongs to an earlier session", id);
+  return q3_set_err("record %d does not exist (never parked, or already resumed or discarded)", id);
+}
+
+extern "C" int q3_row_park(q3_engine* e, int32_t slot, void* stream_, int32_t* id_out) {
+  if (check_row_move(e, "q3_row_park")) return 1;
+  Q3_REQUIRE(id_out, "null argument");
+  Q3_REQUIRE(slot >= 0 && slot < e->B, "q3_row_park: slot %d out of range", slot);
+  Q3_REQUIRE(e->active[slot], "q3_row_park: slot %d has no running request (never admitted, finished, released or parked)", slot);
+  Q3_CUDA(cudaSetDevice(e->cfg.device));
+  q3_engine::Record R{};
+  R.pos = e->len0[slot] + e->frames_issued;
+  R.f = e->frames_issued - e->frame0[slot];
+  R.trailing_len = e->trailing_len[slot];
+  R.key = e->row_key[slot]; R.sp = e->row_sp[slot]; R.text_open = e->text_open[slot]; R.held = e->held[slot];
+  // no zero fill: the launch writes every byte that resume reads, and a zeroed block would drain the device
+  if (e->store.alloc(&R.blk, record_layout(e, R.pos, R.trailing_len).bytes, false)) return 1;
+  if (launch_row_move<false>(e, R, slot, (cudaStream_t)stream_)) {
+    cudaStreamSynchronize((cudaStream_t)stream_);
+    e->store.release(R.blk);
+    return 1;
+  }
+  e->active[slot] = e->text_open[slot] = e->held[slot] = false;
+  const int id = e->next_record++;
+  e->records[id] = R;
+  *id_out = id;
+  return 0;
+}
+
+extern "C" int q3_row_resume(q3_engine* e, int32_t id, int32_t slot, void* stream_) {
+  if (check_row_move(e, "q3_row_resume")) return 1;
+  const auto it = e->records.find(id);
+  if (it == e->records.end()) return record_missing(e, id);
+  const q3_engine::Record R = it->second;
+  Q3_REQUIRE(slot >= 0 && slot < e->B, "q3_row_resume: slot %d out of range", slot);
+  Q3_REQUIRE(R.pos < e->cfg.max_ctx, "record %d: its next position %d does not fit max_ctx %d", id, R.pos, e->cfg.max_ctx);
+  Q3_CUDA(cudaSetDevice(e->cfg.device));
+  cudaStream_t stream = (cudaStream_t)stream_;
+  // the global frame at which the row continues = frames completed so far, as for an admission
+  DevState hs;
+  Q3_CUDA(cudaStreamSynchronize(stream));
+  Q3_CUDA(cudaMemcpy(&hs, e->st, sizeof(hs), cudaMemcpyDeviceToHost));
+  Q3_REQUIRE(hs.error == 0, "device-side error %d", hs.error);
+  Q3_REQUIRE(!(e->active[slot] && !hs.finished[slot]), "q3_row_resume: slot %d is still running (park or release it first)", slot);
+  const int F = hs.step;
+  if (launch_row_move<true>(e, R, slot, stream)) return 1;
+  // the row's frame counter (frame - frame0) and position (len0 + frame) continue from where they were at the park
+  e->frame0[slot] = F - R.f; e->len0[slot] = R.pos - F; e->trailing_len[slot] = R.trailing_len;
+  e->row_key[slot] = R.key; e->row_sp[slot] = R.sp; e->text_open[slot] = R.text_open; e->held[slot] = R.held;
+  e->active[slot] = true;
+  e->frames_issued = F;
+  e->max_len0 = 1;
+  for (int b = 0; b < e->B; ++b)
+    if (e->active[b]) e->max_len0 = std::max(e->max_len0, e->len0[b]);
+  // the record is freed once the launch that reads it is done
+  Q3_CUDA(cudaStreamSynchronize(stream));
+  e->records.erase(id);
+  return e->store.release(R.blk);
+}
+
+extern "C" int q3_row_discard(q3_engine* e, int32_t id, void* stream_) {
+  Q3_REQUIRE(e && e->finalized && e->session, "q3_row_discard: q3_session_begin first");
+  const auto it = e->records.find(id);
+  if (it == e->records.end()) return record_missing(e, id);
+  Q3_CUDA(cudaSetDevice(e->cfg.device));
+  Q3_CUDA(cudaStreamSynchronize((cudaStream_t)stream_));  // the park's gather may still be queued
+  unsigned char* blk = it->second.blk;
+  e->records.erase(it);
+  return e->store.release(blk);
 }
 
 extern "C" int q3_get_progress(q3_engine* e, int32_t* frames_done, int32_t* n_valid, int32_t* finished) {

@@ -56,6 +56,26 @@ struct PfPrefix {
   uint4 *kc, *vc;
   int lh, cap;
 };
+// Talker K/V of sequence b at positions [0, len) between the caches kc / vc ([seq][lh][cap][HD]) and a block in the
+// registered-prefix layout ([2 (K, V)][lh][len][HD]), in 16-byte chunks: thread i of `stride` threads copies chunks i,
+// i + stride, ... of K and of V, into the caches (kToCache) or out of them into the block
+template <bool kToCache>
+__device__ __forceinline__ void kv_block_copy(uint4* blk, uint4* kc, uint4* vc, int lh, int cap, int b, int len, size_t i,
+                                              size_t stride) {
+  const int row = len * (HD / 8);
+  const size_t n = (size_t)lh * row;
+  for (size_t j = i; j < n; j += stride) {
+    const size_t l = j / row, c = j - l * row, d = ((size_t)b * lh + l) * cap * (HD / 8) + c;
+    if (kToCache) {
+      kc[d] = blk[j];
+      vc[d] = blk[n + j];
+    } else {
+      blk[j] = kc[d];
+      blk[n + j] = vc[d];
+    }
+  }
+}
+
 // grid (x, row r): slice r resets row r's device state and seen bytes, gathers its trailing text (element-wise: the
 // source may be any bf16 pointer) and copies its prefix K/V; slice 0 also writes the token index
 __global__ void pf_index_kernel(PfLens L, PfRows R, PfPrefix X, DevState* st, unsigned char* seen, int V, int* tok_seq, int* tok_pos) {
@@ -72,13 +92,49 @@ __global__ void pf_index_kernel(PfLens L, PfRows R, PfPrefix X, DevState* st, un
   }
   if (i < V) seen[(size_t)b * V + i] = 0;
   if (i < R.trailing_len[r] * R.H) R.dst[(size_t)b * R.cap * R.H + i] = R.src[(size_t)r * R.stride * R.H + i];
-  if (X.kv[r]) {  // one 16-byte chunk of K and one of V per thread and step; a position is HD / 8 chunks
-    const int row = L.p0[r] * (HD / 8);
-    const size_t n = (size_t)X.lh * row;
-    for (size_t j = i; j < n; j += (size_t)gridDim.x * blockDim.x) {
-      const size_t lh = j / row, c = j - lh * row, d = ((size_t)b * X.lh + lh) * X.cap * (HD / 8) + c;
-      X.kc[d] = X.kv[r][j];
-      X.vc[d] = X.kv[r][n + j];
+  if (X.kv[r])  // one 16-byte chunk of K and one of V per thread and step; a position is HD / 8 chunks
+    kv_block_copy<true>(const_cast<uint4*>(X.kv[r]), X.kc, X.vc, X.lh, X.cap, b, L.p0[r], i, (size_t)gridDim.x * blockDim.x);
+}
+
+// A parked row (q3_row_park / q3_row_resume): its talker K/V at positions [0, pos) go to or come from the record's block
+// kv (kv_block_copy, the layout of a registered prefix); every other piece of its state that a frame-step reads before
+// it writes it is a span of 16-byte chunks on the slot's side and in the record, and its DevState fields are ints
+constexpr int kRowSpans = 6;                        // x_cp rows of blocks 0 and 1, past_hidden, past_keep, trailing text, seen
+constexpr int kRowInts = 6 + Q3_NUM_GROUPS_MAX;     // len0, finished, n_valid, n_gen, c0, trailing_len, cur[0..]
+struct RowSpan { uint4* slot; uint4* rec; int n; };
+struct RowMove {
+  RowSpan span[kRowSpans];
+  uint4 *kc, *vc, *kv;
+  int lh, cap, pos, slot;
+  int* ints;
+};
+// kResume = false (park): gather the slot into the record, then mark the slot's row finished as release_state_kernel
+// does; kResume = true: scatter the record into the slot.  Any grid: every thread strides over every piece.
+template <bool kResume>
+__global__ void row_move_kernel(RowMove M, DevState* st) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
+  kv_block_copy<kResume>(M.kv, M.kc, M.vc, M.lh, M.cap, M.slot, M.pos, i, stride);
+#pragma unroll 1
+  for (int s = 0; s < kRowSpans; ++s) {
+    const RowSpan& S = M.span[s];
+    for (size_t j = i; j < (size_t)S.n; j += stride) {
+      if (kResume) S.slot[j] = S.rec[j];
+      else S.rec[j] = S.slot[j];
+    }
+  }
+  if (i == 0) {
+    const int b = M.slot;
+    int* f[kRowInts];
+    f[0] = &st->len0[b]; f[1] = &st->finished[b]; f[2] = &st->n_valid[b]; f[3] = &st->n_gen[b]; f[4] = &st->c0[b];
+    f[5] = &st->trailing_len[b];
+    for (int g = 0; g < Q3_NUM_GROUPS_MAX; ++g) f[6 + g] = &st->cur[b][g];
+    for (int k = 0; k < kRowInts; ++k) {
+      if (kResume) *f[k] = M.ints[k];
+      else M.ints[k] = *f[k];
+    }
+    if (!kResume && !st->finished[b]) {
+      st->finished[b] = 1;
+      st->n_valid[b] = 0x3fffffff;
     }
   }
 }

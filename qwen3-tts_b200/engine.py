@@ -235,6 +235,26 @@ class AREngine:
         stream = torch.cuda.current_stream(self.device).cuda_stream
         _lib.check(self.lib.q3_release_slots(self.h, n, (C.c_int32 * max(n, 1))(*[int(x) for x in slots]), C.c_void_p(stream)))
 
+    def park(self, slot: int) -> int:
+        """Move the running request of `slot` out of the session into a record on the device (q3_row_park): its talker
+        K/V and every per-row state the frame-step reads.  The slot is free afterwards, as after release_slots.  The
+        caller keeps the request's codes, which live in its own buffer.  Returns the record id for resume / discard."""
+        out = C.c_int32()
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        _lib.check(self.lib.q3_row_park(self.h, int(slot), C.c_void_p(stream), C.byref(out)))
+        return out.value
+
+    def resume(self, record: int, slot: int):
+        """Continue a parked request in the free slot `slot` of the same session (q3_row_resume): it generates exactly
+        what it would have generated never parked.  The record is consumed."""
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        _lib.check(self.lib.q3_row_resume(self.h, int(record), int(slot), C.c_void_p(stream)))
+
+    def discard(self, record: int):
+        """Free a parked request's record without resuming it (q3_row_discard)."""
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        _lib.check(self.lib.q3_row_discard(self.h, int(record), C.c_void_p(stream)))
+
     def decode(self, max_frames: int, codes: torch.Tensor):
         """codes: int32 [B][stride][G] device tensor that accumulates frames across calls."""
         assert codes.dtype == torch.int32 and codes.is_cuda and codes.is_contiguous()

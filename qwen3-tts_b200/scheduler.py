@@ -42,6 +42,15 @@ admits a request or some running row can produce a frame: a closed row always ca
 the frames it has reported.  Otherwise the step launches nothing and returns no frames, and `stream()` / `packets()`
 yield empty results, so a single-threaded caller feeds text between iterations.  `cancel` drops a request, pending or
 running (a client that disconnected).
+
+Parking: a running request can leave its slot and continue later in any free slot (AREngine.park / resume): its talker
+K/V and row state wait in an engine record, its codes so far on the request, its codec row in a row of the decoder's
+bank (CodecDecoder.bank_copy), so it generates and streams exactly what it would have never parked
+(tests/test_gpu_park.py).  `park(rid)` / `resume(rid)` do this on request, for example for a client that stopped
+reading.  With `park_waiting=True` the batcher parks live-text requests that wait for text whenever a pending or a
+resumable parked request needs a slot and none is free, and resumes them once their text covers their next frame.
+Each step parks first, then resumes parked requests into free slots (oldest park first, ahead of admissions), then
+admits.
 """
 from collections import deque
 from dataclasses import dataclass, field
@@ -66,18 +75,26 @@ class _Request:
     voice: Optional[Any] = None   # a registered voice (model.Voice): its prompt prefix and reference state
     text_open: bool = False    # submitted with text that may still grow
     closed: bool = False       # close_text() was called
-    n_text: int = 0            # trailing rows given so far
+    n_text: int = 0            # trailing rows given so far (`trailing`: those the engine does not have yet)
     slot: int = -1
     emitted: int = 0
     chunks: List[torch.Tensor] = field(default_factory=list)
+    paused: bool = False       # park(rid) without resume(rid): not admitted, parked at the next step, not resumed
+    record: int = -1           # while parked: the engine's record, the codec bank row and the codes so far
+    bank: Optional[Tuple[int, int]] = None
+    codes: Optional[torch.Tensor] = None
 
 
 class ContinuousBatcher:
     def __init__(self, engine: AREngine, tts_pad_embed: torch.Tensor, sp: SamplingParams, n_slots: int = 8, packet_frames: int = 4,
-                 max_trailing: int = 256, codec: Union[CodecDecoder, CodecStream, None] = None):
+                 max_trailing: int = 256, codec: Union[CodecDecoder, CodecStream, None] = None, park_waiting: bool = False):
         """`codec`: a CodecDecoder, whose stream of `n_slots` rows the batcher opens, or an open CodecStream of
-        `n_slots` rows taking packets of at least `packet_frames` frames."""
+        `n_slots` rows taking packets of at least `packet_frames` frames.  `park_waiting`: park running live-text
+        requests that wait for text when another request needs their slot (see the module docstring)."""
         self.eng, self.sp = engine, sp
+        self.park_waiting = bool(park_waiting)
+        self.parked: Dict[int, _Request] = {}      # request id -> parked request, oldest park first
+        self.moves: List[Tuple[str, int, int]] = []   # ("park" | "resume", request id, slot), in order
         self.n_slots, self.packet = int(n_slots), int(packet_frames)
         self.G = engine.cfg.num_code_groups
         self.max_frames = max(int(sp.max_new_tokens) - 1, 1)
@@ -162,12 +179,18 @@ class ContinuousBatcher:
             voice.pending += 1
         return rid
 
-    def _live(self, rid: int, what: str) -> _Request:
-        """The pending or running request `rid` whose text is still open, else ValueError."""
-        r = next((q for q in self.pending if q.rid == rid), None) or next((q for q in self.running.values() if q.rid == rid), None)
+    def _find(self, rid: int, what: str) -> _Request:
+        """The pending, running or parked request `rid`, else ValueError."""
+        r = next((q for q in self.pending if q.rid == rid), None) or next((q for q in self.running.values() if q.rid == rid), None) \
+            or self.parked.get(rid)
         if r is None:
             state = "was cancelled" if rid in self._cancelled else "has finished" if rid in self.done else "is unknown"
             raise ValueError(f"{what}: request {rid} {state}")
+        return r
+
+    def _live(self, rid: int, what: str) -> _Request:
+        """The pending, running or parked request `rid` whose text is still open, else ValueError."""
+        r = self._find(rid, what)
         if not r.text_open:
             raise ValueError(f"{what}: request {rid} was not submitted with text_open=True")
         if r.closed:
@@ -175,7 +198,7 @@ class ContinuousBatcher:
         return r
 
     def append_text(self, rid: int, rows: torch.Tensor):
-        """More trailing text rows (n, H) for an open request, pending or running (Qwen3TTSModel.live_text_rows makes
+        """More trailing text rows (n, H) for an open request, pending, running or parked (Qwen3TTSModel.live_text_rows makes
         them from a piece of text).  ValueError for an unknown, finished or cancelled request, one that was not
         submitted open or is already closed, or text beyond max_trailing."""
         r = self._live(rid, "append_text")
@@ -217,7 +240,67 @@ class ContinuousBatcher:
                 del self.running[slot]
                 self._cancelled.add(rid)
                 return True
+        r = self.parked.pop(rid, None)
+        if r is not None:    # its record and its codec bank row are freed
+            self.eng.discard(r.record)
+            if r.bank is not None:
+                self.codec.bank_release(*r.bank)
+            self._cancelled.add(rid)
+            return True
         return False
+
+    def park(self, rid: int):
+        """Take request `rid` out of its slot until resume(rid): a running request is parked at the next step boundary
+        (its slot is then free for others), a pending one is not admitted.  ValueError for an unknown, finished or
+        cancelled request."""
+        self._find(rid, "park").paused = True
+
+    def resume(self, rid: int):
+        """Make a request of park(rid) eligible again: a parked one is resumed into the next free slot (a live-text
+        request once its text covers its next frame), a pending one may be admitted, a running one stays.  ValueError as
+        for park."""
+        self._find(rid, "resume").paused = False
+
+    def _waiting(self, r: _Request) -> bool:
+        """An open live-text request whose text does not cover its next frame (the negation of _runnable's test)."""
+        return r.text_open and not r.closed and r.n_text < r.emitted
+
+    def _resumable(self, r: _Request) -> bool:
+        return not r.paused and not self._waiting(r)
+
+    def _park(self, slot: int):
+        """Park the running request of `slot`: its engine row into a record, its codes so far onto the request, its codec
+        row into a bank row."""
+        r = self.running.pop(slot)
+        r.codes = self.codes[slot, :r.emitted].clone()
+        r.record = self.eng.park(slot)
+        if self.cstream is not None:
+            r.bank = self.codec.bank_copy(self.cstream, slot)
+        r.trailing = r.trailing.reshape(-1, self.eng.cfg.talker.hidden_size)[:0]   # the record holds the text so far
+        r.slot = -1
+        self.parked[r.rid] = r
+        self.moves.append(("park", r.rid, slot))
+
+    def _resume(self, r: _Request, slot: int):
+        """Put parked request r into the free slot `slot`: the engine row, its codes, its codec row, the text that
+        arrived while it was parked and its live-text state."""
+        self.eng.resume(r.record, slot)
+        del self.parked[r.rid]
+        r.record, r.slot = -1, slot
+        self.running[slot] = r
+        if r.emitted > 0:
+            self.codes[slot, :r.emitted] = r.codes
+        r.codes = None
+        if r.bank is not None:
+            self.cstream.copy_from(self.codec.bank_stream(r.bank[0]), [r.bank[1]], [slot])
+            self.codec.bank_release(*r.bank)   # a later bank_copy into that row is queued behind this copy
+            r.bank = None
+        if r.trailing.shape[0] > 0:
+            self.eng.append_trailing(slot, r.trailing)
+            r.trailing = r.trailing[:0]
+        if r.text_open:
+            self.eng.set_text_open(slot, not r.closed)
+        self.moves.append(("resume", r.rid, slot))
 
     def step(self) -> List[int]:
         """Admit what fits, decode one packet, collect what finished.  Returns the ids that completed in this step."""
@@ -227,19 +310,19 @@ class ContinuousBatcher:
 
     def stream(self) -> Iterator[Tuple[Dict[int, np.ndarray], List[int]]]:
         """Run the session with audio out: yields per step ({request id: float32 waveform of its new frames},
-        [ids that finished in the step]) while requests are pending or running, so a request submitted between two
-        iterations is admitted at the next one."""
+        [ids that finished in the step]) while requests are pending, running or parked, so a request submitted between
+        two iterations is admitted at the next one."""
         if self.cstream is None:
             raise ValueError("stream() needs a ContinuousBatcher built with a codec")
-        while self.pending or self.running:
+        while self.pending or self.running or self.parked:
             new, finished = self._advance()
             yield self._push_audio(new), finished
 
     def packets(self) -> Iterator[Tuple[Dict[int, torch.Tensor], List[int]]]:
         """Run the session with codes out: yields per step ({request id: (k, G) int64 codes of its k new frames},
-        [ids that finished in the step]) while requests are pending or running.  The codec stream, if any, is not
-        pushed."""
-        while self.pending or self.running:
+        [ids that finished in the step]) while requests are pending, running or parked.  The codec stream, if any, is
+        not pushed."""
+        while self.pending or self.running or self.parked:
             new, finished = self._advance()
             yield {r.rid: self.codes[slot, e0:e0 + k].to(torch.int64) for slot, (r, e0, k) in new.items() if k > 0}, finished
 
@@ -251,10 +334,25 @@ class ContinuousBatcher:
 
     def _advance(self):
         """One step of the session: ({slot: (request, first new frame, new frames)}, [ids that finished])."""
+        # parks: requests of park(rid), then as many waiting live-text requests as the others need slots
+        for slot, r in list(self.running.items()):
+            if r.paused:
+                self._park(slot)
+        if self.park_waiting:
+            short = sum(not r.paused for r in self.pending) + sum(self._resumable(r) for r in self.parked.values()) \
+                - (self.n_slots - len(self.running))
+            for slot, r in list(self.running.items()):
+                if short <= 0:
+                    break
+                if self._waiting(r):
+                    self._park(slot)
+                    short -= 1
         free = [s for s in range(self.n_slots) if s not in self.running]
+        for r in [q for q in self.parked.values() if self._resumable(q)][:len(free)]:   # oldest park first
+            self._resume(r, free.pop(0))
         batch = []
-        while free and self.pending:
-            r = self.pending.popleft()
+        for r in [q for q in self.pending if not q.paused][:len(free)]:
+            self.pending.remove(r)
             r.slot = free.pop(0)
             batch.append(r)
         if batch:
@@ -323,10 +421,18 @@ class ContinuousBatcher:
 
     def run(self) -> Dict[int, torch.Tensor]:
         """Drain the queue; returns {request id: (N_i, G) codes}.  Requests with open text must be closed first (or
-        be fed through step() / stream() / packets()): run() raises ValueError when every running request waits for
-        text."""
-        while self.pending or self.running:
-            if not self._runnable() and not (self.pending and len(self.running) < self.n_slots):
+        be fed through step() / stream() / packets()): run() raises ValueError when nothing pending, running or parked
+        can make progress (every running request waits for text, and no other request can take a slot)."""
+        while self.pending or self.running or self.parked:
+            if not self._runnable() and not self._can_enter():
                 raise ValueError("every running request waits for text: close_text() them, or feed them between step()s")
             self.step()
         return self.done
+
+    def _can_enter(self) -> bool:
+        """Some pending or resumable parked request can take a slot at the next step: one is free, or will be freed by
+        a park."""
+        if not (any(not r.paused for r in self.pending) or any(self._resumable(r) for r in self.parked.values())):
+            return False
+        return len(self.running) < self.n_slots or any(r.paused or (self.park_waiting and self._waiting(r))
+                                                       for r in self.running.values())

@@ -16,6 +16,10 @@ With --live-text TOKENS_PER_S every request is live (submit(text_open=True)): it
 and its other text rows (horizon // 3 of them, then tts_eos) are appended between steps at that rate from its submit
 time, after which it is closed.  The probe then also reports the share of row-steps held (the host's count of the
 engine's hold rule); first_chunk_ms is then the time from the first text token to the first audio chunk.
+With --park (with --live-text) the batcher parks live requests that wait for text when another request needs a slot
+(ContinuousBatcher(park_waiting=True)).  The probe then also reports parks and resumes per wall second, the time of an
+engine park and resume (host clock around the call, ending in a device synchronise), the park kernel's time (CUDA
+events around the call, which only enqueues it) and the record bytes it gathers over that time.
 With --voices K the requests are drawn from K registered voices, alternately ICL clones (a 38-frame reference and a
 24-token reference text: a 33-row prefix of 3 role, 6 codec-prefix and 24 reference rows, 15 rows of its own) and
 VoiceDesign voices (a 48-token instruct: a 56-row prefix, 1 row of its own), with the engine's random rows of those
@@ -25,7 +29,7 @@ clock around the engine's admission and the codec-row setup of every step that a
 synchronise), the AR step and the first-chunk latency.
 
     python tools/serve_probe.py [--slots 8 32] [--requests-per-slot 3] [--packet 4] [--mix] [--voice-clone]
-                                [--live-text TOKENS_PER_S] [--voices K]
+                                [--live-text TOKENS_PER_S [--park]] [--voices K]
 
 Prints one JSON line.  Writes nothing.
 """
@@ -68,13 +72,22 @@ def mixed_sampling(sp, i):
     return None
 
 
-def run_session(eng, codec, pad, sp, prompts, n_slots, packet, horizons, timed, mix=False, refs=None, live=None, texts=None):
+def record_bytes(eng, pos, trailing):
+    """Bytes of a parked row's record (q3_row_park): talker K/V of pos positions, 4 hidden rows, the trailing text,
+    the seen bytes and the DevState ints."""
+    t, G = eng.cfg.talker, 16
+    return 2 * t.num_layers * t.num_kv_heads * pos * t.head_dim * 2 + (4 + trailing) * t.hidden_size * 2 + t.vocab_size + (6 + G) * 4
+
+
+def run_session(eng, codec, pad, sp, prompts, n_slots, packet, horizons, timed, mix=False, refs=None, live=None, texts=None,
+                park=False):
     """One session: n_slots requests at once, then one more per step until all are in.  refs[i]: request i's
     reference codes or None.  live: text rows per second (texts[i]: request i's rows after the first token, tts_eos
     last), or None.  Returns the measurements."""
     from qwen3_tts_b200.scheduler import ContinuousBatcher
-    cb = ContinuousBatcher(eng, pad, sp, n_slots=n_slots, packet_frames=packet, codec=codec)
+    cb = ContinuousBatcher(eng, pad, sp, n_slots=n_slots, packet_frames=packet, codec=codec, park_waiting=park)
     t_ar, t_codec, t_seed = [], [], []
+    t_park, t_resume, k_park, b_park = [], [], [], []
     refs = refs or [None] * len(prompts)
 
     def clocked(fn, acc):
@@ -101,9 +114,37 @@ def run_session(eng, codec, pad, sp, prompts, n_slots, packet, horizons, timed, 
             return fn(n, codes)
         return call
 
+    moving = [None]   # the request the batcher is parking or resuming
+
+    def watch(fn):
+        def call(*a):
+            moving[0] = cb.running[a[0]] if fn.__name__ == "_park" else a[0]
+            return fn(*a)
+        return call
+
+    def clocked_park(fn):
+        def call(slot):
+            r = moving[0]
+            torch.cuda.synchronize()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            t0 = time.perf_counter()
+            e0.record()
+            out = fn(slot)
+            e1.record()
+            torch.cuda.synchronize()
+            t_park.append(time.perf_counter() - t0)
+            k_park.append(e0.elapsed_time(e1) * 1e-3)
+            b_park.append(record_bytes(eng, prompts[r.rid].shape[0] + committed.get(r.rid, 0), r.n_text))
+            return out
+        return call
+
     decode = type(eng).decode.__get__(eng)
     if timed:
         decode = clocked(decode, t_ar)
+        if park:
+            cb._park, cb._resume = watch(cb._park), watch(cb._resume)
+            eng.park = clocked_park(type(eng).park.__get__(eng))
+            eng.resume = clocked(type(eng).resume.__get__(eng), t_resume)
     if live:
         decode = count_holds(decode)
     if timed or live:
@@ -151,6 +192,8 @@ def run_session(eng, codec, pad, sp, prompts, n_slots, packet, horizons, timed, 
     finally:
         if timed or live:
             del eng.decode
+        if timed and park:
+            del eng.park, eng.resume
         cb.cstream.close()
     wall = time.perf_counter() - t0
     ms = lambda v: {"median": float(np.median(v)) * 1e3, "p90": float(np.percentile(v, 90)) * 1e3} if v else None  # noqa: E731
@@ -159,6 +202,11 @@ def run_session(eng, codec, pad, sp, prompts, n_slots, packet, horizons, timed, 
            "audio_s_per_wall_s": samples / SAMPLE_RATE / wall}
     if live:
         out["held_row_step_share"] = held[0] / max(held[1], 1)
+    if park:
+        out.update({"parks": len(t_park), "resumes": len(t_resume), "parks_per_s": len(t_park) / wall,
+                    "resumes_per_s": len(t_resume) / wall, "park_ms": ms(t_park), "resume_ms": ms(t_resume),
+                    "park_kernel_ms": ms(k_park), "park_record_mb": ms([b / 1e9 for b in b_park]),   # (ms() scales by 1e3)
+                    "park_gb_per_s": ms([b / k / 1e12 for b, k in zip(b_park, k_park)])})
     if any(r is not None for r in refs):
         out["first_chunk_ms_voice_clone"] = ms([t for rid, t in first.items() if refs[rid] is not None])
         out["first_chunk_ms_plain"] = ms([t for rid, t in first.items() if refs[rid] is None])
@@ -296,9 +344,12 @@ def main():
                     help=f"every second request carries a {REF_FRAMES}-frame reference and a prompt longer by it")
     ap.add_argument("--live-text", type=float, default=None, metavar="TOKENS_PER_S",
                     help="every request is live: its text rows arrive at this rate after submit")
+    ap.add_argument("--park", action="store_true", help="with --live-text: park requests that wait for text when a slot is needed")
     ap.add_argument("--voices", type=int, default=None, metavar="K",
                     help="requests of K registered voices (ICL clones and VoiceDesign), run registered and unregistered")
     args = ap.parse_args()
+    if args.park and not args.live_text:
+        raise SystemExit("--park needs --live-text")
     if not torch.cuda.is_available():
         raise SystemExit("serve_probe needs a CUDA device")
     import qwen3_tts_b200 as q
@@ -326,6 +377,8 @@ def main():
     if args.live_text:
         out["live_text"] = (f"every request live: {args.live_text:g} text tokens/s from submit, horizon // 3 tokens "
                             "after the first, then tts_eos and close")
+        out["park"] = "park_waiting=True" if args.park else "no parking"
+
     if args.voice_clone:
         out["voice_clone"] = (f"every second request: {REF_FRAMES}-frame reference of random valid codes, prompt "
                               f"{args.prompt_len + REF_FRAMES} positions instead of {args.prompt_len}")
@@ -350,9 +403,9 @@ def main():
         texts = [torch.cat([(torch.randn(HORIZONS[i % len(HORIZONS)] // 3, H, generator=g) * 0.1).bfloat16(),
                             (torch.randn(1, H, generator=g) * 0.1).bfloat16()]) for i in range(n_req)] if args.live_text else None
         run_session(eng, codec, pad, sp, prompts[:S], S, args.packet, (8,), timed=False, mix=args.mix,
-                    refs=refs[:S], live=args.live_text, texts=texts)   # warm-up: every shape
+                    refs=refs[:S], live=args.live_text, texts=texts, park=args.park)   # warm-up: every shape
         res = run_session(eng, codec, pad, sp, prompts, S, args.packet, HORIZONS, timed=True, mix=args.mix, refs=refs,
-                          live=args.live_text, texts=texts)
+                          live=args.live_text, texts=texts, park=args.park)
         if args.voice_clone:
             res["naive_push_ms_per_admission"] = naive_seed_ms(codec, S, args.packet, refs[1])
         out["results"][f"n_slots={S}"] = res
