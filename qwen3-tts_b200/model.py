@@ -154,10 +154,12 @@ class Qwen3TTSForConditionalGenerationB200:
         return text_embed + codec_embed, tts_pad_embed
 
     # ------------------------------------------------------------------ batched prefill assembly (SURVEY §8f-3)
-    def _plan_sample(self, input_id, instruct, ref_id, vcp, index, language, speaker, non_streaming_mode):
+    def _plan_sample(self, input_id, instruct, ref_id, vcp, index, language, speaker, non_streaming_mode, live=False):
         """Index plan of one sample (:2086-2234): every prefill / trailing position is `TP(text id) + codec source`
         with either side optional.  Returns (text_ids, codec_src, trailing_ids); text id -1 = no text part; codec_src
-        entries: None | ("ce", id) | ("spk",) | ("icl", frame)."""
+        entries: None | ("ce", id) | ("spk",) | ("icl", frame).  `live` (streaming ICL layout only): the ids are the
+        text known so far, the text stream has no tts_eos yet, and the ICL positions its text has not reached carry their
+        codec part alone (text id -1)."""
         cfg = self.cfg
         ids = [int(x) for x in input_id.reshape(-1).tolist()]
         BOS, EOS, PAD = cfg.tts_bos_token_id, cfg.tts_eos_token_id, cfg.tts_pad_token_id
@@ -202,11 +204,14 @@ class Qwen3TTSForConditionalGenerationB200:
         icl = vcp is not None and vcp["ref_code"] is not None and vcp["icl_mode"][index]
         if icl:                                              # generate_icl_prompt (:1968-2019)
             rid = [int(x) for x in ref_id.reshape(-1).tolist()][3:-2]
-            tstream = rid + ids[3:-5] + [EOS]
+            tstream = rid + ids[3:-5] + ([] if live else [EOS])
             n_ref = int(vcp["ref_code"][index].shape[0])
             cstream = [("ce", cfg.codec_bos_id)] + [("icl", t) for t in range(n_ref)]
             Lt, Lc = len(tstream), len(cstream)
-            if non_streaming_mode:
+            if live:
+                text += tstream[:Lc] + [-1] * (Lc - min(Lt, Lc)); codec += cstream
+                trailing = tstream[Lc:]
+            elif non_streaming_mode:
                 text += tstream + [PAD] * Lc
                 codec += [("ce", cfg.codec_pad_id)] * Lt + cstream
                 trailing = [PAD]
@@ -235,7 +240,6 @@ class Qwen3TTSForConditionalGenerationB200:
         frames, one add) instead of dozens of small launches per sample.  The index plan is host-side integer work;
         `build_prefill_per_sample` is the statement-by-statement restatement it must equal.  The reference's left
         padding / attention mask (:2239-2254) is not materialised: the engine takes per-sequence lengths."""
-        cfg, dev = self.cfg, self.device
         n = len(input_ids)
         if speakers is None:
             speakers = [None] * n
@@ -244,6 +248,12 @@ class Qwen3TTSForConditionalGenerationB200:
             ins = instruct_ids[i] if instruct_ids is not None else None
             rid = ref_ids[i] if ref_ids is not None else None
             plans.append(self._plan_sample(input_ids[i], ins, rid, voice_clone_prompt, i, languages[i], speakers[i], non_streaming_mode))
+        return self._embed_plans(plans, voice_clone_prompt)
+
+    def _embed_plans(self, plans, voice_clone_prompt):
+        """The rows of index plans (_plan_sample) with build_prefill's batched launches: (per-sample prompt rows,
+        per-sample trailing rows, tts_pad_embed)."""
+        cfg, dev = self.cfg, self.device
         H = self.codec_embedding.shape[1]
         # ---- text side: every text id of every sample (prefill + trailing) + the three specials, ONE ResizeMLP
         flat_text, seg = [], []
@@ -308,10 +318,36 @@ class Qwen3TTSForConditionalGenerationB200:
             if int(ids.reshape(-1).shape[0]) < 9:   # 3 role tokens, >= 1 text token, 5 closing tokens
                 raise ValueError(f"request {i}: live text needs at least one text token in the prefill")
             if vcp is not None and vcp["ref_code"] is not None and vcp["icl_mode"][i]:
-                raise ValueError(f"request {i}: an ICL voice-clone prompt cannot take live text (its prefill consumes the "
-                                 f"target text); use an x-vector-only prompt")
+                raise ValueError(f"request {i}: an ICL voice-clone prompt cannot take live text here (its prefill consumes "
+                                 f"the target text); use build_live_icl_prefill")
         embeds, trailing, pad = self.build_prefill(input_ids, instruct_ids, None, vcp, languages, speakers, non_streaming_mode=False)
         return embeds, [t[:-1] for t in trailing], pad
+
+    @torch.no_grad()
+    def build_live_icl_prefill(self, input_ids, ref_ids, voice_clone_prompt, languages):
+        """Live text for ICL voice-clone prompts in the streaming layout (:1968-2019): (inputs_embeds, trailing,
+        tts_pad_embed, overlay), lists per sample but the pad.  The ICL block's position j sums the text stream
+        (reference text R tokens, target text, tts_eos) and the codec stream (codec_bos, the reference's frames: Lc =
+        1 + frames), so its last K = max(0, Lc - R) positions each wait for one row of target text.  `inputs_embeds`
+        are the prompt rows complete with the text known so far (the first min(K, T) target tokens summed onto their
+        reference rows), `overlay` the (K - min(K, T), H) codec parts of the positions still waiting, in order, and
+        `trailing` the known text rows past the ICL block, without tts_eos.  The text's later rows (text_rows, then
+        tts_eos_row) complete the overlay first (overlay[i] + row) and then continue the trailing rows; if the text ends
+        first, the rest of the overlay takes tts_pad_embed and the trailing rows are [tts_pad].  The rows are then
+        exactly those of build_prefill(non_streaming_mode=False) over all the ids.  A text without tokens is accepted;
+        every prompt must be an ICL one (the others take build_live_prefill)."""
+        vcp = voice_clone_prompt
+        for i in range(len(input_ids)):
+            if vcp is None or vcp["ref_code"] is None or vcp["ref_code"][i] is None or not vcp["icl_mode"][i]:
+                raise ValueError(f"request {i}: not an ICL voice-clone prompt; live text of other prompts takes "
+                                 f"build_live_prefill")
+            if int(input_ids[i].reshape(-1).shape[0]) < 8:   # 3 role tokens, 5 closing tokens
+                raise ValueError(f"request {i}: the ids lack the chat wrapper's 3 role and 5 closing tokens")
+        plans = [self._plan_sample(input_ids[i], None, ref_ids[i], vcp, i, languages[i], None, False, live=True)
+                 for i in range(len(input_ids))]
+        embeds, trailing, pad = self._embed_plans(plans, vcp)
+        n_over = [sum(t < 0 for t in text[-int(vcp["ref_code"][i].shape[0]) - 1:]) for i, (text, _, _) in enumerate(plans)]
+        return [e[:e.shape[0] - k] for e, k in zip(embeds, n_over)], trailing, pad, [e[e.shape[0] - k:] for e, k in zip(embeds, n_over)]
 
     @torch.no_grad()
     def text_rows(self, ids) -> torch.Tensor:
@@ -815,6 +851,45 @@ class Qwen3TTSModel:
                                                               speakers=[speaker])
         return embeds[0], trailing[0], pad
 
+    def build_live_clone_request(self, text, voice_clone_prompt=None, voice: Optional["Voice"] = None, language=None):
+        """One live request of an ICL voice clone for ContinuousBatcher.submit(inputs_embeds, trailing_text,
+        text_open=True, overlay=overlay, ref_codes= / voice=): (inputs_embeds, trailing_text, tts_pad_embed, overlay) of
+        the streaming layout for the text known so far (`text`, which may be empty).  Either `voice_clone_prompt`, one
+        ICL item (with ref_codes=item.ref_code at submit), or `voice`, an ICL voice registered with
+        non_streaming_mode=False, whose inputs_embeds are the rows after voice.prefix as build_voice_request returns
+        them (the voice fixes the language).  The prompt's last K = max(0, Lc - R) positions overlay the reference's
+        last frames with target text (Lc = 1 + reference frames, R = reference text tokens), so the request is admitted
+        once K text rows have arrived or its text is closed (Qwen3TTSForConditionalGenerationB200.build_live_icl_prefill).
+        Feed it as any live request (live_text_rows, live_text_end, close_text); it then generates what the whole
+        text's ids generate up front (non_streaming_mode=False).  Other prompts and voices take build_live_request and
+        build_voice_request(live=True)."""
+        if isinstance(text, list):
+            raise ValueError("build_live_clone_request takes one text")
+        if (voice is None) == (voice_clone_prompt is None):
+            raise ValueError("build_live_clone_request takes one of voice_clone_prompt and voice")
+        if voice is not None:
+            if voice.closed:
+                raise ValueError("the voice is closed")
+            if not voice.icl:
+                raise ValueError("not an ICL voice: a live request of it takes build_voice_request(text, voice, live=True)")
+            if voice.non_streaming_mode:
+                raise ValueError("live text needs a voice registered with non_streaming_mode=False (the non-streaming ICL "
+                                 "layout puts the whole text before the reference codes)")
+            if language is not None:
+                raise ValueError("a registered voice fixes its language")
+            input_ids = self._tokenize_texts([self._build_assistant_text(text)])
+            e, t, p, o = self.model.build_live_icl_prefill(input_ids, voice.ref_ids, voice.vcp, [voice.language])
+            return e[0][voice.prefix_len:], t[0], p, o[0]
+        items = voice_clone_prompt if isinstance(voice_clone_prompt, list) else [voice_clone_prompt]
+        if len(items) != 1 or not isinstance(items[0], VoiceClonePromptItem):
+            raise ValueError("build_live_clone_request takes one VoiceClonePromptItem")
+        if items[0].ref_code is None or not items[0].icl_mode:
+            raise ValueError("not an ICL voice-clone prompt: a live request of it takes build_live_request")
+        input_ids, ref_ids, vcp, languages = self._voice_clone_inputs(text, language, None, None, False, items,
+                                                                      "build_live_clone_request")
+        e, t, p, o = self.model.build_live_icl_prefill(input_ids, ref_ids, vcp, languages)
+        return e[0], t[0], p, o[0]
+
     def live_text_rows(self, text: str) -> torch.Tensor:
         """Trailing rows (n, H) of one more piece of a live request's text: its token ids with no chat wrapper."""
         ids = self.processor(text=text, return_tensors="pt", padding=True)["input_ids"]
@@ -1011,13 +1086,15 @@ class Qwen3TTSModel:
         """One request of a registered voice for ContinuousBatcher.submit(suffix_embeds, trailing, voice=voice):
         (suffix_embeds, trailing_text, tts_pad_embed), where cat(voice.prefix, suffix_embeds) and trailing_text are
         the rows build_prefill makes for the same request.  With `live=True` the trailing rows end without tts_eos,
-        as in build_live_request (submit with text_open=True); ICL voices refuse it."""
+        as in build_live_request (submit with text_open=True); ICL voices refuse it (build_live_clone_request)."""
         if voice.closed:
             raise ValueError("the voice is closed")
         if isinstance(text, list):
             raise ValueError("build_voice_request takes one text")
         if live and voice.non_streaming_mode:
             raise ValueError("live text needs a voice registered with non_streaming_mode=False")
+        if live and voice.icl:
+            raise ValueError("a live request of an ICL voice takes build_live_clone_request")
         embeds, trailing, pad, _ = self._voice_rows(voice, text, live)
         return embeds[voice.prefix_len:], trailing, pad
 

@@ -51,6 +51,14 @@ reading.  With `park_waiting=True` the batcher parks live-text requests that wai
 resumable parked request needs a slot and none is free, and resumes them once their text covers their next frame.
 Each step parks first, then resumes parked requests into free slots (oldest park first, ahead of admissions), then
 admits.
+
+Live text of an ICL voice clone (`submit(..., text_open=True, overlay=)`, Qwen3TTSModel.build_live_clone_request): the
+last positions of its prompt overlay reference codes with target text, one text row each, so its prompt is complete
+only once that many text rows have arrived.  Text rows fill the overlay first (row i of the prompt becomes overlay[i] +
+text row, the bf16 add of build_prefill), later rows are trailing text; a close_text before the overlay is full
+completes it with tts_pad and makes the trailing text [tts_pad], build_prefill's layout for a short text.  Until then
+the request is not admitted, takes no slot a park would free, and does not keep run() going; once complete it is
+admitted and runs as any live request, so it generates what its whole text gives up front (tests/test_gpu_live_clone.py).
 """
 from collections import deque
 from dataclasses import dataclass, field
@@ -83,6 +91,7 @@ class _Request:
     record: int = -1           # while parked: the engine's record, the codec bank row and the codes so far
     bank: Optional[Tuple[int, int]] = None
     codes: Optional[torch.Tensor] = None
+    overlay: Optional[torch.Tensor] = None   # prompt rows still waiting for a text row each (None once complete)
 
 
 class ContinuousBatcher:
@@ -91,7 +100,7 @@ class ContinuousBatcher:
         """`codec`: a CodecDecoder, whose stream of `n_slots` rows the batcher opens, or an open CodecStream of
         `n_slots` rows taking packets of at least `packet_frames` frames.  `park_waiting`: park running live-text
         requests that wait for text when another request needs their slot (see the module docstring)."""
-        self.eng, self.sp = engine, sp
+        self.eng, self.sp, self.pad = engine, sp, tts_pad_embed
         self.park_waiting = bool(park_waiting)
         self.parked: Dict[int, _Request] = {}      # request id -> parked request, oldest park first
         self.moves: List[Tuple[str, int, int]] = []   # ("park" | "resume", request id, slot), in order
@@ -121,7 +130,8 @@ class ContinuousBatcher:
     # ------------------------------------------------------------------ API
     def submit(self, inputs_embeds: torch.Tensor, trailing_text: Optional[torch.Tensor] = None, key: Optional[int] = None,
                max_frames: Optional[int] = None, sampling: Optional[SamplingParams] = None,
-               ref_codes: Optional[torch.Tensor] = None, text_open: bool = False, voice=None) -> int:
+               ref_codes: Optional[torch.Tensor] = None, text_open: bool = False, voice=None,
+               overlay: Optional[torch.Tensor] = None) -> int:
         """Queue one request; returns its id (also its Philox row key unless `key` is given).  `sampling`: the
         request's own generation parameters (default: the session's); its max_new_tokens bounds the request's horizon
         and may not exceed the session's.  `ref_codes`: (L, num_quantizers) reference codes of a voice-clone request
@@ -131,10 +141,22 @@ class ContinuousBatcher:
         voice (Qwen3TTSModel.register_voice) of this engine, and of this codec if it clones with a reference; the prompt
         is then the voice's prefix followed by `inputs_embeds` (the suffix of Qwen3TTSModel.build_voice_request), the
         prefix's K/V are copied at admission instead of prefilled, and an ICL voice's codec row is copied from its
-        reference state instead of decoding the reference.  It takes no `ref_codes`.  Bad parameters raise ValueError
-        here, never in a later step()."""
+        reference state instead of decoding the reference.  It takes no `ref_codes`.  `overlay`: (K, H) prompt rows of
+        a live ICL voice clone that still wait for one text row each (Qwen3TTSModel.build_live_clone_request); it needs
+        `text_open`, and an ICL voice if it has a voice.  The trailing rows given here and later fill it first, and the
+        request is admitted once it is full or its text is closed (see the module docstring).  Bad parameters raise
+        ValueError here, never in a later step()."""
         H = self.eng.cfg.talker.hidden_size
         L_ref, P = 0, 0
+        if overlay is not None:
+            if not text_open:
+                raise ValueError("an overlay waits for text: submit it with text_open=True")
+            if overlay.dim() != 2 or overlay.shape[1] != H:
+                raise ValueError(f"overlay must be a (K, {H}) tensor, got {tuple(overlay.shape)}")
+            if voice is not None and (not voice.icl or voice.non_streaming_mode):
+                raise ValueError("an overlay belongs to an ICL voice registered with non_streaming_mode=False")
+            if self.max_trailing < 1:
+                raise ValueError("an overlay may end in a tts_pad trailing row: it needs max_trailing >= 1")
         if voice is not None:
             if ref_codes is not None:
                 raise ValueError("a registered voice carries its own reference: submit it without ref_codes")
@@ -161,20 +183,25 @@ class ContinuousBatcher:
         rid = self._next_id if key is None else int(key)
         self._next_id = max(self._next_id, rid) + 1
         tr = trailing_text if trailing_text is not None else torch.zeros(0, H)
-        if tr.reshape(-1, H).shape[0] > self.max_trailing:
+        K = 0 if overlay is None else int(overlay.shape[0])
+        if max(tr.reshape(-1, H).shape[0] - K, 0) > self.max_trailing:
             raise ValueError(f"trailing text of {tr.shape[0]} positions exceeds max_trailing={self.max_trailing}")
         S = int(inputs_embeds.reshape(-1, H).shape[0])
-        if voice is not None and S < 1:
+        if voice is not None and S + K < 1:
             raise ValueError("a request of a registered voice needs at least one row of its own")
-        L = P + S
+        L = P + S + K
         room = self.eng.max_ctx - L
         if room < 1:
             raise ValueError(f"prompt of {L} positions does not fit max_ctx={self.eng.max_ctx}")
         horizon = min(limit if max_frames is None else max_frames, limit, room)
         if self.codec is not None:
             horizon = min(horizon, self.codec.max_frames - L_ref)  # a codec row's position may not pass its RoPE table
-        self.pending.append(_Request(rid, inputs_embeds, tr, horizon, sampling, ref_codes, voice, text_open=bool(text_open),
-                                     n_text=int(tr.reshape(-1, H).shape[0])))
+        r = _Request(rid, inputs_embeds, tr, horizon, sampling, ref_codes, voice, text_open=bool(text_open),
+                     overlay=overlay if K else None)
+        if r.overlay is not None:
+            r.trailing = self._fill(r, tr.reshape(-1, H))
+        r.n_text = int(r.trailing.reshape(-1, H).shape[0])
+        self.pending.append(r)
         if voice is not None:
             voice.pending += 1
         return rid
@@ -204,9 +231,12 @@ class ContinuousBatcher:
         r = self._live(rid, "append_text")
         H = self.eng.cfg.talker.hidden_size
         rows = rows.reshape(-1, H)
-        if r.n_text + rows.shape[0] > self.max_trailing:
-            raise ValueError(f"append_text: request {rid} would have {r.n_text + rows.shape[0]} trailing rows, more than "
+        n = rows.shape[0] - (0 if r.overlay is None else min(r.overlay.shape[0], rows.shape[0]))
+        if r.n_text + n > self.max_trailing:
+            raise ValueError(f"append_text: request {rid} would have {r.n_text + n} trailing rows, more than "
                              f"max_trailing={self.max_trailing}")
+        if r.overlay is not None:
+            rows = self._fill(r, rows)
         if rows.shape[0] == 0:
             return
         if r.slot >= 0:
@@ -220,8 +250,22 @@ class ContinuousBatcher:
         reads tts_pad and ends.  ValueError as for append_text."""
         r = self._live(rid, "close_text")
         r.closed = True
+        if r.overlay is not None:   # the text ended inside the overlay: build_prefill's layout of a short text
+            pad = self.pad.reshape(1, -1)
+            self._fill(r, pad.expand(r.overlay.shape[0], -1))
+            r.trailing, r.n_text = pad, 1
         if r.slot >= 0:
             self.eng.set_text_open(r.slot, False)
+
+    def _fill(self, r: _Request, rows: torch.Tensor) -> torch.Tensor:
+        """Text rows (n, H) of pending request r go to its overlay first: each completes the next waiting prompt row
+        (overlay row + text row, in bf16 as build_prefill adds them).  Returns the rows left over, trailing text."""
+        m = min(r.overlay.shape[0], rows.shape[0])
+        if m:
+            done = r.overlay[:m] + rows[:m].to(r.overlay.device, r.overlay.dtype)
+            r.embeds = torch.cat([r.embeds.reshape(-1, done.shape[1]).to(done.device, done.dtype), done], 0)
+            r.overlay = r.overlay[m:] if m < r.overlay.shape[0] else None
+        return rows[m:]
 
     def cancel(self, rid: int) -> bool:
         """Drop request `rid`: a pending one leaves the queue, a running one's slot is released (its codec row is reset
@@ -267,6 +311,11 @@ class ContinuousBatcher:
 
     def _resumable(self, r: _Request) -> bool:
         return not r.paused and not self._waiting(r)
+
+    @staticmethod
+    def _admissible(r: _Request) -> bool:
+        """A pending request that may take a slot: not paused, and its prompt complete (no overlay waits for text)."""
+        return not r.paused and r.overlay is None
 
     def _park(self, slot: int):
         """Park the running request of `slot`: its engine row into a record, its codes so far onto the request, its codec
@@ -339,7 +388,7 @@ class ContinuousBatcher:
             if r.paused:
                 self._park(slot)
         if self.park_waiting:
-            short = sum(not r.paused for r in self.pending) + sum(self._resumable(r) for r in self.parked.values()) \
+            short = sum(self._admissible(r) for r in self.pending) + sum(self._resumable(r) for r in self.parked.values()) \
                 - (self.n_slots - len(self.running))
             for slot, r in list(self.running.items()):
                 if short <= 0:
@@ -351,7 +400,7 @@ class ContinuousBatcher:
         for r in [q for q in self.parked.values() if self._resumable(q)][:len(free)]:   # oldest park first
             self._resume(r, free.pop(0))
         batch = []
-        for r in [q for q in self.pending if not q.paused][:len(free)]:
+        for r in [q for q in self.pending if self._admissible(q)][:len(free)]:
             self.pending.remove(r)
             r.slot = free.pop(0)
             batch.append(r)
@@ -422,17 +471,18 @@ class ContinuousBatcher:
     def run(self) -> Dict[int, torch.Tensor]:
         """Drain the queue; returns {request id: (N_i, G) codes}.  Requests with open text must be closed first (or
         be fed through step() / stream() / packets()): run() raises ValueError when nothing pending, running or parked
-        can make progress (every running request waits for text, and no other request can take a slot)."""
+        can make progress (every running request waits for text, and no other request can take a slot: pending ones
+        whose overlay waits for text cannot)."""
         while self.pending or self.running or self.parked:
             if not self._runnable() and not self._can_enter():
-                raise ValueError("every running request waits for text: close_text() them, or feed them between step()s")
+                raise ValueError("every request waits for text: close_text() them, or feed them between step()s")
             self.step()
         return self.done
 
     def _can_enter(self) -> bool:
         """Some pending or resumable parked request can take a slot at the next step: one is free, or will be freed by
         a park."""
-        if not (any(not r.paused for r in self.pending) or any(self._resumable(r) for r in self.parked.values())):
+        if not (any(self._admissible(r) for r in self.pending) or any(self._resumable(r) for r in self.parked.values())):
             return False
         return len(self.running) < self.n_slots or any(r.paused or (self.park_waiting and self._waiting(r))
                                                        for r in self.running.values())

@@ -27,9 +27,15 @@ lengths.  Every request set runs registered (submit(voice=)) and unregistered (t
 clones), the two sessions alternated twice in one run.  The probe reports for each the median admission time (a host
 clock around the engine's admission and the codec-row setup of every step that admits, each ending in a device
 synchronise), the AR step and the first-chunk latency.
+With --live-clone (with --live-text) every request is a live ICL voice clone (a 38-frame reference and a 24-token
+reference text, so K = 39 - 24 = 15 prompt rows wait for target text), alternately unregistered (the known prompt rows
+and ref_codes) and of a registered voice (no rows of its own but the overlay).  Its first text row is given at submit,
+the next K + horizon // 3 rows and tts_eos arrive at TOKENS_PER_S from then, and it is then closed.  The probe reports
+the AR step, the time from the first text row to the admission (host clock after the engine's admission and a device
+synchronise) and from the admission to the first audio chunk, over all requests and for each kind.
 
     python tools/serve_probe.py [--slots 8 32] [--requests-per-slot 3] [--packet 4] [--mix] [--voice-clone]
-                                [--live-text TOKENS_PER_S [--park]] [--voices K]
+                                [--live-text TOKENS_PER_S [--park | --live-clone]] [--voices K]
 
 Prints one JSON line.  Writes nothing.
 """
@@ -311,6 +317,105 @@ def voices_probe(eng, codec, pad, sp, S, K, n_req, packet, g):
     return runs
 
 
+def live_clone_session(eng, codec, pad, sp, reqs, n_slots, packet, horizons, rate):
+    """One session of live ICL clones `reqs` [(voice or None, known prompt rows, overlay, text rows with tts_eos last,
+    reference codes)]: n_slots requests at once, then one more per step; a request's first text row comes with submit,
+    the others at `rate` rows per second from then, after which it is closed."""
+    from qwen3_tts_b200.scheduler import ContinuousBatcher
+    cb = ContinuousBatcher(eng, pad, sp, n_slots=n_slots, packet_frames=packet, codec=codec)
+    t_ar, admitted = [], {}
+
+    def clocked_admit(fn):
+        def call(slots, keys, *a, **k):
+            r = fn(slots, keys, *a, **k)
+            torch.cuda.synchronize()
+            now = time.perf_counter()
+            for key in keys:
+                admitted[key] = now
+            return r
+        return call
+
+    def clocked(fn):
+        def call(*a, **k):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            r = fn(*a, **k)
+            torch.cuda.synchronize()
+            t_ar.append(time.perf_counter() - t0)
+            return r
+        return call
+
+    eng.admit = clocked_admit(type(eng).admit.__get__(eng))
+    eng.decode = clocked(type(eng).decode.__get__(eng))
+    submitted, first, fed = {}, {}, {}
+
+    def submit(i):
+        v, known, ov, text, ref = reqs[i]
+        kw = {"voice": v} if v is not None else {"ref_codes": ref}
+        cb.submit(known, text[:1], key=i, max_frames=horizons[i % len(horizons)], text_open=True, overlay=ov, **kw)
+        submitted[i], fed[i] = time.perf_counter(), 1
+
+    def feed(now):
+        for rid in list(fed):
+            text = reqs[rid][3]
+            due = min(1 + int((now - submitted[rid]) * rate), text.shape[0])
+            if due > fed[rid]:
+                cb.append_text(rid, text[fed[rid]:due])
+                fed[rid] = due
+            if fed[rid] == text.shape[0]:
+                cb.close_text(rid)
+                del fed[rid]
+
+    todo = list(range(len(reqs)))
+    for i in todo[:n_slots]:
+        submit(i)
+    todo = todo[n_slots:]
+    try:
+        for chunks, _ in cb.stream():
+            now = time.perf_counter()
+            for rid in chunks:
+                first.setdefault(rid, now - admitted[rid])
+            if todo:
+                submit(todo.pop(0))
+            feed(time.perf_counter())
+    finally:
+        del eng.admit, eng.decode
+        cb.cstream.close()
+    ms = lambda v: {"median": float(np.median(v)) * 1e3, "p90": float(np.percentile(v, 90)) * 1e3} if v else None  # noqa: E731
+    out = {"requests": len(reqs), "steps": len(t_ar), "ar_ms_per_step": ms(t_ar)}
+    for name, pick in (("all", lambda i: True), ("unregistered", lambda i: reqs[i][0] is None),
+                       ("registered", lambda i: reqs[i][0] is not None)):
+        out[name] = {"first_token_to_admission_ms": ms([admitted[i] - submitted[i] for i in admitted if pick(i)]),
+                     "admission_to_first_chunk_ms": ms([t for i, t in first.items() if pick(i)])}
+    return out
+
+
+def live_clone_probe(eng, codec, pad, sp, S, n_req, packet, rate, g):
+    """--live-clone: requests alternately unregistered and of one registered ICL voice; one warm-up session, then the
+    timed one."""
+    from types import SimpleNamespace
+    H = eng.cfg.talker.hidden_size
+    P = VOICE_OVERLAY + VOICE_REF_TEXT
+    K = REF_FRAMES + 1 - VOICE_REF_TEXT
+    prefix = (torch.randn(P, H, generator=g) * 0.5).bfloat16()
+    ref = torch.randint(0, codec.cfg.codebook_size, (REF_FRAMES, codec.cfg.num_quantizers), generator=g)
+    voice = SimpleNamespace(engine=eng, codec=codec, prefix=prefix, prefix_len=P, prefix_id=eng.create_prefix(prefix),
+                            ref_codes=ref, ref_len=REF_FRAMES, bank=codec.bank_reference(ref), icl=True,
+                            non_streaming_mode=False, pending=0, closed=False)
+    reqs = []
+    for i in range(n_req):
+        v = voice if i % 2 else None
+        known = prefix[:0] if v is not None else prefix
+        ov = (torch.randn(K, H, generator=g) * 0.5).bfloat16()
+        text = (torch.randn(K + HORIZONS[i % len(HORIZONS)] // 3 + 1, H, generator=g) * 0.1).bfloat16()
+        reqs.append((v, known, ov, text, ref))
+    live_clone_session(eng, codec, pad, sp, reqs[:S], S, packet, (8,), rate)   # warm-up: every shape
+    res = live_clone_session(eng, codec, pad, sp, reqs, S, packet, HORIZONS, rate)
+    eng.free_prefix(voice.prefix_id)
+    codec.bank_release(*voice.bank)
+    return res
+
+
 def naive_seed_ms(codec, n_slots, packet, ref, reps=5):
     """The path seeding avoids: one reference pushed through an n_slots-row stream of the session's packet size (every
     row computed each step, the other rows with count 0).  Sync-clocked; median over `reps` after one warm-up."""
@@ -345,11 +450,15 @@ def main():
     ap.add_argument("--live-text", type=float, default=None, metavar="TOKENS_PER_S",
                     help="every request is live: its text rows arrive at this rate after submit")
     ap.add_argument("--park", action="store_true", help="with --live-text: park requests that wait for text when a slot is needed")
+    ap.add_argument("--live-clone", action="store_true",
+                    help="with --live-text: every request is a live ICL voice clone, unregistered and registered")
     ap.add_argument("--voices", type=int, default=None, metavar="K",
                     help="requests of K registered voices (ICL clones and VoiceDesign), run registered and unregistered")
     args = ap.parse_args()
-    if args.park and not args.live_text:
-        raise SystemExit("--park needs --live-text")
+    if (args.park or args.live_clone) and not args.live_text:
+        raise SystemExit("--park and --live-clone need --live-text")
+    if args.park and args.live_clone:
+        raise SystemExit("--park and --live-clone are separate probes")
     if not torch.cuda.is_available():
         raise SystemExit("serve_probe needs a CUDA device")
     import qwen3_tts_b200 as q
@@ -359,7 +468,7 @@ def main():
     dev = "cuda:0"
     cfg, ccfg = synthetic.cfg_1p7b(), q.CodecConfig()
     max_b = max(args.slots)
-    extra = REF_FRAMES if (args.voice_clone or args.voices) else 0   # the reference's frames in the prompt and the codec row
+    extra = REF_FRAMES if (args.voice_clone or args.voices or args.live_clone) else 0   # the reference's frames in the prompt and the codec row
     if args.voices:
         extra += VOICE_OVERLAY + VOICE_INSTRUCT
     eng = AREngine(cfg, synthetic.random_tts_weights(cfg, device="cpu", seed=0), device=dev, max_batch=max_b,
@@ -375,10 +484,22 @@ def main():
                    "more per step", "sampling": "mixed: 1/4 top-p 0.8, 1/4 greedy, 1/2 session (top-k 50, T 0.9)" if args.mix
            else "uniform: top-k 50, T 0.9", "card": card(), "results": {}}
     if args.live_text:
-        out["live_text"] = (f"every request live: {args.live_text:g} text tokens/s from submit, horizon // 3 tokens "
-                            "after the first, then tts_eos and close")
+        out["live_text"] = (f"every request live: {args.live_text:g} text tokens/s from submit, "
+                            f"{'15 + ' if args.live_clone else ''}horizon // 3 tokens after the first, then tts_eos and close")
         out["park"] = "park_waiting=True" if args.park else "no parking"
 
+    if args.live_clone:
+        out["live_clone"] = (f"every request a live ICL clone ({REF_FRAMES}-frame reference, {VOICE_REF_TEXT}-token reference "
+                             f"text: {REF_FRAMES + 1 - VOICE_REF_TEXT} rows wait for target text), alternately unregistered "
+                             "and of one registered voice; first text row at submit")
+        for S in args.slots:
+            out["results"][f"n_slots={S}"] = live_clone_probe(eng, codec, pad, sp, S, S * args.requests_per_slot, args.packet,
+                                                              args.live_text, g)
+        out["card_after"] = card()
+        print(json.dumps(out))
+        codec.close()
+        eng.close()
+        return
     if args.voice_clone:
         out["voice_clone"] = (f"every second request: {REF_FRAMES}-frame reference of random valid codes, prompt "
                               f"{args.prompt_len + REF_FRAMES} positions instead of {args.prompt_len}")
