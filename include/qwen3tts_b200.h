@@ -365,6 +365,52 @@ int q3_codec_enc_stream_reset_rows(q3_codec_enc_stream* s, int32_t n, const int3
 int q3_codec_enc_stream_row_position(q3_codec_enc_stream* s, int32_t row);
 void q3_codec_enc_stream_close(q3_codec_enc_stream* s);
 
+/* ---------------------------------------------------------------- audio rate and encoding (streaming resampler)
+ * Stands beside the reference's librosa.resample / scipy.signal.resample_poly calls (qwen3_tts_tokenizer.py:156,204):
+ * the polyphase FIR rate conversion of resample_poly, streamed over many rows, with an encoding epilogue.  For a rate
+ * pair up/down (reduced) and taps h[0..ntaps), ntaps = 2*hl + 1 (resample_poly's firwin(2*hl+1, 1/max(up,down),
+ * ("kaiser", 5.0)) * up, designed by the caller; [1.0] for equal rates), output j of a clip x[0..n) is
+ *   y[j] = sum_m x[m] * h[hl + j*down - m*up]  over 0 <= m < n, 0 <= hl + j*down - m*up <= 2*hl,
+ * an fp32 sum in ascending m, and the clip has ceil(n*up/down) outputs.  Output j is emitted once input
+ * floor((hl + j*down)/up) has arrived, so after n inputs without an end a row has emitted
+ * E(n) = max(0, floor((n*up - 1 - hl)/down) + 1); the end emits the rest, with x = 0 past the clip.  A clip streamed in
+ * pushes of any sizes equals the clip pushed at once, bit for bit.  Encodings of y: F32 as is; S16 =
+ * clamp(rint(y*32768), -32768, 32767) (round half to even); ULAW = G.711 mu-law of that S16 value as
+ * audioop.lin2ulaw(..., 2) computes it.
+ * open: `rows` rows; a step gives each row at most max_in inputs; each row's output capacity is max_out samples
+ *   (4*max_out bytes).  Device memory of the object is its own.
+ * add_filter: copies the device taps (fp32 [ntaps]) into the object and returns their id in *id_out.  A filter may
+ *   not read more than Q3_RESAMPLE_HIST inputs back (floor(2*hl/up)), nor emit more than max_out samples from a push of
+ *   max_in inputs plus its end (ceil(max_in*up/down) + ceil(hl/down) + 1).  At most 16 filters.
+ * reset_rows: the n rows in rows_host start new clips with filter filters_host[i] and encoding encodings_host[i]
+ *   (Q3_RESAMPLE_F32 / S16 / ULAW).  Host state only, no device work.
+ * step_rows: one launch over every row.  Row r takes counts_host[r] (0..max_in) fp32 inputs at in_dev + r*ld and, when
+ *   end_host[r] != 0, ends its clip (it then starts a new one with the same filter and encoding).  Its new outputs go
+ *   to out_dev + r*4*max_out bytes in its encoding (4, 2 or 1 bytes each), and their count to nout_host[r], known
+ *   without a sync.  A row with count 0 and no end is untouched.  A row never reset may take neither inputs nor an end.
+ *   Asynchronous on `stream`; the rows' histories move on the device.
+ * save_rows: the n listed rows' state (filter id, encoding, inputs so far, history) to dst_dev, Q3_RESAMPLE_ROW_BYTES
+ *   bytes per row in list order.  Asynchronous.
+ * load_rows: the n listed rows continue the states saved at src_dev (by this object): reads the records' headers back
+ *   to the host (synchronises `stream`), then copies the histories asynchronously.
+ * Bad arguments (a row out of range or listed twice, a count outside [0, max_in] or above ld, an unknown filter or
+ *   encoding, a row never reset, null pointers) are rejected before any device work and change nothing. */
+#define Q3_RESAMPLE_HIST 128
+#define Q3_RESAMPLE_ROW_BYTES 528
+#define Q3_RESAMPLE_F32 0
+#define Q3_RESAMPLE_S16 1
+#define Q3_RESAMPLE_ULAW 2
+typedef struct q3_resampler q3_resampler;
+int q3_resample_open(int32_t rows, int32_t max_in, int32_t max_out, int32_t device, q3_resampler** out);
+void q3_resample_close(q3_resampler* s);
+int q3_resample_add_filter(q3_resampler* s, int32_t up, int32_t down, const float* taps_dev, int32_t ntaps, int32_t* id_out);
+int q3_resample_reset_rows(q3_resampler* s, int32_t n, const int32_t* rows_host, const int32_t* filters_host,
+                           const int32_t* encodings_host);
+int q3_resample_step_rows(q3_resampler* s, const float* in_dev, int64_t ld, const int32_t* counts_host,
+                          const int32_t* end_host, void* out_dev, int32_t* nout_host, void* stream);
+int q3_resample_save_rows(q3_resampler* s, int32_t n, const int32_t* rows_host, void* dst_dev, void* stream);
+int q3_resample_load_rows(q3_resampler* s, int32_t n, const int32_t* rows_host, const void* src_dev, void* stream);
+
 /* ---------------------------------------------------------------- speaker x-vector (voice cloning)
  * Replaces Qwen3TTSForConditionalGeneration.extract_speaker_embedding (core/models/modeling_qwen3_tts.py:1941-1954):
  * mel_spectrogram (:396-448) + Qwen3TTSSpeakerEncoder.forward (:371-393).  fp32. */

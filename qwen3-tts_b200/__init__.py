@@ -2,9 +2,9 @@
 
 Importable as `qwen3_tts_b200` (see the shim module at the repo root; the directory name carries a hyphen).
 """
-from .config import CodecConfig, SamplingParams, StackConfig, TTSConfig  # noqa: F401
+from .config import AudioFormat, CodecConfig, SamplingParams, StackConfig, TTSConfig  # noqa: F401
 
-__all__ = ["TTSConfig", "StackConfig", "SamplingParams", "CodecConfig",
+__all__ = ["TTSConfig", "StackConfig", "SamplingParams", "CodecConfig", "AudioFormat",
            "Qwen3TTSModel", "Qwen3TTSTokenizer", "VoiceClonePromptItem", "Voice"]
 
 _PUBLIC = {"Qwen3TTSModel", "Qwen3TTSTokenizer", "VoiceClonePromptItem", "Voice"}

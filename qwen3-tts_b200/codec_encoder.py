@@ -145,10 +145,15 @@ class CodecEncoder:
     def last_launches(self) -> int:
         return self.lib.q3_codec_enc_last_launch_count(self.h)
 
-    def open_stream(self, batch: int, max_packet_frames: int = 8) -> "EncoderStream":
+    def open_stream(self, batch: int, max_packet_frames: int = 8, sample_rate=None):
         """A streaming encoder of `batch` rows (see EncoderStream): codes come back as each 1920-sample frame completes,
-        and a clip ended with end() has exactly the codes of forward() on that clip alone."""
-        return EncoderStream(self, batch, max_packet_frames)
+        and a clip ended with end() has exactly the codes of forward() on that clip alone.  `sample_rate` (None: the
+        encoder's 24 kHz) other than 24 kHz: pushes are resampled on the device first (audio.ResampledEncoderStream),
+        and a clip's codes equal forward(Resampler.oneshot(clip))."""
+        from . import audio
+        if sample_rate is None or sample_rate == audio.CODEC_RATE:
+            return EncoderStream(self, batch, max_packet_frames)
+        return audio.ResampledEncoderStream(self, batch, max_packet_frames, sample_rate)
 
     def forward_with_stages(self, wav: torch.Tensor):
         """Test helper: one forward that also returns every stage activation (name -> (B, C, T) fp32)."""

@@ -1,6 +1,7 @@
 """Shape/config records for the hot path; every value is read from the loaded HF config objects
 (never hard-coded: SURVEY §0 F6).  Mirrors core/models/configuration_qwen3_tts.py:187-212,370-404 and
 core/tokenizer_12hz/configuration_qwen3_tts_tokenizer_v2.py:72-93 of the reference."""
+import operator
 from dataclasses import dataclass, field
 from typing import Tuple
 
@@ -187,3 +188,26 @@ class SpeakerEncoderConfig:
         base = SpeakerEncoderConfig()
         kw = {k: (tuple(v) if isinstance(v, (list, tuple)) else v) for k, v in d.items() if hasattr(base, k)}
         return SpeakerEncoderConfig(**kw)
+
+
+SUPPORTED_RATES = (8000, 11025, 16000, 22050, 24000, 32000, 44100, 48000)
+ENCODINGS = ("f32", "s16", "ulaw")
+
+
+@dataclass(frozen=True)
+class AudioFormat:
+    """The sample rate and encoding of a client's audio: "f32" float32 samples, "s16" 16-bit PCM (int16), "ulaw" 8-bit
+    G.711 mu-law (uint8).  Rates: SUPPORTED_RATES.  Anything else raises ValueError on construction."""
+    sample_rate: int
+    encoding: str = "f32"
+
+    def __post_init__(self):
+        try:
+            sr = operator.index(self.sample_rate)   # int or numpy integer; not a float
+        except TypeError:
+            sr = None
+        if sr is None or isinstance(self.sample_rate, bool) or sr not in SUPPORTED_RATES:
+            raise ValueError(f"sample_rate {self.sample_rate!r} is not supported; supported rates: {SUPPORTED_RATES}")
+        if not isinstance(self.encoding, str) or self.encoding not in ENCODINGS:
+            raise ValueError(f"encoding {self.encoding!r} is not supported; supported encodings: {ENCODINGS}")
+        object.__setattr__(self, "sample_rate", sr)

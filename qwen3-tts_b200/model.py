@@ -628,14 +628,18 @@ class Qwen3TTSTokenizer:
         from types import SimpleNamespace
         return SimpleNamespace(audio_codes=codes)
 
-    def open_encode_stream(self, batch: int = 1, max_packet_frames: int = 8):
+    def open_encode_stream(self, batch: int = 1, max_packet_frames: int = 8, sample_rate=None):
         """A streaming encoder of `batch` rows (codec_encoder.EncoderStream): push({row: samples}) returns the (n_i, 16)
         codes of the frames each push completes, end(rows) the clip's last frame, in the layout of encode().audio_codes;
-        a clip's pushes plus its end equal encode() of the whole clip.  Audio must already be at
-        get_input_sample_rate(): resampling chunk by chunk would not match encode()'s whole-clip resampling."""
+        a clip's pushes plus its end equal encode() of the whole clip.  `sample_rate`: the rate of the pushed audio
+        (None: get_input_sample_rate()).  At another supported rate (audio.SUPPORTED_RATES) the pushes are resampled on
+        the GPU as they arrive (audio.ResampledEncoderStream), and a clip's codes equal
+        encoder.forward(Resampler.oneshot(clip)) bit for bit.  encode(..., sr=) keeps resampling on the host with
+        scipy.signal.resample_poly: the same filter and sum in another rounding order, so its waveform agrees with the
+        GPU's to within 1e-5, and the codes of the two may differ only where the RVQ has a near-tie."""
         if self.encoder is None:
             raise RuntimeError("this tokenizer was built without encoder weights (decode-only)")
-        return self.encoder.open_stream(batch, max_packet_frames)
+        return self.encoder.open_stream(batch, max_packet_frames, sample_rate=sample_rate)
 
     def decode(self, encoded) -> Tuple[List[np.ndarray], int]:
         """:259-365 — accepts an encode()-style output (has .audio_codes), a dict or a list of dicts whose

@@ -59,6 +59,16 @@ text row, the bf16 add of build_prefill), later rows are trailing text; a close_
 completes it with tts_pad and makes the trailing text [tts_pad], build_prefill's layout for a short text.  Until then
 the request is not admitted, takes no slot a park would free, and does not keep run() going; once complete it is
 admitted and runs as any live request, so it generates what its whole text gives up front (tests/test_gpu_live_clone.py).
+
+Audio formats (`ContinuousBatcher(audio_format=)` for the session, `submit(audio_format=)` per request, an AudioFormat):
+a request with a rate or encoding other than the codec's 24 kHz float32 has a row of one audio.Resampler of `n_slots`
+rows, opened when the first such request is admitted.  After each codec push its slot's new samples go through one
+resampler launch with every other such slot, including the tails of requests that finished in the step (even with no
+new frame), and stream() yields its chunk as float32, int16 or uint8.  Its row is reset at admission (by reset, seed or
+bank copy alike: the resampled audio is the generated part's), saved on the request when it is parked and loaded into
+its new slot when resumed.  A request's concatenated chunks equal Resampler.oneshot of its whole audio
+(tests/test_gpu_scheduler_audio_format.py).  Requests in the codec's own format take today's path, so a session
+without formats makes the same calls as before.
 """
 from collections import deque
 from dataclasses import dataclass, field
@@ -67,8 +77,9 @@ from typing import Any, Deque, Dict, Iterator, List, Optional, Tuple, Union
 import numpy as np
 import torch
 
+from . import audio
 from .codec import CodecDecoder, CodecStream, check_ref_codes
-from .config import SamplingParams
+from .config import AudioFormat, SamplingParams
 from .engine import AREngine
 
 
@@ -92,14 +103,19 @@ class _Request:
     bank: Optional[Tuple[int, int]] = None
     codes: Optional[torch.Tensor] = None
     overlay: Optional[torch.Tensor] = None   # prompt rows still waiting for a text row each (None once complete)
+    fmt: Optional[AudioFormat] = None        # the client's audio format; None: the codec's own (no resampler row)
+    res_state: Optional[torch.Tensor] = None   # while parked: its resampler row's saved state
 
 
 class ContinuousBatcher:
     def __init__(self, engine: AREngine, tts_pad_embed: torch.Tensor, sp: SamplingParams, n_slots: int = 8, packet_frames: int = 4,
-                 max_trailing: int = 256, codec: Union[CodecDecoder, CodecStream, None] = None, park_waiting: bool = False):
+                 max_trailing: int = 256, codec: Union[CodecDecoder, CodecStream, None] = None, park_waiting: bool = False,
+                 audio_format: Optional[AudioFormat] = None):
         """`codec`: a CodecDecoder, whose stream of `n_slots` rows the batcher opens, or an open CodecStream of
         `n_slots` rows taking packets of at least `packet_frames` frames.  `park_waiting`: park running live-text
-        requests that wait for text when another request needs their slot (see the module docstring)."""
+        requests that wait for text when another request needs their slot (see the module docstring).
+        `audio_format`: the sample rate and encoding of stream()'s audio for requests submitted without one (None:
+        the codec's 24 kHz float32)."""
         self.eng, self.sp, self.pad = engine, sp, tts_pad_embed
         self.park_waiting = bool(park_waiting)
         self.parked: Dict[int, _Request] = {}      # request id -> parked request, oldest park first
@@ -126,12 +142,23 @@ class ContinuousBatcher:
             self.cstream = codec.open_stream(self.n_slots, max_packet_frames=self.packet) if codec is not None else None
         else:
             raise ValueError(f"codec must be a CodecDecoder or a CodecStream, got {type(codec).__name__}")
+        self.audio_format = self._check_format(audio_format)
+        self.resampler: Optional[audio.Resampler] = None   # opened when the first request with a format is admitted
+
+    def _check_format(self, fmt: Optional[AudioFormat]) -> Optional[AudioFormat]:
+        """The format a request streams in: None for the codec's own 24 kHz float32 (no resampling)."""
+        if fmt is None:
+            return None
+        audio.check_format(fmt)
+        if self.codec is None:
+            raise ValueError("an audio format needs a ContinuousBatcher built with a codec")
+        return None if fmt == AudioFormat(audio.CODEC_RATE) else fmt
 
     # ------------------------------------------------------------------ API
     def submit(self, inputs_embeds: torch.Tensor, trailing_text: Optional[torch.Tensor] = None, key: Optional[int] = None,
                max_frames: Optional[int] = None, sampling: Optional[SamplingParams] = None,
                ref_codes: Optional[torch.Tensor] = None, text_open: bool = False, voice=None,
-               overlay: Optional[torch.Tensor] = None) -> int:
+               overlay: Optional[torch.Tensor] = None, audio_format: Optional[AudioFormat] = None) -> int:
         """Queue one request; returns its id (also its Philox row key unless `key` is given).  `sampling`: the
         request's own generation parameters (default: the session's); its max_new_tokens bounds the request's horizon
         and may not exceed the session's.  `ref_codes`: (L, num_quantizers) reference codes of a voice-clone request
@@ -144,8 +171,10 @@ class ContinuousBatcher:
         reference state instead of decoding the reference.  It takes no `ref_codes`.  `overlay`: (K, H) prompt rows of
         a live ICL voice clone that still wait for one text row each (Qwen3TTSModel.build_live_clone_request); it needs
         `text_open`, and an ICL voice if it has a voice.  The trailing rows given here and later fill it first, and the
-        request is admitted once it is full or its text is closed (see the module docstring).  Bad parameters raise
+        request is admitted once it is full or its text is closed (see the module docstring).  `audio_format`: the
+        sample rate and encoding of the request's stream() chunks (default: the session's).  Bad parameters raise
         ValueError here, never in a later step()."""
+        fmt = self._check_format(audio_format) if audio_format is not None else self.audio_format
         H = self.eng.cfg.talker.hidden_size
         L_ref, P = 0, 0
         if overlay is not None:
@@ -197,7 +226,7 @@ class ContinuousBatcher:
         if self.codec is not None:
             horizon = min(horizon, self.codec.max_frames - L_ref)  # a codec row's position may not pass its RoPE table
         r = _Request(rid, inputs_embeds, tr, horizon, sampling, ref_codes, voice, text_open=bool(text_open),
-                     overlay=overlay if K else None)
+                     overlay=overlay if K else None, fmt=fmt)
         if r.overlay is not None:
             r.trailing = self._fill(r, tr.reshape(-1, H))
         r.n_text = int(r.trailing.reshape(-1, H).shape[0])
@@ -285,10 +314,11 @@ class ContinuousBatcher:
                 self._cancelled.add(rid)
                 return True
         r = self.parked.pop(rid, None)
-        if r is not None:    # its record and its codec bank row are freed
+        if r is not None:    # its record, its codec bank row and its resampler state are freed
             self.eng.discard(r.record)
             if r.bank is not None:
                 self.codec.bank_release(*r.bank)
+            r.res_state = None
             self._cancelled.add(rid)
             return True
         return False
@@ -325,6 +355,8 @@ class ContinuousBatcher:
         r.record = self.eng.park(slot)
         if self.cstream is not None:
             r.bank = self.codec.bank_copy(self.cstream, slot)
+        if r.fmt is not None:
+            r.res_state = self.resampler.save([slot])
         r.trailing = r.trailing.reshape(-1, self.eng.cfg.talker.hidden_size)[:0]   # the record holds the text so far
         r.slot = -1
         self.parked[r.rid] = r
@@ -344,6 +376,9 @@ class ContinuousBatcher:
             self.cstream.copy_from(self.codec.bank_stream(r.bank[0]), [r.bank[1]], [slot])
             self.codec.bank_release(*r.bank)   # a later bank_copy into that row is queued behind this copy
             r.bank = None
+        if r.res_state is not None:
+            self.resampler.load([slot], r.res_state)
+            r.res_state = None
         if r.trailing.shape[0] > 0:
             self.eng.append_trailing(slot, r.trailing)
             r.trailing = r.trailing[:0]
@@ -358,9 +393,11 @@ class ContinuousBatcher:
         return finished
 
     def stream(self) -> Iterator[Tuple[Dict[int, np.ndarray], List[int]]]:
-        """Run the session with audio out: yields per step ({request id: float32 waveform of its new frames},
+        """Run the session with audio out: yields per step ({request id: waveform of its new frames},
         [ids that finished in the step]) while requests are pending, running or parked, so a request submitted between
-        two iterations is admitted at the next one."""
+        two iterations is admitted at the next one.  A waveform is float32 at the codec's 24 kHz, or in the request's
+        audio format (float32, int16 or uint8 at its rate); a request with a format also gets an entry in the step it
+        finishes, holding its resampler's tail."""
         if self.cstream is None:
             raise ValueError("stream() needs a ContinuousBatcher built with a codec")
         while self.pending or self.running or self.parked:
@@ -428,6 +465,10 @@ class ContinuousBatcher:
                 for bank in sorted({r.voice.bank[0] for r in banked}):   # one copy per bank, no reference decode
                     rs = [r for r in banked if r.voice.bank[0] == bank]
                     self.cstream.copy_from(self.codec.bank_stream(bank), [r.voice.bank[1] for r in rs], [r.slot for r in rs])
+                for fmt in dict.fromkeys(r.fmt for r in batch if r.fmt is not None):   # one reset per format
+                    if self.resampler is None:
+                        self.resampler = audio.Resampler(self.eng.device, self.n_slots, self.packet * self.codec.total_upsample)
+                    self.resampler.reset([r.slot for r in batch if r.fmt == fmt], audio.CODEC_RATE, fmt)
         if not batch and not self._runnable():
             return {}, []   # every running row is open and waiting for text: launch nothing
         n = min([self.packet] + [r.max_frames - r.emitted for r in self.running.values()])
@@ -452,12 +493,17 @@ class ContinuousBatcher:
         return new, finished
 
     def _push_audio(self, new) -> Dict[int, np.ndarray]:
-        """One codec step over all slots: slot s takes its new frames codes[s, e0:e0+k] as its count k, idle slots 0."""
+        """One codec step over all slots: slot s takes its new frames codes[s, e0:e0+k] as its count k, idle slots 0.
+        Slots of requests with a format then take their new audio through one resampler launch, and those whose
+        request finished in this step end their clips there (their tails come even without new frames)."""
         if self.cstream is None:
             return {}
         m = max([k for _, _, k in new.values()], default=0)
-        if m == 0:
+        ending = [slot for slot, (r, _, _) in new.items() if r.fmt is not None and self.running.get(slot) is not r]
+        if m == 0 and not ending:
             return {}
+        if any(r.fmt is not None for r, _, _ in new.values()):
+            return self._push_formats(new, m, ending)
         start, counts = [0] * self.n_slots, [0] * self.n_slots
         for slot, (_, e0, k) in new.items():
             start[slot], counts[slot] = e0, k
@@ -467,6 +513,32 @@ class ContinuousBatcher:
         wav = self.cstream.push(codes, counts)[:, 0].cpu().numpy()
         up = self.codec.total_upsample
         return {r.rid: wav[slot, :k * up] for slot, (r, _, k) in new.items() if k > 0}
+
+    def _push_formats(self, new, m: int, ending: List[int]) -> Dict[int, np.ndarray]:
+        """_push_audio of a step in which some request has a format: the codec push stays on the device, the default
+        slots' audio comes back as before, the others' through the resampler."""
+        up = self.codec.total_upsample
+        out: Dict[int, np.ndarray] = {}
+        wav = None
+        if m > 0:
+            start, counts = [0] * self.n_slots, [0] * self.n_slots
+            for slot, (_, e0, k) in new.items():
+                start[slot], counts[slot] = e0, k
+            idx = (torch.tensor(start)[:, None] + torch.arange(m)[None]).clamp_(max=self.max_frames - 1)
+            rows = torch.arange(self.n_slots)[:, None]
+            codes = self.codes[rows.to(self.codes.device), idx.to(self.codes.device)].transpose(1, 2)  # [S][G][m]
+            wav = self.cstream.push(codes, counts)[:, 0]
+            plain = [slot for slot, (r, _, k) in new.items() if r.fmt is None and k > 0]
+            if plain:
+                host = wav[plain].cpu().numpy()
+                for i, slot in enumerate(plain):
+                    out[new[slot][0].rid] = host[i, :new[slot][2] * up]
+        res = {slot: k * up for slot, (r, _, k) in new.items() if r.fmt is not None and k > 0}
+        got = self.resampler.push_rows(wav, res, ending)
+        for slot, y in got.items():
+            if y.shape[0] or slot in ending:   # the filter's delay can hold a short push back entirely
+                out[new[slot][0].rid] = y
+        return out
 
     def run(self) -> Dict[int, torch.Tensor]:
         """Drain the queue; returns {request id: (N_i, G) codes}.  Requests with open text must be closed first (or

@@ -1,0 +1,116 @@
+"""Cost of audio formats in the continuous batcher, on the GPU: the resampler kernel's time (CUDA events around its
+launches) and the batcher's _push_audio time per step (host clock ending in a synchronise), at 8 and 32 slots with the
+default codec and 4-frame packets, for all rows in the default format, all rows 8 kHz mu-law and all rows 48 kHz
+float32.  Prints one JSON line, with the card's name and power limit read in the same run.
+
+    python tools/format_probe.py [--steps 60] [--warmup 10]
+"""
+import argparse
+import ctypes as C
+import json
+import os
+import subprocess
+import sys
+import time
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+
+class _Cfg:          # the few engine fields ContinuousBatcher.__init__ reads
+    class talker:
+        hidden_size = 8
+    num_code_groups = 16
+
+
+class _Engine:
+    cfg, max_ctx = _Cfg, 1 << 20
+
+    def __init__(self, device):
+        import torch
+        self.device = torch.device(device)
+
+    def session_begin(self, *a, **k):
+        pass
+
+
+def _card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                           text=True, timeout=30).stdout.strip().splitlines()[0]
+        name, power = [s.strip() for s in q.split(",")]
+        return name, power
+    except Exception as e:   # the numbers stay, the card is reported as unknown
+        return f"unknown ({e!r})", "unknown"
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=60)
+    ap.add_argument("--warmup", type=int, default=10)
+    a = ap.parse_args()
+    import torch
+    import qwen3_tts_b200 as q
+    from qwen3_tts_b200 import _lib, audio, synthetic
+    from qwen3_tts_b200.codec import CodecDecoder
+    from qwen3_tts_b200.scheduler import ContinuousBatcher, _Request
+    if not torch.cuda.is_available():
+        raise SystemExit("format_probe needs a GPU")
+    dev = "cuda:0"
+    ccfg = q.CodecConfig()
+    dec = CodecDecoder(ccfg, synthetic.random_codec_weights(ccfg, device="cpu", seed=0), device=dev, max_frames=1024)
+    P, up = 4, dec.total_upsample
+    formats = {"default": None, "8k_ulaw": q.AudioFormat(8000, "ulaw"), "48k_f32": q.AudioFormat(48000, "f32")}
+    results = []
+    g = torch.Generator().manual_seed(0)
+    for S in (8, 32):
+        for name, fmt in formats.items():
+            cb = ContinuousBatcher(_Engine(dev), torch.zeros(8), q.SamplingParams(max_new_tokens=2048), n_slots=S,
+                                   packet_frames=P, codec=dec)
+            cb.codes.copy_(torch.randint(0, ccfg.codebook_size, cb.codes.shape, generator=g).to(cb.codes))
+            reqs = [_Request(s, None, None, 2000, fmt=cb._check_format(fmt)) for s in range(S)]
+            for s, r in enumerate(reqs):
+                r.slot = s
+                cb.running[s] = r
+            cb.cstream.reset()
+            if fmt is not None:
+                cb.resampler = audio.Resampler(dev, S, P * up)
+                cb.resampler.reset(range(S), audio.CODEC_RATE, fmt)
+            times = []
+            for it in range(a.warmup + a.steps):
+                new = {s: (r, it * P, P) for s, r in enumerate(reqs)}
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                cb._push_audio(new)
+                torch.cuda.synchronize()
+                if it >= a.warmup:
+                    times.append(time.perf_counter() - t0)
+            row = {"slots": S, "format": name, "push_audio_ms_mean": 1e3 * sum(times) / len(times),
+                   "push_audio_ms_min": 1e3 * min(times)}
+            if fmt is not None:    # one resampler step (its job upload and kernel) of one packet per row
+                res = cb.resampler
+                x = torch.rand(S, P * up, device=dev) * 2 - 1
+                cnt, end = (C.c_int32 * S)(*[P * up] * S), (C.c_int32 * S)()
+                nout = (C.c_int32 * S)()
+                st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+                step = lambda: _lib.check(res.lib.q3_resample_step_rows(res.h, x.data_ptr(), x.stride(0), cnt, end,  # noqa: E731
+                                                                        res._out.data_ptr(), nout, st))
+                for _ in range(a.warmup):
+                    step()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                n = 200
+                e0.record()
+                for _ in range(n):
+                    step()
+                e1.record()
+                torch.cuda.synchronize()
+                row["resample_step_us"] = 1e3 * e0.elapsed_time(e1) / n
+                row["outputs_per_row"] = int(nout[0])
+                res.close()
+            cb.cstream.close()
+            results.append(row)
+    name, power = _card()
+    print(json.dumps({"gpu": name, "power_limit": power, "packet_frames": P, "results": results}))
+
+
+if __name__ == "__main__":
+    main()
