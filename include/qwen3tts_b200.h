@@ -411,6 +411,39 @@ int q3_resample_step_rows(q3_resampler* s, const float* in_dev, int64_t ld, cons
 int q3_resample_save_rows(q3_resampler* s, int32_t n, const int32_t* rows_host, void* dst_dev, void* stream);
 int q3_resample_load_rows(q3_resampler* s, int32_t n, const int32_t* rows_host, const void* src_dev, void* stream);
 
+/* ---------------------------------------------------------------- speaking rate (streaming WSOLA time-stretch)
+ * Waveform-similarity overlap-add at the codec's 24 kHz with fixed geometry: frame N = 960, synthesis hop Hs = 480,
+ * search tolerance D = 240, analysis hop Ha in [240, 960] (Ha = floor(speed*480 + 0.5)), window w[n] = sin^2(pi*n/960)
+ * (fp32, designed by the caller).  Frame k has nominal position a_k = k*Ha and chosen position p_k = a_k + d_k, d_0 = 0;
+ * for k >= 1, d_k in [-D, D] maximises C_k(d) = sum_{n<480} x[p_{k-1} + 480 + n] * x[a_k + d + n] (fp32, acc = 0 then
+ * one fused multiply-add per n in ascending n), ties to the smallest |d|, then to the negative d.  Output:
+ *   y[m] = x[m]  (m < 480);  y[k*480 + i] = fl(fl(w[i]*x[p_k + i]) + fl(w[i+480]*x[p_{k-1} + i + 480]))  (k >= 1, i < 480),
+ * and a clip x[0..n) gives M(n) = ceil(n*480/Ha) samples, with x = 0 past n.  Frame k is done once input
+ * a_k + D + N - 1 has arrived, so after n inputs without an end a row has emitted E(n) = 480*(floor((n - 1200)/Ha) + 1)
+ * (0 for n < 1200); an end emits [E(n), M(n)).  A clip streamed in pushes of any sizes equals the clip pushed at once.
+ * open: `rows` rows; a step gives each row at most max_in (1 .. 32768) inputs; each row's output capacity is max_out fp32
+ *   samples, at least ceil((max_in + 1199)*480/240).  Device memory of the object is its own.
+ * set_window: copies the device window (fp32 [960]) into the object.  Required before the first step.
+ * reset_rows: the n rows in rows_host start new clips with analysis hop hops_host[i].  Host state only.
+ * step_rows: one launch, one CTA per row with inputs or an end.  Row r takes counts_host[r] (0..max_in) fp32 inputs at
+ *   in_dev + r*ld and, when end_host[r] != 0, ends its clip (it then starts a new one with the same hop).  Its new
+ *   outputs go to out_dev + r*max_out (fp32), their count to nout_host[r], known without a sync.  A row with count 0 and
+ *   no end is untouched.  A row never reset may take neither inputs nor an end.  Asynchronous on `stream`.
+ * save_rows / load_rows: as q3_resample_save_rows / load_rows, Q3_STRETCH_ROW_BYTES per row (hop, inputs so far, frames
+ *   done, p of the last frame done, its windowed second half, the last Q3_STRETCH_HIST inputs).  load synchronises.
+ * Bad arguments are rejected before any device work and change nothing. */
+#define Q3_STRETCH_HIST 2048
+#define Q3_STRETCH_ROW_BYTES 10144
+typedef struct q3_stretcher q3_stretcher;
+int q3_stretch_open(int32_t rows, int32_t max_in, int32_t max_out, int32_t device, q3_stretcher** out);
+void q3_stretch_close(q3_stretcher* s);
+int q3_stretch_set_window(q3_stretcher* s, const float* window_dev);
+int q3_stretch_reset_rows(q3_stretcher* s, int32_t n, const int32_t* rows_host, const int32_t* hops_host);
+int q3_stretch_step_rows(q3_stretcher* s, const float* in_dev, int64_t ld, const int32_t* counts_host,
+                         const int32_t* end_host, float* out_dev, int32_t* nout_host, void* stream);
+int q3_stretch_save_rows(q3_stretcher* s, int32_t n, const int32_t* rows_host, void* dst_dev, void* stream);
+int q3_stretch_load_rows(q3_stretcher* s, int32_t n, const int32_t* rows_host, const void* src_dev, void* stream);
+
 /* ---------------------------------------------------------------- speaker x-vector (voice cloning)
  * Replaces Qwen3TTSForConditionalGeneration.extract_speaker_embedding (core/models/modeling_qwen3_tts.py:1941-1954):
  * mel_spectrogram (:396-448) + Qwen3TTSSpeakerEncoder.forward (:371-393).  fp32. */

@@ -78,7 +78,9 @@ CODEC_SYMBOLS = ["q3_codec_create", "q3_codec_destroy", "q3_codec_load_tensor", 
                  "q3_spk_create", "q3_spk_destroy", "q3_spk_load_tensor", "q3_spk_finalize", "q3_spk_frames", "q3_spk_mel",
                  "q3_spk_embed", "q3_spk_last_launch_count",
                  "q3_resample_open", "q3_resample_close", "q3_resample_add_filter", "q3_resample_reset_rows",
-                 "q3_resample_step_rows", "q3_resample_save_rows", "q3_resample_load_rows"]
+                 "q3_resample_step_rows", "q3_resample_save_rows", "q3_resample_load_rows",
+                 "q3_stretch_open", "q3_stretch_close", "q3_stretch_set_window", "q3_stretch_reset_rows",
+                 "q3_stretch_step_rows", "q3_stretch_save_rows", "q3_stretch_load_rows"]
 
 _lib = None
 
@@ -188,6 +190,14 @@ def load():
         lib.q3_resample_step_rows.argtypes = [vp, vp, i64, C.POINTER(i32), C.POINTER(i32), vp, C.POINTER(i32), vp]
         lib.q3_resample_save_rows.argtypes = [vp, i32, C.POINTER(i32), vp, vp]
         lib.q3_resample_load_rows.argtypes = [vp, i32, C.POINTER(i32), vp, vp]
+        lib.q3_stretch_open.argtypes = [i32, i32, i32, i32, C.POINTER(vp)]
+        lib.q3_stretch_close.argtypes = [vp]
+        lib.q3_stretch_close.restype = None
+        lib.q3_stretch_set_window.argtypes = [vp, vp]
+        lib.q3_stretch_reset_rows.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(i32)]
+        lib.q3_stretch_step_rows.argtypes = [vp, vp, i64, C.POINTER(i32), C.POINTER(i32), vp, C.POINTER(i32), vp]
+        lib.q3_stretch_save_rows.argtypes = [vp, i32, C.POINTER(i32), vp, vp]
+        lib.q3_stretch_load_rows.argtypes = [vp, i32, C.POINTER(i32), vp, vp]
     _lib = lib
     return lib
 

@@ -12,6 +12,9 @@ Streaming: each row keeps its filter, encoding, input count and last inputs on t
 emitted as soon as input floor((hl + j*down) / up) has arrived, so after n inputs a row has emitted emitted(n) samples;
 an end emits the rest, as if the clip were followed by zeros.  A clip pushed in pieces of any sizes and ended equals
 oneshot() of the whole clip bit for bit, and one launch serves every row of a push.
+
+Speaking rate: TimeStretch, a streaming per-row WSOLA time-stretch at 24 kHz (q3_stretch_*, csrc/stretch.cu, DESIGN
+§4.7), with the same streaming contract; the batcher runs it before the resampler.
 """
 import ctypes as C
 from math import gcd
@@ -250,6 +253,199 @@ class Resampler:
         one = Resampler(self.device, 1, max(t.numel(), 1))
         try:
             one.reset([0], in_rate, fmt)
+            return one.push({0: t}, end=[0])[0]
+        finally:
+            one.close()
+
+
+class TimeStretch:
+    """`rows` streaming WSOLA time-stretch rows at the codec's 24 kHz on `device` (q3_stretch_*, csrc/stretch.cu, DESIGN
+    §4.7): the speaking rate of float32 audio changes, its pitch does not.  Frames of N = 960 samples, synthesis hop
+    480, search tolerance 240, analysis hop Ha = hop(speed) in [240, 960], window sin^2(pi*n/960).  A clip of n samples
+    becomes total(n, Ha) samples; after n samples without an end a row has emitted emitted(n, Ha).  A push gives each
+    row at most `max_in` samples per launch (longer pushes take several launches).  reset(rows, speed) starts new clips;
+    push({row: samples}, end=rows) returns {row: float32 numpy array of the row's new output}; push_device keeps them on
+    the device; save(rows) / load(rows, state) move rows' state; oneshot(x, speed) stretches a whole clip.  A clip pushed
+    in pieces of any sizes and ended equals oneshot() of the whole clip bit for bit."""
+
+    N, HS, DELTA = 960, 480, 240
+    HIST = 2048                       # Q3_STRETCH_HIST: inputs a row keeps
+    ROW_BYTES = 10144                 # Q3_STRETCH_ROW_BYTES: one row's saved state
+    MAX_IN = 32768                    # the largest max_in the native stretcher takes
+
+    @staticmethod
+    def hop(speed) -> int:
+        """The analysis hop of `speed`: floor(speed*480 + 0.5); the effective speed is hop/480.  ValueError outside
+        [0.5, 2.0] (AudioFormat's check)."""
+        return int(np.floor(AudioFormat(CODEC_RATE, speed=speed).speed * 480 + 0.5))
+
+    @staticmethod
+    def emitted(n: int, ha: int) -> int:
+        """Outputs a row has emitted after n inputs without an end: 480*(floor((n - 1200)/Ha) + 1), 0 for n < 1200."""
+        return 0 if n < 1200 else 480 * ((n - 1200) // ha + 1)
+
+    @staticmethod
+    def total(n: int, ha: int) -> int:
+        """Outputs of a whole clip of n inputs: ceil(n*480 / Ha)."""
+        return -(-n * 480 // ha)
+
+    @staticmethod
+    def out_bound(max_in: int, ha: int = 240) -> int:
+        """The most outputs one push of max_in inputs plus its end can emit: ceil((max_in + 1199)*480 / Ha) (the
+        slowest speed by default)."""
+        return -(-(max_in + 1199) * 480 // ha)
+
+    @staticmethod
+    def window() -> np.ndarray:
+        """w[n] = sin^2(pi*n/960), n in [0, 960), in fp64 (uploaded as fp32)."""
+        return np.sin(np.pi * np.arange(960) / 960) ** 2
+
+    def __init__(self, device, rows: int, max_in: int):
+        self.lib = _lib.load()
+        self.device = torch.device(device)
+        if self.device.type != "cuda":
+            raise RuntimeError("TimeStretch needs a CUDA device (no CPU fallback)")
+        self.rows, self.max_in = int(rows), int(max_in)
+        if not 1 <= self.max_in <= self.MAX_IN:
+            raise ValueError(f"max_in {max_in} outside [1, {self.MAX_IN}]")
+        self.max_out = self.out_bound(self.max_in)
+        h = C.c_void_p()
+        _lib.check(self.lib.q3_stretch_open(self.rows, self.max_in, self.max_out, self.device.index or 0, C.byref(h)))
+        self.h = h
+        w = torch.from_numpy(self.window()).to(self.device, torch.float32)
+        _lib.check(self.lib.q3_stretch_set_window(self.h, w.data_ptr()))
+        self._ha: List[Optional[int]] = [None] * self.rows
+        self._out = torch.empty(self.rows, self.max_out, dtype=torch.float32, device=self.device)
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.q3_stretch_close(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _stream(self):
+        if not self.h:
+            raise RuntimeError("time-stretch is closed")
+        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def reset(self, rows, speed):
+        """Start new clips in `rows` at `speed` (analysis hop hop(speed))."""
+        rows = check_rows(rows, self.rows)
+        ha = self.hop(speed)
+        n = len(rows)
+        if n == 0:
+            return
+        i32n = C.c_int32 * n
+        _lib.check(self.lib.q3_stretch_reset_rows(self.h, n, i32n(*rows), i32n(*[ha] * n)))
+        for r in rows:
+            self._ha[r] = ha
+
+    def _check_ready(self, rows):
+        for r in rows:
+            if self._ha[r] is None:
+                raise ValueError(f"row {r} was never reset")
+
+    def _run(self, x: Optional[torch.Tensor], cnt: List[int], end: List[int], host: bool, listed=()):
+        """Resampler._run for the stretch: launches of at most max_in samples per row, a row ends in the launch that
+        takes its last sample; returns {row: float32 output} for rows with samples or an end and the rows `listed`."""
+        if x is not None and (x.dim() != 2 or x.shape[0] != self.rows or x.dtype != torch.float32
+                              or x.device != self.device or x.stride(1) != 1 or max(cnt) > x.shape[1]):
+            raise ValueError(f"expected fp32 samples of shape ({self.rows}, L >= counts) on {self.device}")
+        if x is None and any(cnt):
+            raise ValueError("counts without samples")
+        touched = sorted(set(end) | set(listed) | {r for r in range(self.rows) if cnt[r]})
+        self._check_ready(touched)
+        st = self._stream()
+        parts: Dict[int, list] = {r: [] for r in touched}
+        for s0 in range(0, max(max(cnt), 1), self.max_in):
+            k = [min(max(c - s0, 0), self.max_in) for c in cnt]
+            e = [int(r in end and (s0 == 0 if cnt[r] == 0 else s0 < cnt[r] <= s0 + self.max_in)) for r in range(self.rows)]
+            nout = (C.c_int32 * self.rows)()
+            ptr = x.data_ptr() + 4 * s0 if x is not None and any(k) else None
+            _lib.check(self.lib.q3_stretch_step_rows(self.h, ptr, x.stride(0) if x is not None else 0,
+                                                     (C.c_int32 * self.rows)(*k), (C.c_int32 * self.rows)(*e),
+                                                     self._out.data_ptr(), nout, st))
+            nb = {r: nout[r] for r in touched}
+            if host:
+                top = max(nb.values(), default=0)
+                buf = self._out[:, :top].cpu().numpy() if top else None
+                for r in touched:
+                    parts[r].append(buf[r, :nb[r]].copy() if nb[r] else None)
+            else:
+                for r in touched:
+                    parts[r].append(self._out[r, :nb[r]].clone() if nb[r] else None)
+        out = {}
+        for r in touched:
+            v = [p for p in parts[r] if p is not None]
+            if host:
+                out[r] = np.concatenate(v) if v else np.zeros(0, np.float32)
+            else:
+                out[r] = torch.cat(v) if v else torch.zeros(0, dtype=torch.float32, device=self.device)
+        return out
+
+    def push_rows(self, x: Optional[torch.Tensor], counts: Dict[int, int], end: Iterable[int] = (), host: bool = True):
+        """Row r takes x[r, :counts[r]] of x, fp32 (rows, L) on the device with contiguous rows, and the rows in `end`
+        end their clips: one launch per max_in samples.  Returns {row: its new float32 output} (numpy arrays when
+        `host`, else device tensors) for every row with samples or an end and every row of `counts`."""
+        cnt = [0] * self.rows
+        for r, k in counts.items():
+            if int(k) < 0:
+                raise ValueError(f"row {r}: negative count {k}")
+            cnt[check_rows(r, self.rows)[0]] = int(k)
+        return self._run(x, cnt, check_rows(end, self.rows), host, listed=[int(r) for r in counts])
+
+    _pack = Resampler._pack
+
+    def push(self, chunks: Dict, end: Iterable[int] = ()) -> Dict[int, np.ndarray]:
+        """chunks {row: 1-D float samples at 24 kHz} (numpy or torch, any length); the rows in `end` end their clips
+        after their samples.  Returns {row: float32 numpy array of its new output} for every row of chunks or end."""
+        x, counts, end = self._pack(chunks, end)
+        out = self.push_rows(x, counts, end, host=True)
+        return {r: out[r] for r in sorted(set(chunks) | set(end))}
+
+    def push_device(self, chunks: Dict, end: Iterable[int] = ()) -> Dict[int, torch.Tensor]:
+        """push() with the outputs left on the device."""
+        x, counts, end = self._pack(chunks, end)
+        out = self.push_rows(x, counts, end, host=False)
+        return {r: out[r] for r in sorted(set(chunks) | set(end))}
+
+    def save(self, rows) -> torch.Tensor:
+        """The rows' state (hop, inputs so far, frames done, last frame's position and tail, history): a uint8
+        (len(rows), ROW_BYTES) device tensor."""
+        rows = check_rows(rows, self.rows)
+        self._check_ready(rows)
+        state = torch.empty(len(rows), self.ROW_BYTES, dtype=torch.uint8, device=self.device)
+        n = len(rows)
+        if n:
+            _lib.check(self.lib.q3_stretch_save_rows(self.h, n, (C.c_int32 * n)(*rows), state.data_ptr(), self._stream()))
+        return state
+
+    def load(self, rows, state: torch.Tensor):
+        """Rows `rows` continue the states save() returned, in order."""
+        rows = check_rows(rows, self.rows)
+        if not isinstance(state, torch.Tensor) or state.dtype != torch.uint8 \
+                or tuple(state.shape) != (len(rows), self.ROW_BYTES) or state.device != self.device:
+            raise ValueError(f"expected a saved state of shape ({len(rows)}, {self.ROW_BYTES}) on {self.device}")
+        n = len(rows)
+        if n == 0:
+            return
+        state = state.contiguous()
+        _lib.check(self.lib.q3_stretch_load_rows(self.h, n, (C.c_int32 * n)(*rows), state.data_ptr(), self._stream()))
+        has = state[:, 0:4].cpu().numpy().view(np.int32)[:, 0]   # the header's hop (already read back natively)
+        for r, ha in zip(rows, has):
+            self._ha[r] = int(ha)
+
+    def oneshot(self, x, speed) -> np.ndarray:
+        """The whole clip x (1-D float samples at 24 kHz) stretched at once: the reference of the streamed result."""
+        t = check_chunks({0: x}, 1)[0]
+        one = TimeStretch(self.device, 1, min(max(t.numel(), 1), self.MAX_IN))
+        try:
+            one.reset([0], speed)
             return one.push({0: t}, end=[0])[0]
         finally:
             one.close()

@@ -1,6 +1,8 @@
 """Shape/config records for the hot path; every value is read from the loaded HF config objects
 (never hard-coded: SURVEY §0 F6).  Mirrors core/models/configuration_qwen3_tts.py:187-212,370-404 and
 core/tokenizer_12hz/configuration_qwen3_tts_tokenizer_v2.py:72-93 of the reference."""
+import math
+import numbers
 import operator
 from dataclasses import dataclass, field
 from typing import Tuple
@@ -192,14 +194,18 @@ class SpeakerEncoderConfig:
 
 SUPPORTED_RATES = (8000, 11025, 16000, 22050, 24000, 32000, 44100, 48000)
 ENCODINGS = ("f32", "s16", "ulaw")
+SPEED_RANGE = (0.5, 2.0)
 
 
 @dataclass(frozen=True)
 class AudioFormat:
-    """The sample rate and encoding of a client's audio: "f32" float32 samples, "s16" 16-bit PCM (int16), "ulaw" 8-bit
-    G.711 mu-law (uint8).  Rates: SUPPORTED_RATES.  Anything else raises ValueError on construction."""
+    """The sample rate, encoding and speaking rate of a client's audio: "f32" float32 samples, "s16" 16-bit PCM (int16),
+    "ulaw" 8-bit G.711 mu-law (uint8).  Rates: SUPPORTED_RATES.  `speed`: a real number in SPEED_RANGE, the pace of the
+    speech (1.25 is 25 % faster, same pitch; audio.TimeStretch, resolution 1/480).  Anything else raises ValueError on
+    construction."""
     sample_rate: int
     encoding: str = "f32"
+    speed: float = 1.0
 
     def __post_init__(self):
         try:
@@ -210,4 +216,9 @@ class AudioFormat:
             raise ValueError(f"sample_rate {self.sample_rate!r} is not supported; supported rates: {SUPPORTED_RATES}")
         if not isinstance(self.encoding, str) or self.encoding not in ENCODINGS:
             raise ValueError(f"encoding {self.encoding!r} is not supported; supported encodings: {ENCODINGS}")
+        sp = self.speed
+        if isinstance(sp, bool) or not isinstance(sp, numbers.Real) or not math.isfinite(float(sp)) \
+                or not SPEED_RANGE[0] <= float(sp) <= SPEED_RANGE[1]:
+            raise ValueError(f"speed {sp!r} is not a real number in [{SPEED_RANGE[0]}, {SPEED_RANGE[1]}]")
         object.__setattr__(self, "sample_rate", sr)
+        object.__setattr__(self, "speed", float(sp))

@@ -69,6 +69,16 @@ bank copy alike: the resampled audio is the generated part's), saved on the requ
 its new slot when resumed.  A request's concatenated chunks equal Resampler.oneshot of its whole audio
 (tests/test_gpu_scheduler_audio_format.py).  Requests in the codec's own format take today's path, so a session
 without formats makes the same calls as before.
+
+Speaking rate (`AudioFormat(speed=)`): a request whose speed gives an analysis hop other than 480
+(audio.TimeStretch.hop) has a row of one audio.TimeStretch of `n_slots` rows, opened when the first such request is
+admitted.  Its slot's new samples go through one time-stretch launch with every other such slot on the device, then
+through its resampler row if its rate or encoding is not 24 kHz float32; a finishing request ends its stretch row and
+passes that tail into its resampler end in the same step.  The row is reset at admission after the codec row's reset,
+seed or bank copy (it stretches the generated part only), saved on park, loaded on resume and dropped on cancel.  A
+request's concatenated chunks equal Resampler.oneshot(TimeStretch.oneshot(w, speed), 24000, its rate and encoding), w
+its whole waveform (tests/test_gpu_scheduler_speed.py).  A session where no request has another speed makes the same
+calls as before.
 """
 from collections import deque
 from dataclasses import dataclass, field
@@ -103,8 +113,15 @@ class _Request:
     bank: Optional[Tuple[int, int]] = None
     codes: Optional[torch.Tensor] = None
     overlay: Optional[torch.Tensor] = None   # prompt rows still waiting for a text row each (None once complete)
-    fmt: Optional[AudioFormat] = None        # the client's audio format; None: the codec's own (no resampler row)
+    fmt: Optional[AudioFormat] = None        # the client's rate and encoding; None: the codec's own (no resampler row)
     res_state: Optional[torch.Tensor] = None   # while parked: its resampler row's saved state
+    speed: Optional[float] = None            # the client's speaking rate; None: as generated (no time-stretch row)
+    st_state: Optional[torch.Tensor] = None    # while parked: its time-stretch row's saved state
+
+    @property
+    def shaped(self) -> bool:
+        """Its audio goes through a time-stretch or a resampler row."""
+        return self.fmt is not None or self.speed is not None
 
 
 class ContinuousBatcher:
@@ -142,17 +159,28 @@ class ContinuousBatcher:
             self.cstream = codec.open_stream(self.n_slots, max_packet_frames=self.packet) if codec is not None else None
         else:
             raise ValueError(f"codec must be a CodecDecoder or a CodecStream, got {type(codec).__name__}")
-        self.audio_format = self._check_format(audio_format)
+        self._check_format(audio_format)
+        self.audio_format = audio_format
         self.resampler: Optional[audio.Resampler] = None   # opened when the first request with a format is admitted
+        self.stretcher: Optional[audio.TimeStretch] = None   # opened when the first request with a speed is admitted
 
     def _check_format(self, fmt: Optional[AudioFormat]) -> Optional[AudioFormat]:
-        """The format a request streams in: None for the codec's own 24 kHz float32 (no resampling)."""
+        """The rate and encoding a request's resampler row converts to: None for the codec's own 24 kHz float32 (no
+        resampling)."""
         if fmt is None:
             return None
         audio.check_format(fmt)
         if self.codec is None:
             raise ValueError("an audio format needs a ContinuousBatcher built with a codec")
+        fmt = AudioFormat(fmt.sample_rate, fmt.encoding)
         return None if fmt == AudioFormat(audio.CODEC_RATE) else fmt
+
+    @staticmethod
+    def _speed(fmt: Optional[AudioFormat]) -> Optional[float]:
+        """The speed a request's time-stretch row runs at: None when its hop is 480 (no stretch)."""
+        if fmt is None or audio.TimeStretch.hop(fmt.speed) == audio.TimeStretch.HS:
+            return None
+        return fmt.speed
 
     # ------------------------------------------------------------------ API
     def submit(self, inputs_embeds: torch.Tensor, trailing_text: Optional[torch.Tensor] = None, key: Optional[int] = None,
@@ -174,7 +202,8 @@ class ContinuousBatcher:
         request is admitted once it is full or its text is closed (see the module docstring).  `audio_format`: the
         sample rate and encoding of the request's stream() chunks (default: the session's).  Bad parameters raise
         ValueError here, never in a later step()."""
-        fmt = self._check_format(audio_format) if audio_format is not None else self.audio_format
+        src = audio_format if audio_format is not None else self.audio_format
+        fmt, speed = self._check_format(src), self._speed(src)
         H = self.eng.cfg.talker.hidden_size
         L_ref, P = 0, 0
         if overlay is not None:
@@ -226,7 +255,7 @@ class ContinuousBatcher:
         if self.codec is not None:
             horizon = min(horizon, self.codec.max_frames - L_ref)  # a codec row's position may not pass its RoPE table
         r = _Request(rid, inputs_embeds, tr, horizon, sampling, ref_codes, voice, text_open=bool(text_open),
-                     overlay=overlay if K else None, fmt=fmt)
+                     overlay=overlay if K else None, fmt=fmt, speed=speed)
         if r.overlay is not None:
             r.trailing = self._fill(r, tr.reshape(-1, H))
         r.n_text = int(r.trailing.reshape(-1, H).shape[0])
@@ -314,11 +343,11 @@ class ContinuousBatcher:
                 self._cancelled.add(rid)
                 return True
         r = self.parked.pop(rid, None)
-        if r is not None:    # its record, its codec bank row and its resampler state are freed
+        if r is not None:    # its record, its codec bank row and its resampler and time-stretch states are freed
             self.eng.discard(r.record)
             if r.bank is not None:
                 self.codec.bank_release(*r.bank)
-            r.res_state = None
+            r.res_state = r.st_state = None
             self._cancelled.add(rid)
             return True
         return False
@@ -357,6 +386,8 @@ class ContinuousBatcher:
             r.bank = self.codec.bank_copy(self.cstream, slot)
         if r.fmt is not None:
             r.res_state = self.resampler.save([slot])
+        if r.speed is not None:
+            r.st_state = self.stretcher.save([slot])
         r.trailing = r.trailing.reshape(-1, self.eng.cfg.talker.hidden_size)[:0]   # the record holds the text so far
         r.slot = -1
         self.parked[r.rid] = r
@@ -379,6 +410,9 @@ class ContinuousBatcher:
         if r.res_state is not None:
             self.resampler.load([slot], r.res_state)
             r.res_state = None
+        if r.st_state is not None:
+            self.stretcher.load([slot], r.st_state)
+            r.st_state = None
         if r.trailing.shape[0] > 0:
             self.eng.append_trailing(slot, r.trailing)
             r.trailing = r.trailing[:0]
@@ -469,6 +503,10 @@ class ContinuousBatcher:
                     if self.resampler is None:
                         self.resampler = audio.Resampler(self.eng.device, self.n_slots, self.packet * self.codec.total_upsample)
                     self.resampler.reset([r.slot for r in batch if r.fmt == fmt], audio.CODEC_RATE, fmt)
+                for speed in dict.fromkeys(r.speed for r in batch if r.speed is not None):   # one reset per speed
+                    if self.stretcher is None:
+                        self.stretcher = audio.TimeStretch(self.eng.device, self.n_slots, self.packet * self.codec.total_upsample)
+                    self.stretcher.reset([r.slot for r in batch if r.speed == speed], speed)
         if not batch and not self._runnable():
             return {}, []   # every running row is open and waiting for text: launch nothing
         n = min([self.packet] + [r.max_frames - r.emitted for r in self.running.values()])
@@ -499,10 +537,10 @@ class ContinuousBatcher:
         if self.cstream is None:
             return {}
         m = max([k for _, _, k in new.values()], default=0)
-        ending = [slot for slot, (r, _, _) in new.items() if r.fmt is not None and self.running.get(slot) is not r]
+        ending = [slot for slot, (r, _, _) in new.items() if r.shaped and self.running.get(slot) is not r]
         if m == 0 and not ending:
             return {}
-        if any(r.fmt is not None for r, _, _ in new.values()):
+        if any(r.shaped for r, _, _ in new.values()):
             return self._push_formats(new, m, ending)
         start, counts = [0] * self.n_slots, [0] * self.n_slots
         for slot, (_, e0, k) in new.items():
@@ -516,7 +554,8 @@ class ContinuousBatcher:
 
     def _push_formats(self, new, m: int, ending: List[int]) -> Dict[int, np.ndarray]:
         """_push_audio of a step in which some request has a format: the codec push stays on the device, the default
-        slots' audio comes back as before, the others' through the resampler."""
+        slots' audio comes back as before, the others' through the time-stretch (requests with a speed), then the
+        resampler (requests with a rate or encoding other than 24 kHz float32)."""
         up = self.codec.total_upsample
         out: Dict[int, np.ndarray] = {}
         wav = None
@@ -528,17 +567,49 @@ class ContinuousBatcher:
             rows = torch.arange(self.n_slots)[:, None]
             codes = self.codes[rows.to(self.codes.device), idx.to(self.codes.device)].transpose(1, 2)  # [S][G][m]
             wav = self.cstream.push(codes, counts)[:, 0]
-            plain = [slot for slot, (r, _, k) in new.items() if r.fmt is None and k > 0]
+            plain = [slot for slot, (r, _, k) in new.items() if not r.shaped and k > 0]
             if plain:
                 host = wav[plain].cpu().numpy()
                 for i, slot in enumerate(plain):
                     out[new[slot][0].rid] = host[i, :new[slot][2] * up]
-        res = {slot: k * up for slot, (r, _, k) in new.items() if r.fmt is not None and k > 0}
-        got = self.resampler.push_rows(wav, res, ending)
-        for slot, y in got.items():
-            if y.shape[0] or slot in ending:   # the filter's delay can hold a short push back entirely
-                out[new[slot][0].rid] = y
+        x, res = wav, {slot: k * up for slot, (r, _, k) in new.items() if r.fmt is not None and k > 0}
+        resample = True
+        if any(r.speed is not None for r, _, _ in new.values()):
+            x, res = self._push_speeds(new, wav, x, res, ending, out)
+            resample = any(new[slot][0].fmt is not None for slot in list(res) + ending)
+        if resample:
+            got = self.resampler.push_rows(x, res, [slot for slot in ending if new[slot][0].fmt is not None])
+            for slot, y in got.items():
+                if y.shape[0] or slot in ending:   # the filter's delay can hold a short push back entirely
+                    out[new[slot][0].rid] = y
         return out
+
+    def _push_speeds(self, new, wav, x, res, ending: List[int], out):
+        """The time-stretch launch of _push_formats: slots of requests with a speed take their new samples, and those
+        that finished in the step end their clips (their tails come even without new frames).  A stretched request
+        without a resampler row gets its output in `out`; for the others, returns the resampler's (input, counts):
+        the stretched output in their rows, each finished one's tail passed into its resampler end."""
+        up = self.codec.total_upsample
+        st = {slot: k * up for slot, (r, _, k) in new.items() if r.speed is not None and k > 0}
+        st_end = [slot for slot in ending if new[slot][0].speed is not None]
+        both = any(new[slot][0].fmt is not None for slot in set(st) | set(st_end))
+        got = self.stretcher.push_rows(wav if st else None, st, st_end, host=not both)
+        for slot, y in got.items():
+            if new[slot][0].fmt is None and (y.shape[0] or slot in ending):   # frames wait for 1200 samples
+                out[new[slot][0].rid] = y if not both else y.cpu().numpy()
+        if not both:
+            return x, res
+        chained = {slot: y for slot, y in got.items() if new[slot][0].fmt is not None}
+        res = {slot: c for slot, c in res.items() if slot not in chained}
+        res.update({slot: int(y.shape[0]) for slot, y in chained.items()})
+        L = max(res.values(), default=0)
+        if L == 0:
+            return None, res
+        x = torch.zeros(self.n_slots, L, dtype=torch.float32, device=self.eng.device)
+        for slot, c in res.items():
+            if c:
+                x[slot, :c] = chained[slot] if slot in chained else wav[slot, :c]
+        return x, res
 
     def run(self) -> Dict[int, torch.Tensor]:
         """Drain the queue; returns {request id: (N_i, G) codes}.  Requests with open text must be closed first (or

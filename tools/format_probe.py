@@ -1,9 +1,11 @@
 """Cost of audio formats in the continuous batcher, on the GPU: the resampler kernel's time (CUDA events around its
 launches) and the batcher's _push_audio time per step (host clock ending in a synchronise), at 8 and 32 slots with the
 default codec and 4-frame packets, for all rows in the default format, all rows 8 kHz mu-law and all rows 48 kHz
-float32.  Prints one JSON line, with the card's name and power limit read in the same run.
+float32.  With --speed, the same for every row at each of the given speaking rates (24 kHz float32, so only the
+time-stretch runs), and the time-stretch step (CUDA events around q3_stretch_step_rows calls of one packet per row)
+instead of the resampler's.  Prints one JSON line, with the card's name and power limit read in the same run.
 
-    python tools/format_probe.py [--steps 60] [--warmup 10]
+    python tools/format_probe.py [--steps 60] [--warmup 10] [--speed 0.5 1.25 2.0]
 """
 import argparse
 import ctypes as C
@@ -47,6 +49,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=60)
     ap.add_argument("--warmup", type=int, default=10)
+    ap.add_argument("--speed", type=float, nargs="*", default=None)
     a = ap.parse_args()
     import torch
     import qwen3_tts_b200 as q
@@ -60,6 +63,8 @@ def main():
     dec = CodecDecoder(ccfg, synthetic.random_codec_weights(ccfg, device="cpu", seed=0), device=dev, max_frames=1024)
     P, up = 4, dec.total_upsample
     formats = {"default": None, "8k_ulaw": q.AudioFormat(8000, "ulaw"), "48k_f32": q.AudioFormat(48000, "f32")}
+    if a.speed:
+        formats = {"default": None, **{f"speed_{sp}": q.AudioFormat(24000, speed=sp) for sp in a.speed}}
     results = []
     g = torch.Generator().manual_seed(0)
     for S in (8, 32):
@@ -67,14 +72,17 @@ def main():
             cb = ContinuousBatcher(_Engine(dev), torch.zeros(8), q.SamplingParams(max_new_tokens=2048), n_slots=S,
                                    packet_frames=P, codec=dec)
             cb.codes.copy_(torch.randint(0, ccfg.codebook_size, cb.codes.shape, generator=g).to(cb.codes))
-            reqs = [_Request(s, None, None, 2000, fmt=cb._check_format(fmt)) for s in range(S)]
+            reqs = [_Request(s, None, None, 2000, fmt=cb._check_format(fmt), speed=cb._speed(fmt)) for s in range(S)]
             for s, r in enumerate(reqs):
                 r.slot = s
                 cb.running[s] = r
             cb.cstream.reset()
-            if fmt is not None:
+            if reqs[0].fmt is not None:
                 cb.resampler = audio.Resampler(dev, S, P * up)
-                cb.resampler.reset(range(S), audio.CODEC_RATE, fmt)
+                cb.resampler.reset(range(S), audio.CODEC_RATE, reqs[0].fmt)
+            if reqs[0].speed is not None:
+                cb.stretcher = audio.TimeStretch(dev, S, P * up)
+                cb.stretcher.reset(range(S), reqs[0].speed)
             times = []
             for it in range(a.warmup + a.steps):
                 new = {s: (r, it * P, P) for s, r in enumerate(reqs)}
@@ -86,14 +94,14 @@ def main():
                     times.append(time.perf_counter() - t0)
             row = {"slots": S, "format": name, "push_audio_ms_mean": 1e3 * sum(times) / len(times),
                    "push_audio_ms_min": 1e3 * min(times)}
-            if fmt is not None:    # one resampler step (its job upload and kernel) of one packet per row
-                res = cb.resampler
+            if fmt is not None:    # one resampler or time-stretch step (its job upload and kernel) of one packet per row
+                res = cb.stretcher if reqs[0].speed is not None else cb.resampler
+                fn = res.lib.q3_stretch_step_rows if reqs[0].speed is not None else res.lib.q3_resample_step_rows
                 x = torch.rand(S, P * up, device=dev) * 2 - 1
                 cnt, end = (C.c_int32 * S)(*[P * up] * S), (C.c_int32 * S)()
                 nout = (C.c_int32 * S)()
                 st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-                step = lambda: _lib.check(res.lib.q3_resample_step_rows(res.h, x.data_ptr(), x.stride(0), cnt, end,  # noqa: E731
-                                                                        res._out.data_ptr(), nout, st))
+                step = lambda: _lib.check(fn(res.h, x.data_ptr(), x.stride(0), cnt, end, res._out.data_ptr(), nout, st))  # noqa: E731
                 for _ in range(a.warmup):
                     step()
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -103,7 +111,7 @@ def main():
                     step()
                 e1.record()
                 torch.cuda.synchronize()
-                row["resample_step_us"] = 1e3 * e0.elapsed_time(e1) / n
+                row["stretch_step_us" if reqs[0].speed is not None else "resample_step_us"] = 1e3 * e0.elapsed_time(e1) / n
                 row["outputs_per_row"] = int(nout[0])
                 res.close()
             cb.cstream.close()
