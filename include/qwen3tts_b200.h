@@ -381,7 +381,12 @@ void q3_codec_enc_stream_close(q3_codec_enc_stream* s);
  *   (4*max_out bytes).  Device memory of the object is its own.
  * add_filter: copies the device taps (fp32 [ntaps]) into the object and returns their id in *id_out.  A filter may
  *   not read more than Q3_RESAMPLE_HIST inputs back (floor(2*hl/up)), nor emit more than max_out samples from a push of
- *   max_in inputs plus its end (ceil(max_in*up/down) + ceil(hl/down) + 1).  At most 16 filters.
+ *   max_in inputs plus its end (ceil(max_in*up/down) + ceil(hl/down) + 1).  At most 64 filters at a time; a new filter
+ *   takes the lowest free id, so an id dropped by drop_filter may come back for another filter.
+ * drop_filter: frees filter `id` and its id.  Refused while any row uses it (reset or loaded with it and not released
+ *   since).  Drains the device first, as launches queued on any stream may read its taps.
+ * release_rows: the n rows in rows_host no longer use their filters; they may take neither inputs nor an end until they
+ *   are reset or loaded again.  Host state only.
  * reset_rows: the n rows in rows_host start new clips with filter filters_host[i] and encoding encodings_host[i]
  *   (Q3_RESAMPLE_F32 / S16 / ULAW).  Host state only, no device work.
  * step_rows: one launch over every row.  Row r takes counts_host[r] (0..max_in) fp32 inputs at in_dev + r*ld and, when
@@ -392,7 +397,9 @@ void q3_codec_enc_stream_close(q3_codec_enc_stream* s);
  * save_rows: the n listed rows' state (filter id, encoding, inputs so far, history) to dst_dev, Q3_RESAMPLE_ROW_BYTES
  *   bytes per row in list order.  Asynchronous.
  * load_rows: the n listed rows continue the states saved at src_dev (by this object): reads the records' headers back
- *   to the host (synchronises `stream`), then copies the histories asynchronously.
+ *   to the host (synchronises `stream`), then copies the histories asynchronously.  A record's filter id (its first 4
+ *   bytes) must name a live filter: a caller that dropped the filter since the save adds it again and writes its new
+ *   id there first.
  * Bad arguments (a row out of range or listed twice, a count outside [0, max_in] or above ld, an unknown filter or
  *   encoding, a row never reset, null pointers) are rejected before any device work and change nothing. */
 #define Q3_RESAMPLE_HIST 128
@@ -406,6 +413,8 @@ void q3_resample_close(q3_resampler* s);
 int q3_resample_add_filter(q3_resampler* s, int32_t up, int32_t down, const float* taps_dev, int32_t ntaps, int32_t* id_out);
 int q3_resample_reset_rows(q3_resampler* s, int32_t n, const int32_t* rows_host, const int32_t* filters_host,
                            const int32_t* encodings_host);
+int q3_resample_drop_filter(q3_resampler* s, int32_t id);
+int q3_resample_release_rows(q3_resampler* s, int32_t n, const int32_t* rows_host);
 int q3_resample_step_rows(q3_resampler* s, const float* in_dev, int64_t ld, const int32_t* counts_host,
                           const int32_t* end_host, void* out_dev, int32_t* nout_host, void* stream);
 int q3_resample_save_rows(q3_resampler* s, int32_t n, const int32_t* rows_host, void* dst_dev, void* stream);
@@ -443,6 +452,36 @@ int q3_stretch_step_rows(q3_stretcher* s, const float* in_dev, int64_t ld, const
                          const int32_t* end_host, float* out_dev, int32_t* nout_host, void* stream);
 int q3_stretch_save_rows(q3_stretcher* s, int32_t n, const int32_t* rows_host, void* dst_dev, void* stream);
 int q3_stretch_load_rows(q3_stretcher* s, int32_t n, const int32_t* rows_host, const void* src_dev, void* stream);
+
+/* ---------------------------------------------------------------- volume (streaming look-ahead limiter)
+ * A gain that cannot clip, at the codec's 24 kHz, with peaks held at c = fp32(10^(-1/20)) (-1 dBFS).  Row gain g (fp32,
+ * designed by the caller), u[n] = g*x[n] (x = 0 before the clip and past its end):
+ *   a[n] = 1 if |u[n]| <= c, else c/|u[n]|;   b[m] = min a[m .. m+119];
+ *   s[n] = min(a[n], (b[n] + b[n-1] + ... + b[n-119]) * fp32(1/120))   summed from b[n] down;
+ *   G[n] = min over m in [max(0, n-1200), n] of s[m] + fp32(n-m) * fp32(1/1200);   y[n] = u[n] * G[n],
+ * every operation fp32 round-to-nearest in that order, without contraction.  A clip of n samples gives n samples; output
+ * n reads inputs up to n + 119, so after n inputs without an end a row has emitted E(n) = max(0, n - 119), and an end
+ * emits the rest.  A clip streamed in pushes of any sizes equals the clip pushed at once, bit for bit.
+ * open: `rows` rows; a step gives each row at most max_in inputs; each row's output capacity is max_out fp32 samples, at
+ *   least max_in + 119.  Device memory of the object is its own.
+ * reset_rows: the n rows in rows_host start new clips with gain gains_host[i] (positive, finite).  Host state only.
+ * step_rows: one launch over every row.  Row r takes counts_host[r] (0..max_in) fp32 inputs at in_dev + r*ld and, when
+ *   end_host[r] != 0, ends its clip (it then starts a new one with the same gain).  Its new outputs go to
+ *   out_dev + r*max_out, their count to nout_host[r], known without a sync.  A row with count 0 and no end is
+ *   untouched.  A row never reset may take neither inputs nor an end.  Asynchronous on `stream`.
+ * save_rows / load_rows: as q3_resample_save_rows / load_rows, Q3_LIMIT_ROW_BYTES per row (gain, inputs so far, the last
+ *   Q3_LIMIT_HIST inputs).  load synchronises.
+ * Bad arguments are rejected before any device work and change nothing. */
+#define Q3_LIMIT_HIST 1536
+#define Q3_LIMIT_ROW_BYTES 6160
+typedef struct q3_limiter q3_limiter;
+int q3_limit_open(int32_t rows, int32_t max_in, int32_t max_out, int32_t device, q3_limiter** out);
+void q3_limit_close(q3_limiter* s);
+int q3_limit_reset_rows(q3_limiter* s, int32_t n, const int32_t* rows_host, const float* gains_host);
+int q3_limit_step_rows(q3_limiter* s, const float* in_dev, int64_t ld, const int32_t* counts_host,
+                       const int32_t* end_host, float* out_dev, int32_t* nout_host, void* stream);
+int q3_limit_save_rows(q3_limiter* s, int32_t n, const int32_t* rows_host, void* dst_dev, void* stream);
+int q3_limit_load_rows(q3_limiter* s, int32_t n, const int32_t* rows_host, const void* src_dev, void* stream);
 
 /* ---------------------------------------------------------------- speaker x-vector (voice cloning)
  * Replaces Qwen3TTSForConditionalGeneration.extract_speaker_embedding (core/models/modeling_qwen3_tts.py:1941-1954):

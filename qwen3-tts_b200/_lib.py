@@ -79,8 +79,11 @@ CODEC_SYMBOLS = ["q3_codec_create", "q3_codec_destroy", "q3_codec_load_tensor", 
                  "q3_spk_embed", "q3_spk_last_launch_count",
                  "q3_resample_open", "q3_resample_close", "q3_resample_add_filter", "q3_resample_reset_rows",
                  "q3_resample_step_rows", "q3_resample_save_rows", "q3_resample_load_rows",
+                 "q3_resample_drop_filter", "q3_resample_release_rows",
                  "q3_stretch_open", "q3_stretch_close", "q3_stretch_set_window", "q3_stretch_reset_rows",
-                 "q3_stretch_step_rows", "q3_stretch_save_rows", "q3_stretch_load_rows"]
+                 "q3_stretch_step_rows", "q3_stretch_save_rows", "q3_stretch_load_rows",
+                 "q3_limit_open", "q3_limit_close", "q3_limit_reset_rows", "q3_limit_step_rows", "q3_limit_save_rows",
+                 "q3_limit_load_rows"]
 
 _lib = None
 
@@ -190,6 +193,8 @@ def load():
         lib.q3_resample_step_rows.argtypes = [vp, vp, i64, C.POINTER(i32), C.POINTER(i32), vp, C.POINTER(i32), vp]
         lib.q3_resample_save_rows.argtypes = [vp, i32, C.POINTER(i32), vp, vp]
         lib.q3_resample_load_rows.argtypes = [vp, i32, C.POINTER(i32), vp, vp]
+        lib.q3_resample_drop_filter.argtypes = [vp, i32]
+        lib.q3_resample_release_rows.argtypes = [vp, i32, C.POINTER(i32)]
         lib.q3_stretch_open.argtypes = [i32, i32, i32, i32, C.POINTER(vp)]
         lib.q3_stretch_close.argtypes = [vp]
         lib.q3_stretch_close.restype = None
@@ -198,6 +203,13 @@ def load():
         lib.q3_stretch_step_rows.argtypes = [vp, vp, i64, C.POINTER(i32), C.POINTER(i32), vp, C.POINTER(i32), vp]
         lib.q3_stretch_save_rows.argtypes = [vp, i32, C.POINTER(i32), vp, vp]
         lib.q3_stretch_load_rows.argtypes = [vp, i32, C.POINTER(i32), vp, vp]
+        lib.q3_limit_open.argtypes = [i32, i32, i32, i32, C.POINTER(vp)]
+        lib.q3_limit_close.argtypes = [vp]
+        lib.q3_limit_close.restype = None
+        lib.q3_limit_reset_rows.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(C.c_float)]
+        lib.q3_limit_step_rows.argtypes = [vp, vp, i64, C.POINTER(i32), C.POINTER(i32), vp, C.POINTER(i32), vp]
+        lib.q3_limit_save_rows.argtypes = [vp, i32, C.POINTER(i32), vp, vp]
+        lib.q3_limit_load_rows.argtypes = [vp, i32, C.POINTER(i32), vp, vp]
     _lib = lib
     return lib
 

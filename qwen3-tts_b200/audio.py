@@ -13,10 +13,20 @@ emitted as soon as input floor((hl + j*down) / up) has arrived, so after n input
 an end emits the rest, as if the clip were followed by zeros.  A clip pushed in pieces of any sizes and ended equals
 oneshot() of the whole clip bit for bit, and one launch serves every row of a push.
 
+Pitch: a clip time-stretched at 24 kHz and then taken as sampled at 50*Lp Hz (AudioFormat.pitch_step) is resampled
+from that rate in one pass: reset / oneshot take such a rate (a multiple of 50 Hz in [12000, 48000]) as in_rate.  The
+native table holds MAX_FILTERS filters; each pair's filter is designed on its first use and kept until the table is full
+and a new pair needs its entry, when the least recently used pair no row uses is dropped.  save() keeps each row's pair
+with its state, so load() adds a dropped filter again.
+
 Speaking rate: TimeStretch, a streaming per-row WSOLA time-stretch at 24 kHz (q3_stretch_*, csrc/stretch.cu, DESIGN
 §4.7), with the same streaming contract; the batcher runs it before the resampler.
+
+Volume: Limiter, a streaming per-row look-ahead limiter at 24 kHz (q3_limit_*, csrc/limit.cu, DESIGN §4.8), with the
+same streaming contract; the batcher runs it between the time-stretch and the resampler.
 """
 import ctypes as C
+from dataclasses import dataclass
 from math import gcd
 from typing import Dict, Iterable, List, Optional, Tuple
 
@@ -35,11 +45,20 @@ _NP_DTYPE = {"f32": np.float32, "s16": np.int16, "ulaw": np.uint8}
 _WIDTH = {"f32": 4, "s16": 2, "ulaw": 1}
 
 
-def ratio(sr_in: int, sr_out: int) -> Tuple[int, int]:
-    """(up, down): sr_out / sr_in in lowest terms.  ValueError for a rate outside SUPPORTED_RATES."""
-    for sr in (sr_in, sr_out):
-        if isinstance(sr, bool) or not isinstance(sr, (int, np.integer)) or int(sr) not in SUPPORTED_RATES:
-            raise ValueError(f"sample rate {sr!r} is not supported; supported rates: {SUPPORTED_RATES}")
+MAX_FILTERS = 64                   # kMaxFilters: filters a resampler holds at a time
+PITCHED_RATES = (12000, 48000)     # the range of 50*Lp, the rate a pitch-shifted clip is resampled from
+
+
+def ratio(sr_in: int, sr_out: int, pitched: bool = False) -> Tuple[int, int]:
+    """(up, down): sr_out / sr_in in lowest terms.  ValueError for a rate outside SUPPORTED_RATES, except that with
+    `pitched` sr_in may also be a multiple of 50 Hz in PITCHED_RATES."""
+    for sr, alt in ((sr_in, pitched), (sr_out, False)):
+        ok = not isinstance(sr, bool) and isinstance(sr, (int, np.integer)) and (
+            int(sr) in SUPPORTED_RATES
+            or (alt and int(sr) % 50 == 0 and PITCHED_RATES[0] <= int(sr) <= PITCHED_RATES[1]))
+        if not ok:
+            raise ValueError(f"sample rate {sr!r} is not supported; supported rates: {SUPPORTED_RATES}"
+                             + (f", or as input a multiple of 50 Hz in {list(PITCHED_RATES)}" if alt else ""))
     g = gcd(int(sr_in), int(sr_out))
     return int(sr_out) // g, int(sr_in) // g
 
@@ -79,11 +98,20 @@ def check_format(fmt) -> AudioFormat:
     return fmt
 
 
+@dataclass
+class ResamplerState:
+    """Rows' saved resampler state: the native records (uint8 (n, ROW_BYTES) on the device) and each row's (up, down)
+    pair, whose filter may have been dropped and added again under another id by the time the rows are loaded."""
+    records: torch.Tensor
+    pairs: List[Tuple[int, int]]
+
+
 class Resampler:
     """`rows` streaming resampler rows on `device`; a push gives each row at most `max_in` samples per launch (longer
     pushes take several launches).  reset(rows, in_rate, fmt) starts new clips; push({row: samples}, end=rows) returns
     {row: numpy array of the row's new output} in the row's encoding (float32, int16 or uint8); push_device keeps them
-    on the device; save(rows) / load(rows, state) move rows' state; oneshot(x, in_rate, fmt) converts a whole clip."""
+    on the device; save(rows) / load(rows, state) move rows' state; release(rows) frees rows' filters for reuse;
+    oneshot(x, in_rate, fmt) converts a whole clip."""
 
     def __init__(self, device, rows: int, max_in: int):
         self.lib = _lib.load()
@@ -96,7 +124,8 @@ class Resampler:
         h = C.c_void_p()
         _lib.check(self.lib.q3_resample_open(self.rows, self.max_in, self.max_out, self.device.index or 0, C.byref(h)))
         self.h = h
-        self._filters: Dict[Tuple[int, int], int] = {}
+        self._filters: Dict[Tuple[int, int], int] = {}     # pair -> filter id, least recently used first
+        self._pair: List[Optional[Tuple[int, int]]] = [None] * self.rows   # the pair each row uses
         self._enc: List[Optional[str]] = [None] * self.rows
         self._out = torch.empty(self.rows, 4 * self.max_out, dtype=torch.uint8, device=self.device)
 
@@ -116,20 +145,32 @@ class Resampler:
             raise RuntimeError("resampler is closed")
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
-    def _filter(self, up: int, down: int) -> int:
-        fid = self._filters.get((up, down))
+    def _filter(self, up: int, down: int, keep=()) -> int:
+        """The id of the pair's filter, designed and added on its first use.  When the table is full, the least
+        recently used pair that no row uses and that is not in `keep` is dropped first."""
+        pair = (up, down)
+        fid = self._filters.pop(pair, None)
         if fid is None:
+            if len(self._filters) >= MAX_FILTERS:
+                used = set(self._pair) | set(keep)
+                old = next((p for p in self._filters if p not in used), None)
+                if old is None:
+                    raise RuntimeError(f"all {MAX_FILTERS} resampler filters are in use by rows")
+                _lib.check(self.lib.q3_resample_drop_filter(self.h, self._filters.pop(old)))
             taps = torch.from_numpy(design(up, down)).to(self.device, torch.float32)
             out = C.c_int32()
             _lib.check(self.lib.q3_resample_add_filter(self.h, up, down, taps.data_ptr(), taps.numel(), C.byref(out)))
-            fid = self._filters[(up, down)] = out.value
+            fid = out.value
+        self._filters[pair] = fid
         return fid
 
     def reset(self, rows, in_rate: int, fmt: AudioFormat):
-        """Start new clips in `rows` converting in_rate -> fmt.sample_rate into fmt.encoding."""
+        """Start new clips in `rows` converting in_rate -> fmt.sample_rate into fmt.encoding.  in_rate is a supported
+        rate, or a multiple of 50 Hz in PITCHED_RATES (a pitch-shifted clip)."""
         rows = check_rows(rows, self.rows)
         fmt = check_format(fmt)
-        fid = self._filter(*ratio(in_rate, fmt.sample_rate))
+        pair = ratio(in_rate, fmt.sample_rate, pitched=True)
+        fid = self._filter(*pair)
         n = len(rows)
         if n == 0:
             return
@@ -137,7 +178,17 @@ class Resampler:
         _lib.check(self.lib.q3_resample_reset_rows(self.h, n, i32n(*rows), i32n(*[fid] * n),
                                                    i32n(*[_ENC_CODE[fmt.encoding]] * n)))
         for r in rows:
-            self._enc[r] = fmt.encoding
+            self._enc[r], self._pair[r] = fmt.encoding, pair
+
+    def release(self, rows):
+        """Rows `rows` no longer use their filters (which may then be dropped); they need a reset or a load before
+        their next push."""
+        rows = check_rows(rows, self.rows)
+        n = len(rows)
+        if n:
+            _lib.check(self.lib.q3_resample_release_rows(self.h, n, (C.c_int32 * n)(*rows)))
+        for r in rows:
+            self._enc[r] = self._pair[r] = None
 
     def _check_ready(self, rows):
         for r in rows:
@@ -221,34 +272,40 @@ class Resampler:
         out = self.push_rows(x, counts, end, host=False)
         return {r: out[r] for r in sorted(set(chunks) | set(end))}
 
-    def save(self, rows) -> torch.Tensor:
-        """The rows' state (filter, encoding, inputs so far, history): a uint8 (len(rows), ROW_BYTES) device tensor."""
+    def save(self, rows) -> ResamplerState:
+        """The rows' state: the native records (filter, encoding, inputs so far, history; a uint8 (len(rows),
+        ROW_BYTES) device tensor) with each row's rate pair."""
         rows = check_rows(rows, self.rows)
         self._check_ready(rows)
         state = torch.empty(len(rows), ROW_BYTES, dtype=torch.uint8, device=self.device)
         n = len(rows)
         if n:
             _lib.check(self.lib.q3_resample_save_rows(self.h, n, (C.c_int32 * n)(*rows), state.data_ptr(), self._stream()))
-        return state
+        return ResamplerState(state, [self._pair[r] for r in rows])
 
-    def load(self, rows, state: torch.Tensor):
-        """Rows `rows` continue the states save() returned (of this resampler), in order."""
+    def load(self, rows, state: ResamplerState):
+        """Rows `rows` continue the states save() returned (of this resampler), in order.  A pair whose filter was
+        dropped since is added again, and the records are loaded with each pair's current filter id."""
         rows = check_rows(rows, self.rows)
-        if not isinstance(state, torch.Tensor) or state.dtype != torch.uint8 or tuple(state.shape) != (len(rows), ROW_BYTES) \
-                or state.device != self.device:
-            raise ValueError(f"expected a saved state of shape ({len(rows)}, {ROW_BYTES}) on {self.device}")
+        rec = state.records if isinstance(state, ResamplerState) else None
+        if not isinstance(rec, torch.Tensor) or rec.dtype != torch.uint8 or tuple(rec.shape) != (len(rows), ROW_BYTES) \
+                or rec.device != self.device or len(state.pairs) != len(rows):
+            raise ValueError(f"expected a ResamplerState of {len(rows)} rows on {self.device}")
         n = len(rows)
         if n == 0:
             return
-        state = state.contiguous()
-        _lib.check(self.lib.q3_resample_load_rows(self.h, n, (C.c_int32 * n)(*rows), state.data_ptr(), self._stream()))
+        fids = [self._filter(*p, keep=state.pairs) for p in state.pairs]
+        rec = rec.clone()
+        rec[:, 0:4] = torch.tensor(fids, dtype=torch.int32).view(torch.uint8).reshape(n, 4).to(self.device)
+        _lib.check(self.lib.q3_resample_load_rows(self.h, n, (C.c_int32 * n)(*rows), rec.data_ptr(), self._stream()))
         inv = {v: k for k, v in _ENC_CODE.items()}
-        codes = state[:, 4:8].cpu().numpy().view(np.int32)[:, 0]   # the header's encoding (already read back natively)
-        for r, c in zip(rows, codes):
-            self._enc[r] = inv[int(c)]
+        codes = rec[:, 4:8].cpu().numpy().view(np.int32)[:, 0]   # the header's encoding (already read back natively)
+        for r, c, p in zip(rows, codes, state.pairs):
+            self._enc[r], self._pair[r] = inv[int(c)], p
 
     def oneshot(self, x, in_rate: int, fmt: AudioFormat) -> np.ndarray:
-        """The whole clip x (1-D float samples at in_rate) converted at once: the reference of the streamed result."""
+        """The whole clip x (1-D float samples at in_rate, which reset() takes) converted at once: the reference of the
+        streamed result."""
         t = check_chunks({0: x}, 1)[0]
         one = Resampler(self.device, 1, max(t.numel(), 1))
         try:
@@ -272,12 +329,14 @@ class TimeStretch:
     HIST = 2048                       # Q3_STRETCH_HIST: inputs a row keeps
     ROW_BYTES = 10144                 # Q3_STRETCH_ROW_BYTES: one row's saved state
     MAX_IN = 32768                    # the largest max_in the native stretcher takes
+    _STEP = "q3_stretch_step_rows"
 
     @staticmethod
-    def hop(speed) -> int:
-        """The analysis hop of `speed`: floor(speed*480 + 0.5); the effective speed is hop/480.  ValueError outside
-        [0.5, 2.0] (AudioFormat's check)."""
-        return int(np.floor(AudioFormat(CODEC_RATE, speed=speed).speed * 480 + 0.5))
+    def hop(speed, pitch=0.0) -> int:
+        """The analysis hop of `speed` at `pitch` semitones (AudioFormat.hop): floor(speed*480*(480/Lp) + 0.5), which
+        is floor(speed*480 + 0.5) at pitch 0; the effective speed is hop*Lp/480^2.  ValueError outside AudioFormat's
+        ranges, or for a hop outside [240, 960]."""
+        return AudioFormat(CODEC_RATE, speed=speed, pitch=pitch).hop
 
     @staticmethod
     def emitted(n: int, ha: int) -> int:
@@ -333,10 +392,10 @@ class TimeStretch:
             raise RuntimeError("time-stretch is closed")
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
-    def reset(self, rows, speed):
-        """Start new clips in `rows` at `speed` (analysis hop hop(speed))."""
+    def reset(self, rows, speed, pitch=0.0):
+        """Start new clips in `rows` at `speed` and `pitch` (analysis hop hop(speed, pitch))."""
         rows = check_rows(rows, self.rows)
-        ha = self.hop(speed)
+        ha = self.hop(speed, pitch)
         n = len(rows)
         if n == 0:
             return
@@ -367,7 +426,7 @@ class TimeStretch:
             e = [int(r in end and (s0 == 0 if cnt[r] == 0 else s0 < cnt[r] <= s0 + self.max_in)) for r in range(self.rows)]
             nout = (C.c_int32 * self.rows)()
             ptr = x.data_ptr() + 4 * s0 if x is not None and any(k) else None
-            _lib.check(self.lib.q3_stretch_step_rows(self.h, ptr, x.stride(0) if x is not None else 0,
+            _lib.check(getattr(self.lib, self._STEP)(self.h, ptr, x.stride(0) if x is not None else 0,
                                                      (C.c_int32 * self.rows)(*k), (C.c_int32 * self.rows)(*e),
                                                      self._out.data_ptr(), nout, st))
             nb = {r: nout[r] for r in touched}
@@ -440,12 +499,130 @@ class TimeStretch:
         for r, ha in zip(rows, has):
             self._ha[r] = int(ha)
 
-    def oneshot(self, x, speed) -> np.ndarray:
+    def oneshot(self, x, speed, pitch=0.0) -> np.ndarray:
         """The whole clip x (1-D float samples at 24 kHz) stretched at once: the reference of the streamed result."""
         t = check_chunks({0: x}, 1)[0]
         one = TimeStretch(self.device, 1, min(max(t.numel(), 1), self.MAX_IN))
         try:
-            one.reset([0], speed)
+            one.reset([0], speed, pitch)
+            return one.push({0: t}, end=[0])[0]
+        finally:
+            one.close()
+
+
+class Limiter:
+    """`rows` streaming look-ahead limiter rows at the codec's 24 kHz on `device` (q3_limit_*, csrc/limit.cu, DESIGN
+    §4.8): a gain of `volume` dB whose peaks are held at -1 dBFS, with 5 ms of look-ahead and a linear release of at most
+    50 ms.  A clip of n samples gives n samples; after n samples without an end a row has emitted emitted(n) = max(0,
+    n - 119), so the limiter delays by 119 samples.  A push gives each row at most `max_in` samples per launch (longer
+    pushes take several launches).  reset(rows, volume) starts new clips; push({row: samples}, end=rows) returns {row:
+    float32 numpy array of the row's new output}; push_device keeps them on the device; save(rows) / load(rows, state)
+    move rows' state; oneshot(x, volume) limits a whole clip.  A clip pushed in pieces of any sizes and ended equals
+    oneshot() of the whole clip bit for bit."""
+
+    L, W = 120, 1200                  # look-ahead, release
+    DELAY = L - 1
+    HIST = 1536                       # Q3_LIMIT_HIST: inputs a row keeps (it reads W + 2L - 2 = 1438 back)
+    ROW_BYTES = 6160                  # Q3_LIMIT_ROW_BYTES: one row's saved state
+    _STEP = "q3_limit_step_rows"
+
+    @staticmethod
+    def gain(volume) -> np.float32:
+        """fp32(10^(volume/20)), designed in fp64.  ValueError outside AudioFormat's volume range."""
+        return np.float32(10.0 ** (AudioFormat(CODEC_RATE, volume=volume).volume / 20))
+
+    @classmethod
+    def emitted(cls, n: int) -> int:
+        """Outputs a row has emitted after n inputs without an end: max(0, n - 119)."""
+        return max(0, n - cls.DELAY)
+
+    @staticmethod
+    def total(n: int) -> int:
+        """Outputs of a whole clip of n inputs: n."""
+        return n
+
+    def __init__(self, device, rows: int, max_in: int):
+        self.lib = _lib.load()
+        self.device = torch.device(device)
+        if self.device.type != "cuda":
+            raise RuntimeError("Limiter needs a CUDA device (no CPU fallback)")
+        self.rows, self.max_in = int(rows), int(max_in)
+        self.max_out = self.max_in + self.DELAY
+        h = C.c_void_p()
+        _lib.check(self.lib.q3_limit_open(self.rows, self.max_in, self.max_out, self.device.index or 0, C.byref(h)))
+        self.h = h
+        self._gain: List[Optional[float]] = [None] * self.rows
+        self._out = torch.empty(self.rows, self.max_out, dtype=torch.float32, device=self.device)
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.q3_limit_close(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _stream(self):
+        if not self.h:
+            raise RuntimeError("limiter is closed")
+        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def reset(self, rows, volume):
+        """Start new clips in `rows` at `volume` dB (gain gain(volume))."""
+        rows = check_rows(rows, self.rows)
+        g = self.gain(volume)
+        n = len(rows)
+        if n == 0:
+            return
+        _lib.check(self.lib.q3_limit_reset_rows(self.h, n, (C.c_int32 * n)(*rows), (C.c_float * n)(*[g] * n)))
+        for r in rows:
+            self._gain[r] = float(g)
+
+    def _check_ready(self, rows):
+        for r in rows:
+            if self._gain[r] is None:
+                raise ValueError(f"row {r} was never reset")
+
+    _run = TimeStretch._run
+    push_rows = TimeStretch.push_rows
+    _pack = Resampler._pack
+    push = TimeStretch.push
+    push_device = TimeStretch.push_device
+
+    def save(self, rows) -> torch.Tensor:
+        """The rows' state (gain, inputs so far, history): a uint8 (len(rows), ROW_BYTES) device tensor."""
+        rows = check_rows(rows, self.rows)
+        self._check_ready(rows)
+        state = torch.empty(len(rows), self.ROW_BYTES, dtype=torch.uint8, device=self.device)
+        n = len(rows)
+        if n:
+            _lib.check(self.lib.q3_limit_save_rows(self.h, n, (C.c_int32 * n)(*rows), state.data_ptr(), self._stream()))
+        return state
+
+    def load(self, rows, state: torch.Tensor):
+        """Rows `rows` continue the states save() returned, in order."""
+        rows = check_rows(rows, self.rows)
+        if not isinstance(state, torch.Tensor) or state.dtype != torch.uint8 \
+                or tuple(state.shape) != (len(rows), self.ROW_BYTES) or state.device != self.device:
+            raise ValueError(f"expected a saved state of shape ({len(rows)}, {self.ROW_BYTES}) on {self.device}")
+        n = len(rows)
+        if n == 0:
+            return
+        state = state.contiguous()
+        _lib.check(self.lib.q3_limit_load_rows(self.h, n, (C.c_int32 * n)(*rows), state.data_ptr(), self._stream()))
+        gains = state[:, 0:4].cpu().numpy().view(np.float32)[:, 0]   # the header's gain (already read back natively)
+        for r, g in zip(rows, gains):
+            self._gain[r] = float(g)
+
+    def oneshot(self, x, volume) -> np.ndarray:
+        """The whole clip x (1-D float samples at 24 kHz) limited at once: the reference of the streamed result."""
+        t = check_chunks({0: x}, 1)[0]
+        one = Limiter(self.device, 1, max(t.numel(), 1))
+        try:
+            one.reset([0], volume)
             return one.push({0: t}, end=[0])[0]
         finally:
             one.close()

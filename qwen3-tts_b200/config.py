@@ -195,17 +195,29 @@ class SpeakerEncoderConfig:
 SUPPORTED_RATES = (8000, 11025, 16000, 22050, 24000, 32000, 44100, 48000)
 ENCODINGS = ("f32", "s16", "ulaw")
 SPEED_RANGE = (0.5, 2.0)
+PITCH_RANGE = (-12.0, 12.0)    # semitones
+VOLUME_RANGE = (-30.0, 12.0)   # dB
+
+
+def _real_in(name: str, v, lo: float, hi: float) -> float:
+    if isinstance(v, bool) or not isinstance(v, numbers.Real) or not math.isfinite(float(v)) or not lo <= float(v) <= hi:
+        raise ValueError(f"{name} {v!r} is not a real number in [{lo}, {hi}]")
+    return float(v)
 
 
 @dataclass(frozen=True)
 class AudioFormat:
-    """The sample rate, encoding and speaking rate of a client's audio: "f32" float32 samples, "s16" 16-bit PCM (int16),
+    """The sample rate, encoding and prosody of a client's audio: "f32" float32 samples, "s16" 16-bit PCM (int16),
     "ulaw" 8-bit G.711 mu-law (uint8).  Rates: SUPPORTED_RATES.  `speed`: a real number in SPEED_RANGE, the pace of the
-    speech (1.25 is 25 % faster, same pitch; audio.TimeStretch, resolution 1/480).  Anything else raises ValueError on
-    construction."""
+    speech (1.25 is 25 % faster, same pitch; audio.TimeStretch, resolution 1/480).  `pitch`: semitones in PITCH_RANGE
+    (time-stretch, then rate conversion from 50*pitch_step Hz; formants move with it).  `volume`: dB in VOLUME_RANGE
+    through audio.Limiter, peaks held at -1 dBFS.  speed / (pitch_step/480) must lie in [0.5, 2] (hop in [240, 960]).
+    Anything else raises ValueError on construction."""
     sample_rate: int
     encoding: str = "f32"
     speed: float = 1.0
+    pitch: float = 0.0
+    volume: float = 0.0
 
     def __post_init__(self):
         try:
@@ -216,9 +228,21 @@ class AudioFormat:
             raise ValueError(f"sample_rate {self.sample_rate!r} is not supported; supported rates: {SUPPORTED_RATES}")
         if not isinstance(self.encoding, str) or self.encoding not in ENCODINGS:
             raise ValueError(f"encoding {self.encoding!r} is not supported; supported encodings: {ENCODINGS}")
-        sp = self.speed
-        if isinstance(sp, bool) or not isinstance(sp, numbers.Real) or not math.isfinite(float(sp)) \
-                or not SPEED_RANGE[0] <= float(sp) <= SPEED_RANGE[1]:
-            raise ValueError(f"speed {sp!r} is not a real number in [{SPEED_RANGE[0]}, {SPEED_RANGE[1]}]")
         object.__setattr__(self, "sample_rate", sr)
-        object.__setattr__(self, "speed", float(sp))
+        object.__setattr__(self, "speed", _real_in("speed", self.speed, *SPEED_RANGE))
+        object.__setattr__(self, "pitch", _real_in("pitch", self.pitch, *PITCH_RANGE))
+        object.__setattr__(self, "volume", _real_in("volume", self.volume, *VOLUME_RANGE))
+        if not 240 <= self.hop <= 960:
+            raise ValueError(f"speed {self.speed} at pitch {self.pitch} gives a time-stretch hop of {self.hop}: speed "
+                             f"divided by the pitch factor {self.pitch_step}/480 must lie in [0.5, 2]")
+
+    @property
+    def pitch_step(self) -> int:
+        """Lp = floor(480 * 2^(pitch/12) + 0.5), in [240, 960]: the pitch factor is Lp/480."""
+        return int(math.floor(480 * 2.0 ** (self.pitch / 12) + 0.5))
+
+    @property
+    def hop(self) -> int:
+        """The time-stretch's analysis hop Ha = floor(speed * 480 * (480/Lp) + 0.5) (floor(speed*480 + 0.5) at pitch 0);
+        the effective speed is Ha*Lp/480^2."""
+        return int(math.floor(self.speed * 480 * (480 / self.pitch_step) + 0.5))

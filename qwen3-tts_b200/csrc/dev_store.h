@@ -83,6 +83,16 @@ class DevStore {
     return 0;
   }
 
+  // free the tensor `name` (load) before the store ends, so the name may be loaded again.  The caller has drained every
+  // stream that may still read it.
+  int drop(const std::string& name) {
+    const auto it = tensors_.find(name);
+    if (it == tensors_.end()) return q3_set_err("%s: tensor %s is missing", engine_, name.c_str());
+    void* p = it->second.p;
+    tensors_.erase(it);
+    return release(p);
+  }
+
   // the tensor `name` of `numel` elements of T (float or bf16); null, with the error recorded, when it is missing or
   // has another element count or type
   template <class T>

@@ -64,10 +64,17 @@ extern "C" int q3_resample_open(int32_t rows, int32_t max_in, int32_t max_out, i
 
 extern "C" void q3_resample_close(q3_resampler* s) { delete s; }
 
+// a filter id in use: added and not dropped (a dropped id keeps a null taps pointer until it is reused)
+static bool filter_live(const q3_resampler* s, int id) {
+  return id >= 0 && id < (int)s->filters.size() && s->filters[id].taps != nullptr;
+}
+
 extern "C" int q3_resample_add_filter(q3_resampler* s, int32_t up, int32_t down, const float* taps_dev, int32_t ntaps,
                                       int32_t* id_out) {
   Q3_REQUIRE(s && taps_dev && id_out, "null argument");
-  Q3_REQUIRE((int)s->filters.size() < kMaxFilters, "a resampler holds at most %d filters", kMaxFilters);
+  int id = 0;
+  while (id < (int)s->filters.size() && s->filters[id].taps) ++id;   // the lowest free id, reused after a drop
+  Q3_REQUIRE(id < kMaxFilters, "a resampler holds at most %d filters", kMaxFilters);
   Q3_REQUIRE(up >= 1 && down >= 1, "up %d and down %d must be positive", up, down);
   Q3_REQUIRE(ntaps >= 1 && ntaps % 2 == 1, "a filter has an odd number of taps, got %d", ntaps);
   const int hl = ntaps / 2;
@@ -78,12 +85,24 @@ extern "C" int q3_resample_add_filter(q3_resampler* s, int32_t up, int32_t down,
              worst, s->max_in, s->max_out);
   Q3_CUDA(cudaSetDevice(s->device));
   const int64_t shape[1] = {ntaps};
-  const std::string name = "filter." + std::to_string(s->filters.size());
+  const std::string name = "filter." + std::to_string(id);
   if (s->store.load(name, taps_dev, shape, 1, DT_F32)) return 1;
   const float* p = s->store.need<float>(name, ntaps);
   if (!p) return 1;
-  *id_out = (int32_t)s->filters.size();
-  s->filters.push_back(Filter{p, up, down, hl});
+  if (id == (int)s->filters.size()) s->filters.push_back(Filter{});
+  s->filters[id] = Filter{p, up, down, hl};
+  *id_out = id;
+  return 0;
+}
+
+extern "C" int q3_resample_drop_filter(q3_resampler* s, int32_t id) {
+  Q3_REQUIRE(s, "null resampler");
+  Q3_REQUIRE(filter_live(s, id), "filter %d not added", id);
+  for (int r = 0; r < s->rows; ++r) Q3_REQUIRE(s->fid[r] != id, "filter %d is in use by row %d", id, r);
+  Q3_CUDA(cudaSetDevice(s->device));
+  Q3_CUDA(cudaDeviceSynchronize());   // launches queued on any stream may still read its taps
+  if (s->store.drop("filter." + std::to_string(id))) return 1;
+  s->filters[id] = Filter{};
   return 0;
 }
 
@@ -103,8 +122,7 @@ extern "C" int q3_resample_reset_rows(q3_resampler* s, int32_t n, const int32_t*
   if (check_rows(s, n, rows_host, "reset")) return 1;
   Q3_REQUIRE(n == 0 || (filters_host && encodings_host), "null argument");
   for (int i = 0; i < n; ++i) {
-    Q3_REQUIRE(filters_host[i] >= 0 && filters_host[i] < (int)s->filters.size(), "row %d: filter %d not added",
-               rows_host[i], filters_host[i]);
+    Q3_REQUIRE(filter_live(s, filters_host[i]), "row %d: filter %d not added", rows_host[i], filters_host[i]);
     Q3_REQUIRE(encodings_host[i] >= Q3_RESAMPLE_F32 && encodings_host[i] <= Q3_RESAMPLE_ULAW, "row %d: encoding %d unknown",
                rows_host[i], encodings_host[i]);
   }
@@ -113,6 +131,16 @@ extern "C" int q3_resample_reset_rows(q3_resampler* s, int32_t n, const int32_t*
     const int r = rows_host[i];
     s->fid[r] = filters_host[i]; s->enc[r] = encodings_host[i];
     s->n_in[r] = 0;
+  }
+  return 0;
+}
+
+extern "C" int q3_resample_release_rows(q3_resampler* s, int32_t n, const int32_t* rows_host) {
+  Q3_REQUIRE(s, "null resampler");
+  if (check_rows(s, n, rows_host, "release")) return 1;
+  for (int i = 0; i < n; ++i) {
+    s->fid[rows_host[i]] = -1;
+    s->n_in[rows_host[i]] = 0;
   }
   return 0;
 }
@@ -199,7 +227,7 @@ extern "C" int q3_resample_load_rows(q3_resampler* s, int32_t n, const int32_t* 
     Q3_CUDA(cudaMemcpyAsync(&rec[i], (const RowRecord*)src_dev + i, offsetof(RowRecord, hist), cudaMemcpyDeviceToHost, st));
   Q3_CUDA(cudaStreamSynchronize(st));
   for (int i = 0; i < n; ++i) {
-    Q3_REQUIRE(rec[i].fid >= 0 && rec[i].fid < (int)s->filters.size() && rec[i].enc >= Q3_RESAMPLE_F32 &&
+    Q3_REQUIRE(filter_live(s, rec[i].fid) && rec[i].enc >= Q3_RESAMPLE_F32 &&
                    rec[i].enc <= Q3_RESAMPLE_ULAW && rec[i].n_in >= 0,
                "load row %d: record %d is not a saved row of this resampler", rows_host[i], i);
   }

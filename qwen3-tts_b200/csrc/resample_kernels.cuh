@@ -4,7 +4,7 @@
 #include "../../include/qwen3tts_b200.h"
 
 constexpr int kHist = Q3_RESAMPLE_HIST;
-constexpr int kMaxFilters = 16;
+constexpr int kMaxFilters = 64;   // the FilterTable is a by-value kernel parameter (1.5 KB)
 constexpr int kThreads = 256;
 
 struct Filter {
@@ -14,6 +14,7 @@ struct Filter {
 struct FilterTable {
   Filter f[kMaxFilters];
 };
+static_assert(sizeof(FilterTable) <= 2048, "the filter table must stay well under the 4 KB kernel parameter limit");
 
 // one row of one launch (or of a save / load)
 struct RowJob {

@@ -79,6 +79,17 @@ seed or bank copy (it stretches the generated part only), saved on park, loaded 
 request's concatenated chunks equal Resampler.oneshot(TimeStretch.oneshot(w, speed), 24000, its rate and encoding), w
 its whole waveform (tests/test_gpu_scheduler_speed.py).  A session where no request has another speed makes the same
 calls as before.
+
+Pitch and volume (`AudioFormat(pitch=, volume=)`): a request whose pitch step Lp (AudioFormat.pitch_step) is not 480
+has its time-stretch row at hop AudioFormat.hop (skipped when that hop is 480) and a resampler row converting from
+50*Lp Hz to its rate and encoding, even at 24 kHz float32.  A request with a volume other than 0 dB has a row of one
+audio.Limiter of `n_slots` rows, opened when the first such request is admitted; it runs after the time-stretch and
+before the resampler, and is reset at admission after the time-stretch's reset, saved on park, loaded on resume and
+dropped on cancel.  A finishing request's stretch tail goes through the limiter's end into the resampler's end in the
+same step.  A request's concatenated chunks equal
+    Resampler.oneshot(Limiter.oneshot(TimeStretch.oneshot(w, speed, pitch), volume), 50*Lp, AudioFormat(rate, encoding))
+bit for bit, each stage skipped when its request does not use it (tests/test_gpu_scheduler_pitch_volume.py).  A session
+where every request has pitch 0 and volume 0 makes the same calls as before.
 """
 from collections import deque
 from dataclasses import dataclass, field
@@ -114,14 +125,18 @@ class _Request:
     codes: Optional[torch.Tensor] = None
     overlay: Optional[torch.Tensor] = None   # prompt rows still waiting for a text row each (None once complete)
     fmt: Optional[AudioFormat] = None        # the client's rate and encoding; None: the codec's own (no resampler row)
-    res_state: Optional[torch.Tensor] = None   # while parked: its resampler row's saved state
+    res_state: Optional[audio.ResamplerState] = None   # while parked: its resampler row's saved state
     speed: Optional[float] = None            # the client's speaking rate; None: as generated (no time-stretch row)
     st_state: Optional[torch.Tensor] = None    # while parked: its time-stretch row's saved state
+    pitch: float = 0.0                       # its pitch in semitones; 0 when its pitch step is 480 (no pitch shift)
+    in_rate: int = audio.CODEC_RATE          # the rate its resampler row converts from: 50 * its pitch step
+    volume: Optional[float] = None           # its volume in dB; None: 0 dB (no limiter row)
+    lim_state: Optional[torch.Tensor] = None   # while parked: its limiter row's saved state
 
     @property
     def shaped(self) -> bool:
-        """Its audio goes through a time-stretch or a resampler row."""
-        return self.fmt is not None or self.speed is not None
+        """Its audio goes through a time-stretch, a limiter or a resampler row."""
+        return self.fmt is not None or self.speed is not None or self.volume is not None
 
 
 class ContinuousBatcher:
@@ -163,22 +178,23 @@ class ContinuousBatcher:
         self.audio_format = audio_format
         self.resampler: Optional[audio.Resampler] = None   # opened when the first request with a format is admitted
         self.stretcher: Optional[audio.TimeStretch] = None   # opened when the first request with a speed is admitted
+        self.limiter: Optional[audio.Limiter] = None   # opened when the first request with a volume is admitted
 
     def _check_format(self, fmt: Optional[AudioFormat]) -> Optional[AudioFormat]:
-        """The rate and encoding a request's resampler row converts to: None for the codec's own 24 kHz float32 (no
-        resampling)."""
+        """The rate and encoding a request's resampler row converts to: None for the codec's own 24 kHz float32 without
+        a pitch shift (no resampling)."""
         if fmt is None:
             return None
         audio.check_format(fmt)
         if self.codec is None:
             raise ValueError("an audio format needs a ContinuousBatcher built with a codec")
-        fmt = AudioFormat(fmt.sample_rate, fmt.encoding)
-        return None if fmt == AudioFormat(audio.CODEC_RATE) else fmt
+        out = AudioFormat(fmt.sample_rate, fmt.encoding)
+        return None if out == AudioFormat(audio.CODEC_RATE) and fmt.pitch_step == 480 else out
 
     @staticmethod
     def _speed(fmt: Optional[AudioFormat]) -> Optional[float]:
         """The speed a request's time-stretch row runs at: None when its hop is 480 (no stretch)."""
-        if fmt is None or audio.TimeStretch.hop(fmt.speed) == audio.TimeStretch.HS:
+        if fmt is None or fmt.hop == audio.TimeStretch.HS:
             return None
         return fmt.speed
 
@@ -204,6 +220,9 @@ class ContinuousBatcher:
         ValueError here, never in a later step()."""
         src = audio_format if audio_format is not None else self.audio_format
         fmt, speed = self._check_format(src), self._speed(src)
+        pitched = src is not None and src.pitch_step != 480
+        shape = dict(pitch=src.pitch if pitched else 0.0, in_rate=50 * src.pitch_step if pitched else audio.CODEC_RATE,
+                     volume=src.volume if src is not None and src.volume != 0 else None)
         H = self.eng.cfg.talker.hidden_size
         L_ref, P = 0, 0
         if overlay is not None:
@@ -255,7 +274,7 @@ class ContinuousBatcher:
         if self.codec is not None:
             horizon = min(horizon, self.codec.max_frames - L_ref)  # a codec row's position may not pass its RoPE table
         r = _Request(rid, inputs_embeds, tr, horizon, sampling, ref_codes, voice, text_open=bool(text_open),
-                     overlay=overlay if K else None, fmt=fmt, speed=speed)
+                     overlay=overlay if K else None, fmt=fmt, speed=speed, **shape)
         if r.overlay is not None:
             r.trailing = self._fill(r, tr.reshape(-1, H))
         r.n_text = int(r.trailing.reshape(-1, H).shape[0])
@@ -343,11 +362,11 @@ class ContinuousBatcher:
                 self._cancelled.add(rid)
                 return True
         r = self.parked.pop(rid, None)
-        if r is not None:    # its record, its codec bank row and its resampler and time-stretch states are freed
+        if r is not None:    # its record, its codec bank row and its resampler, time-stretch and limiter states are freed
             self.eng.discard(r.record)
             if r.bank is not None:
                 self.codec.bank_release(*r.bank)
-            r.res_state = r.st_state = None
+            r.res_state = r.st_state = r.lim_state = None
             self._cancelled.add(rid)
             return True
         return False
@@ -388,6 +407,8 @@ class ContinuousBatcher:
             r.res_state = self.resampler.save([slot])
         if r.speed is not None:
             r.st_state = self.stretcher.save([slot])
+        if r.volume is not None:
+            r.lim_state = self.limiter.save([slot])
         r.trailing = r.trailing.reshape(-1, self.eng.cfg.talker.hidden_size)[:0]   # the record holds the text so far
         r.slot = -1
         self.parked[r.rid] = r
@@ -413,6 +434,9 @@ class ContinuousBatcher:
         if r.st_state is not None:
             self.stretcher.load([slot], r.st_state)
             r.st_state = None
+        if r.lim_state is not None:
+            self.limiter.load([slot], r.lim_state)
+            r.lim_state = None
         if r.trailing.shape[0] > 0:
             self.eng.append_trailing(slot, r.trailing)
             r.trailing = r.trailing[:0]
@@ -499,14 +523,18 @@ class ContinuousBatcher:
                 for bank in sorted({r.voice.bank[0] for r in banked}):   # one copy per bank, no reference decode
                     rs = [r for r in banked if r.voice.bank[0] == bank]
                     self.cstream.copy_from(self.codec.bank_stream(bank), [r.voice.bank[1] for r in rs], [r.slot for r in rs])
-                for fmt in dict.fromkeys(r.fmt for r in batch if r.fmt is not None):   # one reset per format
+                for key in dict.fromkeys((r.in_rate, r.fmt) for r in batch if r.fmt is not None):   # one reset per pair
                     if self.resampler is None:
                         self.resampler = audio.Resampler(self.eng.device, self.n_slots, self.packet * self.codec.total_upsample)
-                    self.resampler.reset([r.slot for r in batch if r.fmt == fmt], audio.CODEC_RATE, fmt)
-                for speed in dict.fromkeys(r.speed for r in batch if r.speed is not None):   # one reset per speed
+                    self.resampler.reset([r.slot for r in batch if (r.in_rate, r.fmt) == key], *key)
+                for key in dict.fromkeys((r.speed, r.pitch) for r in batch if r.speed is not None):   # one per hop
                     if self.stretcher is None:
                         self.stretcher = audio.TimeStretch(self.eng.device, self.n_slots, self.packet * self.codec.total_upsample)
-                    self.stretcher.reset([r.slot for r in batch if r.speed == speed], speed)
+                    self.stretcher.reset([r.slot for r in batch if (r.speed, r.pitch) == key], *key[:1 + (key[1] != 0)])
+                for volume in dict.fromkeys(r.volume for r in batch if r.volume is not None):   # one reset per volume
+                    if self.limiter is None:
+                        self.limiter = audio.Limiter(self.eng.device, self.n_slots, self.packet * self.codec.total_upsample)
+                    self.limiter.reset([r.slot for r in batch if r.volume == volume], volume)
         if not batch and not self._runnable():
             return {}, []   # every running row is open and waiting for text: launch nothing
         n = min([self.packet] + [r.max_frames - r.emitted for r in self.running.values()])
@@ -553,9 +581,11 @@ class ContinuousBatcher:
         return {r.rid: wav[slot, :k * up] for slot, (r, _, k) in new.items() if k > 0}
 
     def _push_formats(self, new, m: int, ending: List[int]) -> Dict[int, np.ndarray]:
-        """_push_audio of a step in which some request has a format: the codec push stays on the device, the default
-        slots' audio comes back as before, the others' through the time-stretch (requests with a speed), then the
-        resampler (requests with a rate or encoding other than 24 kHz float32)."""
+        """_push_audio of a step in which some request is shaped: the codec push stays on the device, the default
+        slots' audio comes back as before, the others' goes through the chain of stages their requests use, in order:
+        the time-stretch (a speed or pitch), the limiter (a volume), the resampler (a pitch, or a rate or encoding other
+        than 24 kHz float32).  One launch per stage serves every slot that uses it; a request that finished in the step
+        ends its row in each of its stages, and each stage's tail goes on into the next stage's end."""
         up = self.codec.total_upsample
         out: Dict[int, np.ndarray] = {}
         wav = None
@@ -572,44 +602,33 @@ class ContinuousBatcher:
                 host = wav[plain].cpu().numpy()
                 for i, slot in enumerate(plain):
                     out[new[slot][0].rid] = host[i, :new[slot][2] * up]
-        x, res = wav, {slot: k * up for slot, (r, _, k) in new.items() if r.fmt is not None and k > 0}
-        resample = True
-        if any(r.speed is not None for r, _, _ in new.values()):
-            x, res = self._push_speeds(new, wav, x, res, ending, out)
-            resample = any(new[slot][0].fmt is not None for slot in list(res) + ending)
-        if resample:
-            got = self.resampler.push_rows(x, res, [slot for slot in ending if new[slot][0].fmt is not None])
+        stages = [(self.stretcher, lambda r: r.speed is not None), (self.limiter, lambda r: r.volume is not None),
+                  (self.resampler, lambda r: r.fmt is not None)]
+        chain = [(obj, uses) for obj, uses in stages if any(uses(r) for r, _, _ in new.values())]
+        x, cnt = wav, {slot: k * up for slot, (r, _, k) in new.items() if r.shaped and k > 0}   # each slot's input
+        for i, (obj, uses) in enumerate(chain):
+            def later(slot, rest=chain[i + 1:]):
+                return any(u(new[slot][0]) for _, u in rest)
+            counts = {slot: c for slot, c in cnt.items() if uses(new[slot][0])}
+            end = [slot for slot in ending if uses(new[slot][0])]
+            if i > 0 and not counts and not end:
+                continue
+            onward = [slot for slot in sorted(set(counts) | set(end)) if later(slot)]
+            got = obj.push_rows(x if counts else None, counts, end, host=not onward)
             for slot, y in got.items():
-                if y.shape[0] or slot in ending:   # the filter's delay can hold a short push back entirely
-                    out[new[slot][0].rid] = y
+                if not later(slot) and (y.shape[0] or slot in ending):   # a stage's delay can hold a short push back
+                    out[new[slot][0].rid] = y if not onward else y.cpu().numpy()
+            cnt = {slot: c for slot, c in cnt.items() if slot not in counts}
+            if not onward:
+                continue
+            cnt.update({slot: int(got[slot].shape[0]) for slot in onward})
+            L = max(cnt.values(), default=0)
+            nx = torch.zeros(self.n_slots, L, dtype=torch.float32, device=self.eng.device) if L else None
+            for slot, c in cnt.items():
+                if c:
+                    nx[slot, :c] = got[slot] if slot in onward else x[slot, :c]
+            x = nx
         return out
-
-    def _push_speeds(self, new, wav, x, res, ending: List[int], out):
-        """The time-stretch launch of _push_formats: slots of requests with a speed take their new samples, and those
-        that finished in the step end their clips (their tails come even without new frames).  A stretched request
-        without a resampler row gets its output in `out`; for the others, returns the resampler's (input, counts):
-        the stretched output in their rows, each finished one's tail passed into its resampler end."""
-        up = self.codec.total_upsample
-        st = {slot: k * up for slot, (r, _, k) in new.items() if r.speed is not None and k > 0}
-        st_end = [slot for slot in ending if new[slot][0].speed is not None]
-        both = any(new[slot][0].fmt is not None for slot in set(st) | set(st_end))
-        got = self.stretcher.push_rows(wav if st else None, st, st_end, host=not both)
-        for slot, y in got.items():
-            if new[slot][0].fmt is None and (y.shape[0] or slot in ending):   # frames wait for 1200 samples
-                out[new[slot][0].rid] = y if not both else y.cpu().numpy()
-        if not both:
-            return x, res
-        chained = {slot: y for slot, y in got.items() if new[slot][0].fmt is not None}
-        res = {slot: c for slot, c in res.items() if slot not in chained}
-        res.update({slot: int(y.shape[0]) for slot, y in chained.items()})
-        L = max(res.values(), default=0)
-        if L == 0:
-            return None, res
-        x = torch.zeros(self.n_slots, L, dtype=torch.float32, device=self.eng.device)
-        for slot, c in res.items():
-            if c:
-                x[slot, :c] = chained[slot] if slot in chained else wav[slot, :c]
-        return x, res
 
     def run(self) -> Dict[int, torch.Tensor]:
         """Drain the queue; returns {request id: (N_i, G) codes}.  Requests with open text must be closed first (or

@@ -3,9 +3,12 @@ launches) and the batcher's _push_audio time per step (host clock ending in a sy
 default codec and 4-frame packets, for all rows in the default format, all rows 8 kHz mu-law and all rows 48 kHz
 float32.  With --speed, the same for every row at each of the given speaking rates (24 kHz float32, so only the
 time-stretch runs), and the time-stretch step (CUDA events around q3_stretch_step_rows calls of one packet per row)
-instead of the resampler's.  Prints one JSON line, with the card's name and power limit read in the same run.
+instead of the resampler's.  With --pitch, every row at each of the given pitches (24 kHz float32: the time-stretch
+and the pitched resampler run), timing the pitched resampler step; with --volume, every row at each of the given
+volumes (only the limiter runs), timing the limiter step.  Prints one JSON line, with the card's name and power limit
+read in the same run.
 
-    python tools/format_probe.py [--steps 60] [--warmup 10] [--speed 0.5 1.25 2.0]
+    python tools/format_probe.py [--steps 60] [--warmup 10] [--speed 0.5 1.25 2.0] [--pitch -7 3] [--volume 6 -6]
 """
 import argparse
 import ctypes as C
@@ -50,6 +53,8 @@ def main():
     ap.add_argument("--steps", type=int, default=60)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--speed", type=float, nargs="*", default=None)
+    ap.add_argument("--pitch", type=float, nargs="*", default=None)
+    ap.add_argument("--volume", type=float, nargs="*", default=None)
     a = ap.parse_args()
     import torch
     import qwen3_tts_b200 as q
@@ -63,8 +68,10 @@ def main():
     dec = CodecDecoder(ccfg, synthetic.random_codec_weights(ccfg, device="cpu", seed=0), device=dev, max_frames=1024)
     P, up = 4, dec.total_upsample
     formats = {"default": None, "8k_ulaw": q.AudioFormat(8000, "ulaw"), "48k_f32": q.AudioFormat(48000, "f32")}
-    if a.speed:
-        formats = {"default": None, **{f"speed_{sp}": q.AudioFormat(24000, speed=sp) for sp in a.speed}}
+    if a.speed or a.pitch or a.volume:
+        formats = {"default": None, **{f"speed_{sp}": q.AudioFormat(24000, speed=sp) for sp in a.speed or ()},
+                   **{f"pitch_{p}": q.AudioFormat(24000, pitch=p) for p in a.pitch or ()},
+                   **{f"volume_{v}": q.AudioFormat(24000, volume=v) for v in a.volume or ()}}
     results = []
     g = torch.Generator().manual_seed(0)
     for S in (8, 32):
@@ -72,17 +79,24 @@ def main():
             cb = ContinuousBatcher(_Engine(dev), torch.zeros(8), q.SamplingParams(max_new_tokens=2048), n_slots=S,
                                    packet_frames=P, codec=dec)
             cb.codes.copy_(torch.randint(0, ccfg.codebook_size, cb.codes.shape, generator=g).to(cb.codes))
-            reqs = [_Request(s, None, None, 2000, fmt=cb._check_format(fmt), speed=cb._speed(fmt)) for s in range(S)]
+            pitched = fmt is not None and fmt.pitch_step != 480
+            shape = dict(pitch=fmt.pitch if pitched else 0.0, in_rate=50 * fmt.pitch_step if pitched else 24000,
+                         volume=fmt.volume if fmt is not None and fmt.volume != 0 else None)
+            reqs = [_Request(s, None, None, 2000, fmt=cb._check_format(fmt), speed=cb._speed(fmt), **shape)
+                    for s in range(S)]
             for s, r in enumerate(reqs):
                 r.slot = s
                 cb.running[s] = r
             cb.cstream.reset()
             if reqs[0].fmt is not None:
                 cb.resampler = audio.Resampler(dev, S, P * up)
-                cb.resampler.reset(range(S), audio.CODEC_RATE, reqs[0].fmt)
+                cb.resampler.reset(range(S), reqs[0].in_rate, reqs[0].fmt)
             if reqs[0].speed is not None:
                 cb.stretcher = audio.TimeStretch(dev, S, P * up)
-                cb.stretcher.reset(range(S), reqs[0].speed)
+                cb.stretcher.reset(range(S), reqs[0].speed, reqs[0].pitch)
+            if reqs[0].volume is not None:
+                cb.limiter = audio.Limiter(dev, S, P * up)
+                cb.limiter.reset(range(S), reqs[0].volume)
             times = []
             for it in range(a.warmup + a.steps):
                 new = {s: (r, it * P, P) for s, r in enumerate(reqs)}
@@ -94,9 +108,13 @@ def main():
                     times.append(time.perf_counter() - t0)
             row = {"slots": S, "format": name, "push_audio_ms_mean": 1e3 * sum(times) / len(times),
                    "push_audio_ms_min": 1e3 * min(times)}
-            if fmt is not None:    # one resampler or time-stretch step (its job upload and kernel) of one packet per row
-                res = cb.stretcher if reqs[0].speed is not None else cb.resampler
-                fn = res.lib.q3_stretch_step_rows if reqs[0].speed is not None else res.lib.q3_resample_step_rows
+            if fmt is not None:    # one step of the timed stage (its job upload and kernel) of one packet per row
+                r0 = reqs[0]
+                stage = "limit" if r0.volume is not None else "resample" if r0.in_rate != 24000 or r0.speed is None \
+                    else "stretch"
+                res = {"limit": cb.limiter, "resample": cb.resampler, "stretch": cb.stretcher}[stage]
+                fn = getattr(res.lib, {"limit": "q3_limit_step_rows", "resample": "q3_resample_step_rows",
+                                       "stretch": "q3_stretch_step_rows"}[stage])
                 x = torch.rand(S, P * up, device=dev) * 2 - 1
                 cnt, end = (C.c_int32 * S)(*[P * up] * S), (C.c_int32 * S)()
                 nout = (C.c_int32 * S)()
@@ -111,9 +129,11 @@ def main():
                     step()
                 e1.record()
                 torch.cuda.synchronize()
-                row["stretch_step_us" if reqs[0].speed is not None else "resample_step_us"] = 1e3 * e0.elapsed_time(e1) / n
+                row[stage + "_step_us"] = 1e3 * e0.elapsed_time(e1) / n
                 row["outputs_per_row"] = int(nout[0])
-                res.close()
+                for obj in (cb.resampler, cb.stretcher, cb.limiter):
+                    if obj is not None:
+                        obj.close()
             cb.cstream.close()
             results.append(row)
     name, power = _card()
