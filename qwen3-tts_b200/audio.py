@@ -20,10 +20,10 @@ and a new pair needs its entry, when the least recently used pair no row uses is
 with its state, so load() adds a dropped filter again.
 
 Speaking rate: TimeStretch, a streaming per-row WSOLA time-stretch at 24 kHz (q3_stretch_*, csrc/stretch.cu, DESIGN
-§4.7), with the same streaming contract; the batcher runs it before the resampler.
+§4.7).  Volume: Limiter, a streaming per-row look-ahead limiter at 24 kHz (q3_limit_*, csrc/limit.cu, DESIGN §4.8).
 
-Volume: Limiter, a streaming per-row look-ahead limiter at 24 kHz (q3_limit_*, csrc/limit.cu, DESIGN §4.8), with the
-same streaming contract; the batcher runs it between the time-stretch and the resampler.
+The three are row stages (_RowStage) with one streaming contract, and stages(fmt) is the chain of them, in the order
+time-stretch, limiter, resampler, that turns the codec's audio into a client's AudioFormat.
 """
 import ctypes as C
 from dataclasses import dataclass
@@ -106,32 +106,49 @@ class ResamplerState:
     pairs: List[Tuple[int, int]]
 
 
-class Resampler:
-    """`rows` streaming resampler rows on `device`; a push gives each row at most `max_in` samples per launch (longer
-    pushes take several launches).  reset(rows, in_rate, fmt) starts new clips; push({row: samples}, end=rows) returns
-    {row: numpy array of the row's new output} in the row's encoding (float32, int16 or uint8); push_device keeps them
-    on the device; save(rows) / load(rows, state) move rows' state; release(rows) frees rows' filters for reuse;
-    oneshot(x, in_rate, fmt) converts a whole clip."""
+def _i32(xs) -> C.Array:
+    return (C.c_int32 * len(xs))(*xs)
+
+
+class _RowStage:
+    """`rows` streaming rows of one audio stage on `device` (the native q3_<PREFIX>_* entries), each with its own clip,
+    setting and counters.  A push gives each row at most `max_in` samples per launch (longer pushes take several
+    launches); output counts follow host formulas, so no push syncs.  reset(rows, ...) starts new clips;
+    push({row: samples}, end=rows) returns {row: numpy array of the row's new output}; push_device keeps them on the
+    device; save(rows) / load(rows, state) move rows' state; oneshot(x, ...) converts a whole clip with reset's
+    settings.  A clip pushed in pieces of any sizes and ended equals oneshot() of the whole clip bit for bit.
+    A subclass gives PREFIX, NAME, ROW_BYTES, reset and _max_out."""
+
+    PREFIX = ""                   # the native entries are q3_<PREFIX>_*
+    NAME = ""                     # the stage in error messages
+    ROW_BYTES = 0                 # one row's saved state
+    MAX_IN = 2 ** 31 - 1          # the largest max_in the native stage takes (oneshot pushes in launches of at most it)
 
     def __init__(self, device, rows: int, max_in: int):
         self.lib = _lib.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise RuntimeError("Resampler needs a CUDA device (no CPU fallback)")
+            raise RuntimeError(f"{type(self).__name__} needs a CUDA device (no CPU fallback)")
         self.rows, self.max_in = int(rows), int(max_in)
-        # capacity for the widest supported pair, so any pair can be added later
-        self.max_out = max(out_bound(self.max_in, *ratio(a, b)) for a in SUPPORTED_RATES for b in SUPPORTED_RATES)
+        self.max_out = self._max_out()
         h = C.c_void_p()
-        _lib.check(self.lib.q3_resample_open(self.rows, self.max_in, self.max_out, self.device.index or 0, C.byref(h)))
+        _lib.check(self._fn("open")(self.rows, self.max_in, self.max_out, self.device.index or 0, C.byref(h)))
         self.h = h
-        self._filters: Dict[Tuple[int, int], int] = {}     # pair -> filter id, least recently used first
-        self._pair: List[Optional[Tuple[int, int]]] = [None] * self.rows   # the pair each row uses
-        self._enc: List[Optional[str]] = [None] * self.rows
+        self._enc: List[Optional[str]] = [None] * self.rows   # each row's output encoding; None until reset or loaded
+        # every native step writes row r's outputs from byte 4*max_out*r on, in the row's encoding
         self._out = torch.empty(self.rows, 4 * self.max_out, dtype=torch.uint8, device=self.device)
+        self._views = {e: self._out.view(dt) for e, dt in _ENC_DTYPE.items()}   # the buffer in each encoding
+
+    def _fn(self, verb: str):
+        return getattr(self.lib, f"q3_{self.PREFIX}_{verb}")
+
+    def _max_out(self) -> int:
+        """The most outputs one push of max_in inputs plus its end can emit in any setting."""
+        raise NotImplementedError
 
     def close(self):
         if getattr(self, "h", None):
-            self.lib.q3_resample_close(self.h)
+            self._fn("close")(self.h)
             self.h = None
 
     def __del__(self):
@@ -142,8 +159,162 @@ class Resampler:
 
     def _stream(self):
         if not self.h:
-            raise RuntimeError("resampler is closed")
+            raise RuntimeError(f"{self.NAME} is closed")
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def _check_ready(self, rows):
+        for r in rows:
+            if self._enc[r] is None:
+                raise ValueError(f"row {r} was never reset")
+
+    def _reset(self, rows: List[int], *args, enc: str = "f32"):
+        """The native reset of the checked `rows` with the per-row arrays `args`; the rows then output `enc`."""
+        if rows:
+            _lib.check(self._fn("reset_rows")(self.h, len(rows), _i32(rows), *args))
+        for r in rows:
+            self._enc[r] = enc
+
+    def _run(self, x: Optional[torch.Tensor], cnt: List[int], end: List[int], host: bool, listed=()) -> Dict[int, object]:
+        """Row r takes x[r, :cnt[r]] and the rows in `end` end their clips, in launches of at most max_in samples per
+        row; a row ends in the launch that takes its last sample.  Each launch's outputs reach the host in one copy
+        (host=True) or stay on the device.  Returns {row: its new output} for rows with samples or an end and the rows
+        `listed`."""
+        if x is not None and (x.dim() != 2 or x.shape[0] != self.rows or x.dtype != torch.float32
+                              or x.device != self.device or x.stride(1) != 1 or max(cnt) > x.shape[1]):
+            raise ValueError(f"expected fp32 samples of shape ({self.rows}, L >= counts) on {self.device}")
+        if x is None and any(cnt):
+            raise ValueError("counts without samples")
+        touched = sorted(set(end) | set(listed) | {r for r in range(self.rows) if cnt[r]})
+        self._check_ready(touched)
+        enc = {r: self._enc[r] for r in touched}
+        st = self._stream()
+        parts: Dict[int, list] = {r: [] for r in touched}
+        for s0 in range(0, max(max(cnt), 1), self.max_in):
+            k = [min(max(c - s0, 0), self.max_in) for c in cnt]
+            e = [int(r in end and (s0 == 0 if cnt[r] == 0 else s0 < cnt[r] <= s0 + self.max_in)) for r in range(self.rows)]
+            nout = (C.c_int32 * self.rows)()
+            ptr = x.data_ptr() + 4 * s0 if x is not None and any(k) else None
+            _lib.check(self._fn("step_rows")(self.h, ptr, x.stride(0) if x is not None else 0, _i32(k), _i32(e),
+                                             self._out.data_ptr(), nout, st))
+            if host:
+                nb = {r: nout[r] * _WIDTH[enc[r]] for r in touched}
+                top = max(nb.values(), default=0)
+                buf = self._out[:, :top].cpu().numpy() if top else None
+                for r in touched:
+                    parts[r].append(buf[r, :nb[r]].view(_NP_DTYPE[enc[r]]) if nb[r] else None)
+            else:
+                for r in touched:
+                    parts[r].append(self._views[enc[r]][r, :nout[r]].clone() if nout[r] else None)
+        out = {}
+        for r in touched:
+            v = [p for p in parts[r] if p is not None]
+            if host:
+                out[r] = np.concatenate(v) if v else np.zeros(0, _NP_DTYPE[enc[r]])
+            else:
+                out[r] = torch.cat(v) if v else torch.zeros(0, dtype=_ENC_DTYPE[enc[r]], device=self.device)
+        return out
+
+    def push_rows(self, x: Optional[torch.Tensor], counts: Dict[int, int], end: Iterable[int] = (), host: bool = True):
+        """Row r takes x[r, :counts[r]] of x, fp32 (rows, L) on the device with contiguous rows (the layout the codec
+        stream returns), and the rows in `end` end their clips: one launch per max_in samples.  Returns {row: its new
+        output} (numpy arrays when `host`, else device tensors) for every row with samples or an end and every row of
+        `counts`."""
+        cnt = [0] * self.rows
+        for r, k in counts.items():
+            if int(k) < 0:
+                raise ValueError(f"row {r}: negative count {k}")
+            cnt[check_rows(r, self.rows)[0]] = int(k)
+        return self._run(x, cnt, check_rows(end, self.rows), host, listed=[int(r) for r in counts])
+
+    def _pack(self, chunks: Dict, end) -> Tuple[Optional[torch.Tensor], Dict[int, int], List[int]]:
+        chunks = check_chunks(chunks, self.rows)
+        end = check_rows(end, self.rows)
+        L = max([t.numel() for t in chunks.values()], default=0)
+        if L == 0:
+            return None, {r: 0 for r in chunks}, end
+        on_dev = any(t.device.type == "cuda" for t in chunks.values())
+        x = torch.zeros(self.rows, L, dtype=torch.float32, device=self.device if on_dev else "cpu")
+        for r, t in chunks.items():
+            x[r, : t.numel()] = t.to(x.device)
+        return x.to(self.device), {r: t.numel() for r, t in chunks.items()}, end
+
+    def push(self, chunks: Dict, end: Iterable[int] = ()) -> Dict[int, np.ndarray]:
+        """chunks {row: 1-D float samples at the row's input rate} (numpy or torch, any length); the rows in `end` end
+        their clips after their samples.  Returns {row: numpy array of its new output} for every row of chunks or
+        end, in the row's encoding.  One device-to-host copy per launch."""
+        x, counts, end = self._pack(chunks, end)
+        out = self.push_rows(x, counts, end, host=True)
+        return {r: out[r] for r in sorted(set(chunks) | set(end))}
+
+    def push_device(self, chunks: Dict, end: Iterable[int] = ()) -> Dict[int, torch.Tensor]:
+        """push() with the outputs left on the device (for an onward stage or the encoder stream)."""
+        x, counts, end = self._pack(chunks, end)
+        out = self.push_rows(x, counts, end, host=False)
+        return {r: out[r] for r in sorted(set(chunks) | set(end))}
+
+    def save(self, rows) -> torch.Tensor:
+        """The rows' state: the native records, a uint8 (len(rows), ROW_BYTES) device tensor."""
+        rows = check_rows(rows, self.rows)
+        self._check_ready(rows)
+        state = torch.empty(len(rows), self.ROW_BYTES, dtype=torch.uint8, device=self.device)
+        if rows:
+            _lib.check(self._fn("save_rows")(self.h, len(rows), _i32(rows), state.data_ptr(), self._stream()))
+        return state
+
+    def _fits(self, rec, n: int) -> bool:
+        return isinstance(rec, torch.Tensor) and rec.dtype == torch.uint8 and tuple(rec.shape) == (n, self.ROW_BYTES) \
+            and rec.device == self.device
+
+    def _records(self, state, n: int) -> torch.Tensor:
+        """The records to load from `state`, what save() of n rows returned; ValueError for anything else."""
+        if not self._fits(state, n):
+            raise ValueError(f"expected a saved state of shape ({n}, {self.ROW_BYTES}) on {self.device}")
+        return state.contiguous()
+
+    def load(self, rows, state):
+        """Rows `rows` continue the states save() returned, in order."""
+        rows = check_rows(rows, self.rows)
+        rec = self._records(state, len(rows))
+        if not rows:
+            return
+        _lib.check(self._fn("load_rows")(self.h, len(rows), _i32(rows), rec.data_ptr(), self._stream()))
+        self._restore(rows, rec, state)
+
+    def _restore(self, rows: List[int], rec: torch.Tensor, state):
+        """The host state of `rows`, just loaded from the records `rec` of `state`."""
+        for r in rows:
+            self._enc[r] = "f32"
+
+    def oneshot(self, x, *setting, **kw) -> np.ndarray:
+        """The whole clip x (1-D float samples) converted at once with reset's `setting`: the reference of the
+        streamed result."""
+        t = check_chunks({0: x}, 1)[0]
+        one = type(self)(self.device, 1, min(max(t.numel(), 1), self.MAX_IN))
+        try:
+            one.reset([0], *setting, **kw)
+            return one.push({0: t}, end=[0])[0]
+        finally:
+            one.close()
+
+
+class Resampler(_RowStage):
+    """`rows` streaming resampler rows on `device`; a push gives each row at most `max_in` samples per launch (longer
+    pushes take several launches).  reset(rows, in_rate, fmt) starts new clips; push({row: samples}, end=rows) returns
+    {row: numpy array of the row's new output} in the row's encoding (float32, int16 or uint8); push_device keeps them
+    on the device; save(rows) / load(rows, state) move rows' state; release(rows) frees rows' filters for reuse;
+    oneshot(x, in_rate, fmt) converts a whole clip."""
+
+    PREFIX, NAME = "resample", "resampler"
+    ROW_BYTES = ROW_BYTES
+
+    def __init__(self, device, rows: int, max_in: int):
+        super().__init__(device, rows, max_in)
+        self._filters: Dict[Tuple[int, int], int] = {}     # pair -> filter id, least recently used first
+        self._pair: List[Optional[Tuple[int, int]]] = [None] * self.rows   # the pair each row uses
+
+    def _max_out(self) -> int:
+        # capacity for the widest supported pair, so any pair can be added later
+        return max(out_bound(self.max_in, *ratio(a, b)) for a in SUPPORTED_RATES for b in SUPPORTED_RATES)
 
     def _filter(self, up: int, down: int, keep=()) -> int:
         """The id of the pair's filter, designed and added on its first use.  When the table is full, the least
@@ -172,150 +343,41 @@ class Resampler:
         pair = ratio(in_rate, fmt.sample_rate, pitched=True)
         fid = self._filter(*pair)
         n = len(rows)
-        if n == 0:
-            return
-        i32n = C.c_int32 * n
-        _lib.check(self.lib.q3_resample_reset_rows(self.h, n, i32n(*rows), i32n(*[fid] * n),
-                                                   i32n(*[_ENC_CODE[fmt.encoding]] * n)))
+        self._reset(rows, _i32([fid] * n), _i32([_ENC_CODE[fmt.encoding]] * n), enc=fmt.encoding)
         for r in rows:
-            self._enc[r], self._pair[r] = fmt.encoding, pair
+            self._pair[r] = pair
 
     def release(self, rows):
         """Rows `rows` no longer use their filters (which may then be dropped); they need a reset or a load before
         their next push."""
         rows = check_rows(rows, self.rows)
-        n = len(rows)
-        if n:
-            _lib.check(self.lib.q3_resample_release_rows(self.h, n, (C.c_int32 * n)(*rows)))
+        if rows:
+            _lib.check(self.lib.q3_resample_release_rows(self.h, len(rows), _i32(rows)))
         for r in rows:
             self._enc[r] = self._pair[r] = None
-
-    def _check_ready(self, rows):
-        for r in rows:
-            if self._enc[r] is None:
-                raise ValueError(f"row {r} was never reset")
-
-    def _run(self, x: Optional[torch.Tensor], cnt: List[int], end: List[int], host: bool, listed=()) -> Dict[int, object]:
-        """Row r takes x[r, :cnt[r]] and the rows in `end` end their clips, in launches of at most max_in samples per
-        row; a row ends in the launch that takes its last sample.  Each launch's outputs reach the host in one copy
-        (host=True) or stay on the device.  Returns {row: its new output} for rows with samples or an end and the rows
-        `listed`."""
-        if x is not None and (x.dim() != 2 or x.shape[0] != self.rows or x.dtype != torch.float32
-                              or x.device != self.device or x.stride(1) != 1 or max(cnt) > x.shape[1]):
-            raise ValueError(f"expected fp32 samples of shape ({self.rows}, L >= counts) on {self.device}")
-        if x is None and any(cnt):
-            raise ValueError("counts without samples")
-        touched = sorted(set(end) | set(listed) | {r for r in range(self.rows) if cnt[r]})
-        self._check_ready(touched)
-        st = self._stream()
-        parts: Dict[int, list] = {r: [] for r in touched}
-        for s0 in range(0, max(max(cnt), 1), self.max_in):
-            k = [min(max(c - s0, 0), self.max_in) for c in cnt]
-            e = [int(r in end and (s0 == 0 if cnt[r] == 0 else s0 < cnt[r] <= s0 + self.max_in)) for r in range(self.rows)]
-            nout = (C.c_int32 * self.rows)()
-            ptr = x.data_ptr() + 4 * s0 if x is not None and any(k) else None
-            _lib.check(self.lib.q3_resample_step_rows(self.h, ptr, x.stride(0) if x is not None else 0,
-                                                      (C.c_int32 * self.rows)(*k), (C.c_int32 * self.rows)(*e),
-                                                      self._out.data_ptr(), nout, st))
-            nb = {r: nout[r] * _WIDTH[self._enc[r]] for r in touched}
-            if host:
-                top = max(nb.values(), default=0)
-                buf = self._out[:, :top].cpu().numpy() if top else None
-                for r in touched:
-                    parts[r].append(buf[r, :nb[r]].view(_NP_DTYPE[self._enc[r]]) if nb[r] else None)
-            else:
-                for r in touched:
-                    parts[r].append(self._out[r, :nb[r]].clone().view(_ENC_DTYPE[self._enc[r]]) if nb[r] else None)
-        out = {}
-        for r in touched:
-            v = [p for p in parts[r] if p is not None]
-            if host:
-                out[r] = np.concatenate(v) if v else np.zeros(0, _NP_DTYPE[self._enc[r]])
-            else:
-                out[r] = torch.cat(v) if v else torch.zeros(0, dtype=_ENC_DTYPE[self._enc[r]], device=self.device)
-        return out
-
-    def push_rows(self, x: Optional[torch.Tensor], counts: Dict[int, int], end: Iterable[int] = (), host: bool = True):
-        """Row r takes x[r, :counts[r]] of x, fp32 (rows, L) on the device with contiguous rows (the layout the codec
-        stream returns), and the rows in `end` end their clips: one launch per max_in samples.  Returns {row: its new
-        output} (numpy arrays when `host`, else device tensors) for every row with samples or an end."""
-        cnt = [0] * self.rows
-        for r, k in counts.items():
-            if int(k) < 0:
-                raise ValueError(f"row {r}: negative count {k}")
-            cnt[check_rows(r, self.rows)[0]] = int(k)
-        return self._run(x, cnt, check_rows(end, self.rows), host, listed=[int(r) for r in counts])
-
-    def _pack(self, chunks: Dict, end) -> Tuple[Optional[torch.Tensor], Dict[int, int], List[int]]:
-        chunks = check_chunks(chunks, self.rows)
-        end = check_rows(end, self.rows)
-        L = max([t.numel() for t in chunks.values()], default=0)
-        if L == 0:
-            return None, {r: 0 for r in chunks}, end
-        on_dev = any(t.device.type == "cuda" for t in chunks.values())
-        x = torch.zeros(self.rows, L, dtype=torch.float32, device=self.device if on_dev else "cpu")
-        for r, t in chunks.items():
-            x[r, : t.numel()] = t.to(x.device)
-        return x.to(self.device), {r: t.numel() for r, t in chunks.items()}, end
-
-    def push(self, chunks: Dict, end: Iterable[int] = ()) -> Dict[int, np.ndarray]:
-        """chunks {row: 1-D float samples at the row's input rate} (numpy or torch, any length); the rows in `end` end
-        their clips after their samples.  Returns {row: numpy array of its new output} for every row of chunks or
-        end, float32, int16 or uint8 by the row's encoding.  One device-to-host copy per launch."""
-        x, counts, end = self._pack(chunks, end)
-        out = self.push_rows(x, counts, end, host=True)
-        return {r: out[r] for r in sorted(set(chunks) | set(end))}
-
-    def push_device(self, chunks: Dict, end: Iterable[int] = ()) -> Dict[int, torch.Tensor]:
-        """push() with the outputs left on the device (for the encoder stream)."""
-        x, counts, end = self._pack(chunks, end)
-        out = self.push_rows(x, counts, end, host=False)
-        return {r: out[r] for r in sorted(set(chunks) | set(end))}
 
     def save(self, rows) -> ResamplerState:
         """The rows' state: the native records (filter, encoding, inputs so far, history; a uint8 (len(rows),
         ROW_BYTES) device tensor) with each row's rate pair."""
         rows = check_rows(rows, self.rows)
-        self._check_ready(rows)
-        state = torch.empty(len(rows), ROW_BYTES, dtype=torch.uint8, device=self.device)
-        n = len(rows)
-        if n:
-            _lib.check(self.lib.q3_resample_save_rows(self.h, n, (C.c_int32 * n)(*rows), state.data_ptr(), self._stream()))
-        return ResamplerState(state, [self._pair[r] for r in rows])
+        return ResamplerState(super().save(rows), [self._pair[r] for r in rows])
 
-    def load(self, rows, state: ResamplerState):
-        """Rows `rows` continue the states save() returned (of this resampler), in order.  A pair whose filter was
-        dropped since is added again, and the records are loaded with each pair's current filter id."""
-        rows = check_rows(rows, self.rows)
-        rec = state.records if isinstance(state, ResamplerState) else None
-        if not isinstance(rec, torch.Tensor) or rec.dtype != torch.uint8 or tuple(rec.shape) != (len(rows), ROW_BYTES) \
-                or rec.device != self.device or len(state.pairs) != len(rows):
-            raise ValueError(f"expected a ResamplerState of {len(rows)} rows on {self.device}")
-        n = len(rows)
-        if n == 0:
-            return
+    def _records(self, state, n: int) -> torch.Tensor:
+        # a pair whose filter was dropped since the save is added again, and the records get each pair's current id
+        if not isinstance(state, ResamplerState) or not self._fits(state.records, n) or len(state.pairs) != n:
+            raise ValueError(f"expected a ResamplerState of {n} rows on {self.device}")
         fids = [self._filter(*p, keep=state.pairs) for p in state.pairs]
-        rec = rec.clone()
+        rec = state.records.clone()
         rec[:, 0:4] = torch.tensor(fids, dtype=torch.int32).view(torch.uint8).reshape(n, 4).to(self.device)
-        _lib.check(self.lib.q3_resample_load_rows(self.h, n, (C.c_int32 * n)(*rows), rec.data_ptr(), self._stream()))
-        inv = {v: k for k, v in _ENC_CODE.items()}
+        return rec
+
+    def _restore(self, rows, rec, state):
         codes = rec[:, 4:8].cpu().numpy().view(np.int32)[:, 0]   # the header's encoding (already read back natively)
         for r, c, p in zip(rows, codes, state.pairs):
-            self._enc[r], self._pair[r] = inv[int(c)], p
-
-    def oneshot(self, x, in_rate: int, fmt: AudioFormat) -> np.ndarray:
-        """The whole clip x (1-D float samples at in_rate, which reset() takes) converted at once: the reference of the
-        streamed result."""
-        t = check_chunks({0: x}, 1)[0]
-        one = Resampler(self.device, 1, max(t.numel(), 1))
-        try:
-            one.reset([0], in_rate, fmt)
-            return one.push({0: t}, end=[0])[0]
-        finally:
-            one.close()
+            self._enc[r], self._pair[r] = ENCODINGS[c], p
 
 
-class TimeStretch:
+class TimeStretch(_RowStage):
     """`rows` streaming WSOLA time-stretch rows at the codec's 24 kHz on `device` (q3_stretch_*, csrc/stretch.cu, DESIGN
     §4.7): the speaking rate of float32 audio changes, its pitch does not.  Frames of N = 960 samples, synthesis hop
     480, search tolerance 240, analysis hop Ha = hop(speed) in [240, 960], window sin^2(pi*n/960).  A clip of n samples
@@ -327,9 +389,9 @@ class TimeStretch:
 
     N, HS, DELTA = 960, 480, 240
     HIST = 2048                       # Q3_STRETCH_HIST: inputs a row keeps
+    PREFIX, NAME = "stretch", "time-stretch"
     ROW_BYTES = 10144                 # Q3_STRETCH_ROW_BYTES: one row's saved state
     MAX_IN = 32768                    # the largest max_in the native stretcher takes
-    _STEP = "q3_stretch_step_rows"
 
     @staticmethod
     def hop(speed, pitch=0.0) -> int:
@@ -360,157 +422,23 @@ class TimeStretch:
         return np.sin(np.pi * np.arange(960) / 960) ** 2
 
     def __init__(self, device, rows: int, max_in: int):
-        self.lib = _lib.load()
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise RuntimeError("TimeStretch needs a CUDA device (no CPU fallback)")
-        self.rows, self.max_in = int(rows), int(max_in)
-        if not 1 <= self.max_in <= self.MAX_IN:
-            raise ValueError(f"max_in {max_in} outside [1, {self.MAX_IN}]")
-        self.max_out = self.out_bound(self.max_in)
-        h = C.c_void_p()
-        _lib.check(self.lib.q3_stretch_open(self.rows, self.max_in, self.max_out, self.device.index or 0, C.byref(h)))
-        self.h = h
+        super().__init__(device, rows, max_in)
         w = torch.from_numpy(self.window()).to(self.device, torch.float32)
         _lib.check(self.lib.q3_stretch_set_window(self.h, w.data_ptr()))
-        self._ha: List[Optional[int]] = [None] * self.rows
-        self._out = torch.empty(self.rows, self.max_out, dtype=torch.float32, device=self.device)
 
-    def close(self):
-        if getattr(self, "h", None):
-            self.lib.q3_stretch_close(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _stream(self):
-        if not self.h:
-            raise RuntimeError("time-stretch is closed")
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+    def _max_out(self) -> int:
+        if not 1 <= self.max_in <= self.MAX_IN:
+            raise ValueError(f"max_in {self.max_in} outside [1, {self.MAX_IN}]")
+        return self.out_bound(self.max_in)
 
     def reset(self, rows, speed, pitch=0.0):
         """Start new clips in `rows` at `speed` and `pitch` (analysis hop hop(speed, pitch))."""
         rows = check_rows(rows, self.rows)
         ha = self.hop(speed, pitch)
-        n = len(rows)
-        if n == 0:
-            return
-        i32n = C.c_int32 * n
-        _lib.check(self.lib.q3_stretch_reset_rows(self.h, n, i32n(*rows), i32n(*[ha] * n)))
-        for r in rows:
-            self._ha[r] = ha
-
-    def _check_ready(self, rows):
-        for r in rows:
-            if self._ha[r] is None:
-                raise ValueError(f"row {r} was never reset")
-
-    def _run(self, x: Optional[torch.Tensor], cnt: List[int], end: List[int], host: bool, listed=()):
-        """Resampler._run for the stretch: launches of at most max_in samples per row, a row ends in the launch that
-        takes its last sample; returns {row: float32 output} for rows with samples or an end and the rows `listed`."""
-        if x is not None and (x.dim() != 2 or x.shape[0] != self.rows or x.dtype != torch.float32
-                              or x.device != self.device or x.stride(1) != 1 or max(cnt) > x.shape[1]):
-            raise ValueError(f"expected fp32 samples of shape ({self.rows}, L >= counts) on {self.device}")
-        if x is None and any(cnt):
-            raise ValueError("counts without samples")
-        touched = sorted(set(end) | set(listed) | {r for r in range(self.rows) if cnt[r]})
-        self._check_ready(touched)
-        st = self._stream()
-        parts: Dict[int, list] = {r: [] for r in touched}
-        for s0 in range(0, max(max(cnt), 1), self.max_in):
-            k = [min(max(c - s0, 0), self.max_in) for c in cnt]
-            e = [int(r in end and (s0 == 0 if cnt[r] == 0 else s0 < cnt[r] <= s0 + self.max_in)) for r in range(self.rows)]
-            nout = (C.c_int32 * self.rows)()
-            ptr = x.data_ptr() + 4 * s0 if x is not None and any(k) else None
-            _lib.check(getattr(self.lib, self._STEP)(self.h, ptr, x.stride(0) if x is not None else 0,
-                                                     (C.c_int32 * self.rows)(*k), (C.c_int32 * self.rows)(*e),
-                                                     self._out.data_ptr(), nout, st))
-            nb = {r: nout[r] for r in touched}
-            if host:
-                top = max(nb.values(), default=0)
-                buf = self._out[:, :top].cpu().numpy() if top else None
-                for r in touched:
-                    parts[r].append(buf[r, :nb[r]].copy() if nb[r] else None)
-            else:
-                for r in touched:
-                    parts[r].append(self._out[r, :nb[r]].clone() if nb[r] else None)
-        out = {}
-        for r in touched:
-            v = [p for p in parts[r] if p is not None]
-            if host:
-                out[r] = np.concatenate(v) if v else np.zeros(0, np.float32)
-            else:
-                out[r] = torch.cat(v) if v else torch.zeros(0, dtype=torch.float32, device=self.device)
-        return out
-
-    def push_rows(self, x: Optional[torch.Tensor], counts: Dict[int, int], end: Iterable[int] = (), host: bool = True):
-        """Row r takes x[r, :counts[r]] of x, fp32 (rows, L) on the device with contiguous rows, and the rows in `end`
-        end their clips: one launch per max_in samples.  Returns {row: its new float32 output} (numpy arrays when
-        `host`, else device tensors) for every row with samples or an end and every row of `counts`."""
-        cnt = [0] * self.rows
-        for r, k in counts.items():
-            if int(k) < 0:
-                raise ValueError(f"row {r}: negative count {k}")
-            cnt[check_rows(r, self.rows)[0]] = int(k)
-        return self._run(x, cnt, check_rows(end, self.rows), host, listed=[int(r) for r in counts])
-
-    _pack = Resampler._pack
-
-    def push(self, chunks: Dict, end: Iterable[int] = ()) -> Dict[int, np.ndarray]:
-        """chunks {row: 1-D float samples at 24 kHz} (numpy or torch, any length); the rows in `end` end their clips
-        after their samples.  Returns {row: float32 numpy array of its new output} for every row of chunks or end."""
-        x, counts, end = self._pack(chunks, end)
-        out = self.push_rows(x, counts, end, host=True)
-        return {r: out[r] for r in sorted(set(chunks) | set(end))}
-
-    def push_device(self, chunks: Dict, end: Iterable[int] = ()) -> Dict[int, torch.Tensor]:
-        """push() with the outputs left on the device."""
-        x, counts, end = self._pack(chunks, end)
-        out = self.push_rows(x, counts, end, host=False)
-        return {r: out[r] for r in sorted(set(chunks) | set(end))}
-
-    def save(self, rows) -> torch.Tensor:
-        """The rows' state (hop, inputs so far, frames done, last frame's position and tail, history): a uint8
-        (len(rows), ROW_BYTES) device tensor."""
-        rows = check_rows(rows, self.rows)
-        self._check_ready(rows)
-        state = torch.empty(len(rows), self.ROW_BYTES, dtype=torch.uint8, device=self.device)
-        n = len(rows)
-        if n:
-            _lib.check(self.lib.q3_stretch_save_rows(self.h, n, (C.c_int32 * n)(*rows), state.data_ptr(), self._stream()))
-        return state
-
-    def load(self, rows, state: torch.Tensor):
-        """Rows `rows` continue the states save() returned, in order."""
-        rows = check_rows(rows, self.rows)
-        if not isinstance(state, torch.Tensor) or state.dtype != torch.uint8 \
-                or tuple(state.shape) != (len(rows), self.ROW_BYTES) or state.device != self.device:
-            raise ValueError(f"expected a saved state of shape ({len(rows)}, {self.ROW_BYTES}) on {self.device}")
-        n = len(rows)
-        if n == 0:
-            return
-        state = state.contiguous()
-        _lib.check(self.lib.q3_stretch_load_rows(self.h, n, (C.c_int32 * n)(*rows), state.data_ptr(), self._stream()))
-        has = state[:, 0:4].cpu().numpy().view(np.int32)[:, 0]   # the header's hop (already read back natively)
-        for r, ha in zip(rows, has):
-            self._ha[r] = int(ha)
-
-    def oneshot(self, x, speed, pitch=0.0) -> np.ndarray:
-        """The whole clip x (1-D float samples at 24 kHz) stretched at once: the reference of the streamed result."""
-        t = check_chunks({0: x}, 1)[0]
-        one = TimeStretch(self.device, 1, min(max(t.numel(), 1), self.MAX_IN))
-        try:
-            one.reset([0], speed, pitch)
-            return one.push({0: t}, end=[0])[0]
-        finally:
-            one.close()
+        self._reset(rows, _i32([ha] * len(rows)))
 
 
-class Limiter:
+class Limiter(_RowStage):
     """`rows` streaming look-ahead limiter rows at the codec's 24 kHz on `device` (q3_limit_*, csrc/limit.cu, DESIGN
     §4.8): a gain of `volume` dB whose peaks are held at -1 dBFS, with 5 ms of look-ahead and a linear release of at most
     50 ms.  A clip of n samples gives n samples; after n samples without an end a row has emitted emitted(n) = max(0,
@@ -523,8 +451,8 @@ class Limiter:
     L, W = 120, 1200                  # look-ahead, release
     DELAY = L - 1
     HIST = 1536                       # Q3_LIMIT_HIST: inputs a row keeps (it reads W + 2L - 2 = 1438 back)
+    PREFIX, NAME = "limit", "limiter"
     ROW_BYTES = 6160                  # Q3_LIMIT_ROW_BYTES: one row's saved state
-    _STEP = "q3_limit_step_rows"
 
     @staticmethod
     def gain(volume) -> np.float32:
@@ -541,91 +469,38 @@ class Limiter:
         """Outputs of a whole clip of n inputs: n."""
         return n
 
-    def __init__(self, device, rows: int, max_in: int):
-        self.lib = _lib.load()
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise RuntimeError("Limiter needs a CUDA device (no CPU fallback)")
-        self.rows, self.max_in = int(rows), int(max_in)
-        self.max_out = self.max_in + self.DELAY
-        h = C.c_void_p()
-        _lib.check(self.lib.q3_limit_open(self.rows, self.max_in, self.max_out, self.device.index or 0, C.byref(h)))
-        self.h = h
-        self._gain: List[Optional[float]] = [None] * self.rows
-        self._out = torch.empty(self.rows, self.max_out, dtype=torch.float32, device=self.device)
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.lib.q3_limit_close(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _stream(self):
-        if not self.h:
-            raise RuntimeError("limiter is closed")
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+    def _max_out(self) -> int:
+        return self.max_in + self.DELAY
 
     def reset(self, rows, volume):
         """Start new clips in `rows` at `volume` dB (gain gain(volume))."""
         rows = check_rows(rows, self.rows)
         g = self.gain(volume)
-        n = len(rows)
-        if n == 0:
-            return
-        _lib.check(self.lib.q3_limit_reset_rows(self.h, n, (C.c_int32 * n)(*rows), (C.c_float * n)(*[g] * n)))
-        for r in rows:
-            self._gain[r] = float(g)
+        self._reset(rows, (C.c_float * len(rows))(*[g] * len(rows)))
 
-    def _check_ready(self, rows):
-        for r in rows:
-            if self._gain[r] is None:
-                raise ValueError(f"row {r} was never reset")
 
-    _run = TimeStretch._run
-    push_rows = TimeStretch.push_rows
-    _pack = Resampler._pack
-    push = TimeStretch.push
-    push_device = TimeStretch.push_device
+STAGES = ("TimeStretch", "Limiter", "Resampler")   # the stage classes above, in the order a stream runs them
 
-    def save(self, rows) -> torch.Tensor:
-        """The rows' state (gain, inputs so far, history): a uint8 (len(rows), ROW_BYTES) device tensor."""
-        rows = check_rows(rows, self.rows)
-        self._check_ready(rows)
-        state = torch.empty(len(rows), self.ROW_BYTES, dtype=torch.uint8, device=self.device)
-        n = len(rows)
-        if n:
-            _lib.check(self.lib.q3_limit_save_rows(self.h, n, (C.c_int32 * n)(*rows), state.data_ptr(), self._stream()))
-        return state
 
-    def load(self, rows, state: torch.Tensor):
-        """Rows `rows` continue the states save() returned, in order."""
-        rows = check_rows(rows, self.rows)
-        if not isinstance(state, torch.Tensor) or state.dtype != torch.uint8 \
-                or tuple(state.shape) != (len(rows), self.ROW_BYTES) or state.device != self.device:
-            raise ValueError(f"expected a saved state of shape ({len(rows)}, {self.ROW_BYTES}) on {self.device}")
-        n = len(rows)
-        if n == 0:
-            return
-        state = state.contiguous()
-        _lib.check(self.lib.q3_limit_load_rows(self.h, n, (C.c_int32 * n)(*rows), state.data_ptr(), self._stream()))
-        gains = state[:, 0:4].cpu().numpy().view(np.float32)[:, 0]   # the header's gain (already read back natively)
-        for r, g in zip(rows, gains):
-            self._gain[r] = float(g)
-
-    def oneshot(self, x, volume) -> np.ndarray:
-        """The whole clip x (1-D float samples at 24 kHz) limited at once: the reference of the streamed result."""
-        t = check_chunks({0: x}, 1)[0]
-        one = Limiter(self.device, 1, max(t.numel(), 1))
-        try:
-            one.reset([0], volume)
-            return one.push({0: t}, end=[0])[0]
-        finally:
-            one.close()
+def stages(fmt: Optional[AudioFormat]) -> Tuple[Tuple[str, tuple], ...]:
+    """The stages the codec's audio runs through to come out in `fmt`, in STAGES order, each as (its class's name in
+    this module, the arguments its reset takes after the rows): the time-stretch when the hop is not 480, (speed, pitch)
+    when the pitch step Lp is not 480 and (speed,) (pitch 0) when it is; the limiter (volume,) at a volume other than
+    0 dB; the resampler (50*Lp, AudioFormat(rate, encoding)) when Lp is not 480 or the rate or encoding is not 24 kHz
+    float32.  () for None (the codec's own audio)."""
+    if fmt is None:
+        return ()
+    fmt = check_format(fmt)
+    pitched = fmt.pitch_step != 480
+    out = AudioFormat(fmt.sample_rate, fmt.encoding)
+    chain = []
+    if fmt.hop != 480:
+        chain.append(("TimeStretch", (fmt.speed, fmt.pitch) if pitched else (fmt.speed,)))
+    if fmt.volume != 0:
+        chain.append(("Limiter", (fmt.volume,)))
+    if pitched or out != AudioFormat(CODEC_RATE):
+        chain.append(("Resampler", (50 * fmt.pitch_step, out)))
+    return tuple(chain)
 
 
 class ResampledEncoderStream:

@@ -18,6 +18,7 @@
 #include "common.cuh"
 #include "conv_f32.cuh"
 #include "dev_store.h"
+#include "row_state.h"
 #include "../../include/qwen3tts_b200.h"
 
 #include <algorithm>
@@ -493,20 +494,10 @@ static int enc_reset(q3_codec_enc_stream* s, int n, const int32_t* rows, cudaStr
   return 0;
 }
 
-static int enc_check_rows(const q3_codec_enc_stream* s, int n, const int32_t* rows, const char* what) {
-  Q3_REQUIRE(n >= 0 && n <= s->B, "%d rows to %s, the stream has %d", n, what, s->B);
-  Q3_REQUIRE(n == 0 || rows, "null argument");
-  for (int i = 0; i < n; ++i) {
-    Q3_REQUIRE(rows[i] >= 0 && rows[i] < s->B, "%s row %d out of range [0, %d)", what, rows[i], s->B);
-    for (int j = 0; j < i; ++j) Q3_REQUIRE(rows[i] != rows[j], "%s row %d listed twice", what, rows[i]);
-  }
-  return 0;
-}
-
 // forget the listed rows: their next packet starts a new clip at position 0; the other rows are untouched
 extern "C" int q3_codec_enc_stream_reset_rows(q3_codec_enc_stream* s, int32_t n, const int32_t* rows_host, void* stream_) {
   Q3_REQUIRE(s, "null stream");
-  if (enc_check_rows(s, n, rows_host, "reset")) return 1;
+  if (check_row_list(s->B, n, rows_host, "reset", "stream")) return 1;
   if (n == 0) return 0;
   Q3_CUDA(cudaSetDevice(s->e->cfg.device));
   return enc_reset(s, n, rows_host, (cudaStream_t)stream_);
@@ -518,7 +509,7 @@ extern "C" int q3_codec_enc_stream_reset_rows(q3_codec_enc_stream* s, int32_t n,
 extern "C" int q3_codec_enc_stream_finish_rows(q3_codec_enc_stream* s, int32_t n, const int32_t* rows_host, const int32_t* tail_host,
                                                const float* wav_dev, int32_t* codes_dev, void* stream_) {
   Q3_REQUIRE(s, "null stream");
-  if (enc_check_rows(s, n, rows_host, "finish")) return 1;
+  if (check_row_list(s->B, n, rows_host, "finish", "stream")) return 1;
   if (n == 0) return 0;
   Q3_REQUIRE(tail_host && wav_dev && codes_dev, "null argument");
   q3_codec_enc* e = s->e;

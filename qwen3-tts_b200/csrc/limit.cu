@@ -12,6 +12,7 @@
 // one-shot bit for bit.
 #include "common.cuh"
 #include "dev_store.h"
+#include "row_state.h"
 
 #include <algorithm>
 #include <cmath>
@@ -61,21 +62,11 @@ extern "C" int q3_limit_open(int32_t rows, int32_t max_in, int32_t max_out, int3
 
 extern "C" void q3_limit_close(q3_limiter* s) { delete s; }
 
-static int check_rows(const q3_limiter* s, int n, const int32_t* rows, const char* what) {
-  Q3_REQUIRE(n >= 0 && n <= s->rows, "%d rows to %s, the limiter has %d", n, what, s->rows);
-  Q3_REQUIRE(n == 0 || rows, "null argument");
-  for (int i = 0; i < n; ++i) {
-    Q3_REQUIRE(rows[i] >= 0 && rows[i] < s->rows, "%s row %d out of range [0, %d)", what, rows[i], s->rows);
-    for (int j = 0; j < i; ++j) Q3_REQUIRE(rows[i] != rows[j], "%s row %d listed twice", what, rows[i]);
-  }
-  return 0;
-}
-
 static bool gain_ok(float g) { return std::isfinite(g) && g > 0.f; }
 
 extern "C" int q3_limit_reset_rows(q3_limiter* s, int32_t n, const int32_t* rows_host, const float* gains_host) {
   Q3_REQUIRE(s, "null limiter");
-  if (check_rows(s, n, rows_host, "reset")) return 1;
+  if (check_row_list(s->rows, n, rows_host, "reset", "limiter")) return 1;
   Q3_REQUIRE(n == 0 || gains_host, "null argument");
   for (int i = 0; i < n; ++i)
     Q3_REQUIRE(gain_ok(gains_host[i]), "row %d: gain %g is not a positive finite number", rows_host[i], gains_host[i]);
@@ -147,7 +138,7 @@ static int move_rows(q3_limiter* s, int n, const int32_t* rows_host, void* rec, 
 
 extern "C" int q3_limit_save_rows(q3_limiter* s, int32_t n, const int32_t* rows_host, void* dst_dev, void* stream) {
   Q3_REQUIRE(s, "null limiter");
-  if (check_rows(s, n, rows_host, "save")) return 1;
+  if (check_row_list(s->rows, n, rows_host, "save", "limiter")) return 1;
   if (n == 0) return 0;
   Q3_REQUIRE(dst_dev, "null argument");
   for (int i = 0; i < n; ++i) Q3_REQUIRE(s->gain[rows_host[i]] > 0.f, "save row %d was never reset", rows_host[i]);
@@ -156,17 +147,13 @@ extern "C" int q3_limit_save_rows(q3_limiter* s, int32_t n, const int32_t* rows_
 
 extern "C" int q3_limit_load_rows(q3_limiter* s, int32_t n, const int32_t* rows_host, const void* src_dev, void* stream) {
   Q3_REQUIRE(s, "null limiter");
-  if (check_rows(s, n, rows_host, "load")) return 1;
+  if (check_row_list(s->rows, n, rows_host, "load", "limiter")) return 1;
   if (n == 0) return 0;
   Q3_REQUIRE(src_dev, "null argument");
   cudaStream_t st = (cudaStream_t)stream;
   Q3_CUDA(cudaSetDevice(s->device));
-  // the headers come back to the host: a row's count sizes its outputs at every later step without a sync
-  std::vector<LimitRecord> rec(n);
-  for (int i = 0; i < n; ++i)
-    Q3_CUDA(cudaMemcpyAsync(&rec[i], (const LimitRecord*)src_dev + i, offsetof(LimitRecord, hist), cudaMemcpyDeviceToHost,
-                            st));
-  Q3_CUDA(cudaStreamSynchronize(st));
+  std::vector<LimitRecord> rec;
+  if (read_headers(rec, src_dev, n, offsetof(LimitRecord, hist), st)) return 1;
   for (int i = 0; i < n; ++i)
     Q3_REQUIRE(gain_ok(rec[i].gain) && rec[i].n_in >= 0, "load row %d: record %d is not a saved row of a limiter",
                rows_host[i], i);

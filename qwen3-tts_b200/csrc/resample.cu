@@ -13,6 +13,7 @@
 // bit.
 #include "common.cuh"
 #include "dev_store.h"
+#include "row_state.h"
 
 #include <algorithm>
 #include <cstddef>
@@ -106,20 +107,10 @@ extern "C" int q3_resample_drop_filter(q3_resampler* s, int32_t id) {
   return 0;
 }
 
-static int check_rows(const q3_resampler* s, int n, const int32_t* rows, const char* what) {
-  Q3_REQUIRE(n >= 0 && n <= s->rows, "%d rows to %s, the resampler has %d", n, what, s->rows);
-  Q3_REQUIRE(n == 0 || rows, "null argument");
-  for (int i = 0; i < n; ++i) {
-    Q3_REQUIRE(rows[i] >= 0 && rows[i] < s->rows, "%s row %d out of range [0, %d)", what, rows[i], s->rows);
-    for (int j = 0; j < i; ++j) Q3_REQUIRE(rows[i] != rows[j], "%s row %d listed twice", what, rows[i]);
-  }
-  return 0;
-}
-
 extern "C" int q3_resample_reset_rows(q3_resampler* s, int32_t n, const int32_t* rows_host, const int32_t* filters_host,
                                       const int32_t* encodings_host) {
   Q3_REQUIRE(s, "null resampler");
-  if (check_rows(s, n, rows_host, "reset")) return 1;
+  if (check_row_list(s->rows, n, rows_host, "reset", "resampler")) return 1;
   Q3_REQUIRE(n == 0 || (filters_host && encodings_host), "null argument");
   for (int i = 0; i < n; ++i) {
     Q3_REQUIRE(filter_live(s, filters_host[i]), "row %d: filter %d not added", rows_host[i], filters_host[i]);
@@ -137,7 +128,7 @@ extern "C" int q3_resample_reset_rows(q3_resampler* s, int32_t n, const int32_t*
 
 extern "C" int q3_resample_release_rows(q3_resampler* s, int32_t n, const int32_t* rows_host) {
   Q3_REQUIRE(s, "null resampler");
-  if (check_rows(s, n, rows_host, "release")) return 1;
+  if (check_row_list(s->rows, n, rows_host, "release", "resampler")) return 1;
   for (int i = 0; i < n; ++i) {
     s->fid[rows_host[i]] = -1;
     s->n_in[rows_host[i]] = 0;
@@ -207,7 +198,7 @@ static int move_rows(q3_resampler* s, int n, const int32_t* rows_host, void* rec
 
 extern "C" int q3_resample_save_rows(q3_resampler* s, int32_t n, const int32_t* rows_host, void* dst_dev, void* stream) {
   Q3_REQUIRE(s, "null resampler");
-  if (check_rows(s, n, rows_host, "save")) return 1;
+  if (check_row_list(s->rows, n, rows_host, "save", "resampler")) return 1;
   if (n == 0) return 0;
   Q3_REQUIRE(dst_dev, "null argument");
   for (int i = 0; i < n; ++i) Q3_REQUIRE(s->fid[rows_host[i]] >= 0, "save row %d was never reset", rows_host[i]);
@@ -216,16 +207,13 @@ extern "C" int q3_resample_save_rows(q3_resampler* s, int32_t n, const int32_t* 
 
 extern "C" int q3_resample_load_rows(q3_resampler* s, int32_t n, const int32_t* rows_host, const void* src_dev, void* stream) {
   Q3_REQUIRE(s, "null resampler");
-  if (check_rows(s, n, rows_host, "load")) return 1;
+  if (check_row_list(s->rows, n, rows_host, "load", "resampler")) return 1;
   if (n == 0) return 0;
   Q3_REQUIRE(src_dev, "null argument");
   cudaStream_t st = (cudaStream_t)stream;
   Q3_CUDA(cudaSetDevice(s->device));
-  // the headers come back to the host: a row's counters size its outputs at every later step without a sync
-  std::vector<RowRecord> rec(n);
-  for (int i = 0; i < n; ++i)
-    Q3_CUDA(cudaMemcpyAsync(&rec[i], (const RowRecord*)src_dev + i, offsetof(RowRecord, hist), cudaMemcpyDeviceToHost, st));
-  Q3_CUDA(cudaStreamSynchronize(st));
+  std::vector<RowRecord> rec;
+  if (read_headers(rec, src_dev, n, offsetof(RowRecord, hist), st)) return 1;
   for (int i = 0; i < n; ++i) {
     Q3_REQUIRE(filter_live(s, rec[i].fid) && rec[i].enc >= Q3_RESAMPLE_F32 &&
                    rec[i].enc <= Q3_RESAMPLE_ULAW && rec[i].n_in >= 0,

@@ -11,6 +11,7 @@
 // bit for bit.
 #include "common.cuh"
 #include "dev_store.h"
+#include "row_state.h"
 
 #include <algorithm>
 #include <cstddef>
@@ -78,19 +79,9 @@ extern "C" int q3_stretch_set_window(q3_stretcher* s, const float* window_dev) {
   return 0;
 }
 
-static int check_rows(const q3_stretcher* s, int n, const int32_t* rows, const char* what) {
-  Q3_REQUIRE(n >= 0 && n <= s->rows, "%d rows to %s, the stretcher has %d", n, what, s->rows);
-  Q3_REQUIRE(n == 0 || rows, "null argument");
-  for (int i = 0; i < n; ++i) {
-    Q3_REQUIRE(rows[i] >= 0 && rows[i] < s->rows, "%s row %d out of range [0, %d)", what, rows[i], s->rows);
-    for (int j = 0; j < i; ++j) Q3_REQUIRE(rows[i] != rows[j], "%s row %d listed twice", what, rows[i]);
-  }
-  return 0;
-}
-
 extern "C" int q3_stretch_reset_rows(q3_stretcher* s, int32_t n, const int32_t* rows_host, const int32_t* hops_host) {
   Q3_REQUIRE(s, "null stretcher");
-  if (check_rows(s, n, rows_host, "reset")) return 1;
+  if (check_row_list(s->rows, n, rows_host, "reset", "stretcher")) return 1;
   Q3_REQUIRE(n == 0 || hops_host, "null argument");
   for (int i = 0; i < n; ++i)
     Q3_REQUIRE(hops_host[i] >= kStDelta && hops_host[i] <= 2 * kStHs, "row %d: hop %d outside [%d, %d]", rows_host[i],
@@ -159,7 +150,7 @@ static int move_rows(q3_stretcher* s, int n, const int32_t* rows_host, void* rec
 
 extern "C" int q3_stretch_save_rows(q3_stretcher* s, int32_t n, const int32_t* rows_host, void* dst_dev, void* stream) {
   Q3_REQUIRE(s, "null stretcher");
-  if (check_rows(s, n, rows_host, "save")) return 1;
+  if (check_row_list(s->rows, n, rows_host, "save", "stretcher")) return 1;
   if (n == 0) return 0;
   Q3_REQUIRE(dst_dev, "null argument");
   for (int i = 0; i < n; ++i) Q3_REQUIRE(s->ha[rows_host[i]] > 0, "save row %d was never reset", rows_host[i]);
@@ -169,17 +160,13 @@ extern "C" int q3_stretch_save_rows(q3_stretcher* s, int32_t n, const int32_t* r
 extern "C" int q3_stretch_load_rows(q3_stretcher* s, int32_t n, const int32_t* rows_host, const void* src_dev,
                                     void* stream) {
   Q3_REQUIRE(s, "null stretcher");
-  if (check_rows(s, n, rows_host, "load")) return 1;
+  if (check_row_list(s->rows, n, rows_host, "load", "stretcher")) return 1;
   if (n == 0) return 0;
   Q3_REQUIRE(src_dev, "null argument");
   cudaStream_t st = (cudaStream_t)stream;
   Q3_CUDA(cudaSetDevice(s->device));
-  // the headers come back to the host: a row's hop and count size its outputs at every later step without a sync
-  std::vector<StretchRecord> rec(n);
-  for (int i = 0; i < n; ++i)
-    Q3_CUDA(cudaMemcpyAsync(&rec[i], (const StretchRecord*)src_dev + i, offsetof(StretchRecord, tail),
-                            cudaMemcpyDeviceToHost, st));
-  Q3_CUDA(cudaStreamSynchronize(st));
+  std::vector<StretchRecord> rec;
+  if (read_headers(rec, src_dev, n, offsetof(StretchRecord, tail), st)) return 1;
   for (int i = 0; i < n; ++i) {
     Q3_REQUIRE(rec[i].ha >= kStDelta && rec[i].ha <= 2 * kStHs && rec[i].n_in >= 0 &&
                    rec[i].frames == frames_done(rec[i].n_in, rec[i].ha),

@@ -60,36 +60,21 @@ completes it with tts_pad and makes the trailing text [tts_pad], build_prefill's
 the request is not admitted, takes no slot a park would free, and does not keep run() going; once complete it is
 admitted and runs as any live request, so it generates what its whole text gives up front (tests/test_gpu_live_clone.py).
 
-Audio formats (`ContinuousBatcher(audio_format=)` for the session, `submit(audio_format=)` per request, an AudioFormat):
-a request with a rate or encoding other than the codec's 24 kHz float32 has a row of one audio.Resampler of `n_slots`
-rows, opened when the first such request is admitted.  After each codec push its slot's new samples go through one
-resampler launch with every other such slot, including the tails of requests that finished in the step (even with no
-new frame), and stream() yields its chunk as float32, int16 or uint8.  Its row is reset at admission (by reset, seed or
-bank copy alike: the resampled audio is the generated part's), saved on the request when it is parked and loaded into
-its new slot when resumed.  A request's concatenated chunks equal Resampler.oneshot of its whole audio
-(tests/test_gpu_scheduler_audio_format.py).  Requests in the codec's own format take today's path, so a session
-without formats makes the same calls as before.
-
-Speaking rate (`AudioFormat(speed=)`): a request whose speed gives an analysis hop other than 480
-(audio.TimeStretch.hop) has a row of one audio.TimeStretch of `n_slots` rows, opened when the first such request is
-admitted.  Its slot's new samples go through one time-stretch launch with every other such slot on the device, then
-through its resampler row if its rate or encoding is not 24 kHz float32; a finishing request ends its stretch row and
-passes that tail into its resampler end in the same step.  The row is reset at admission after the codec row's reset,
-seed or bank copy (it stretches the generated part only), saved on park, loaded on resume and dropped on cancel.  A
-request's concatenated chunks equal Resampler.oneshot(TimeStretch.oneshot(w, speed), 24000, its rate and encoding), w
-its whole waveform (tests/test_gpu_scheduler_speed.py).  A session where no request has another speed makes the same
-calls as before.
-
-Pitch and volume (`AudioFormat(pitch=, volume=)`): a request whose pitch step Lp (AudioFormat.pitch_step) is not 480
-has its time-stretch row at hop AudioFormat.hop (skipped when that hop is 480) and a resampler row converting from
-50*Lp Hz to its rate and encoding, even at 24 kHz float32.  A request with a volume other than 0 dB has a row of one
-audio.Limiter of `n_slots` rows, opened when the first such request is admitted; it runs after the time-stretch and
-before the resampler, and is reset at admission after the time-stretch's reset, saved on park, loaded on resume and
-dropped on cancel.  A finishing request's stretch tail goes through the limiter's end into the resampler's end in the
-same step.  A request's concatenated chunks equal
+Audio formats (`ContinuousBatcher(audio_format=)` for the session, `submit(audio_format=)` per request, an AudioFormat
+of rate, encoding, speed, pitch and volume): a request's audio runs through the chain of stages audio.stages gives its
+format, in order a time-stretch (a speed or pitch), a limiter (a volume) and a resampler (a pitch, or a rate or
+encoding other than 24 kHz float32); a request in the codec's own format has none.  Each stage is one object of
+`n_slots` rows, opened when the first request that uses it is admitted, and a request has a row in each stage of its
+chain, in its slot.  The rows are reset at admission after the codec row's reset, seed or bank copy (they shape the
+generated part only), one reset per stage and setting; saved on the request when it is parked, loaded into its new
+slot when it is resumed, and dropped with it on cancel.  After each codec push one launch per stage serves every slot
+that uses it, the samples going from stage to stage on the device; a request that finished in the step ends its row in
+each stage, so each stage's tail goes on into the next stage's end in the same step (even with no new frame), and
+stream() yields its chunk as float32, int16 or uint8.  A request's concatenated chunks equal
     Resampler.oneshot(Limiter.oneshot(TimeStretch.oneshot(w, speed, pitch), volume), 50*Lp, AudioFormat(rate, encoding))
-bit for bit, each stage skipped when its request does not use it (tests/test_gpu_scheduler_pitch_volume.py).  A session
-where every request has pitch 0 and volume 0 makes the same calls as before.
+bit for bit, w its whole waveform, Lp its pitch step and each stage skipped when its chain has none
+(tests/test_gpu_scheduler_audio_format.py, test_gpu_scheduler_speed.py, test_gpu_scheduler_pitch_volume.py).  A session
+without formats opens no stage and makes the same calls as before.
 """
 from collections import deque
 from dataclasses import dataclass, field
@@ -124,19 +109,17 @@ class _Request:
     bank: Optional[Tuple[int, int]] = None
     codes: Optional[torch.Tensor] = None
     overlay: Optional[torch.Tensor] = None   # prompt rows still waiting for a text row each (None once complete)
-    fmt: Optional[AudioFormat] = None        # the client's rate and encoding; None: the codec's own (no resampler row)
-    res_state: Optional[audio.ResamplerState] = None   # while parked: its resampler row's saved state
-    speed: Optional[float] = None            # the client's speaking rate; None: as generated (no time-stretch row)
-    st_state: Optional[torch.Tensor] = None    # while parked: its time-stretch row's saved state
-    pitch: float = 0.0                       # its pitch in semitones; 0 when its pitch step is 480 (no pitch shift)
-    in_rate: int = audio.CODEC_RATE          # the rate its resampler row converts from: 50 * its pitch step
-    volume: Optional[float] = None           # its volume in dB; None: 0 dB (no limiter row)
-    lim_state: Optional[torch.Tensor] = None   # while parked: its limiter row's saved state
+    chain: Dict[str, tuple] = field(default_factory=dict)   # its stages in order: {name: reset arguments} (audio.stages)
+    saved: Dict[str, Any] = field(default_factory=dict)     # while parked: {stage name: its row's saved state}
+    # while parked: its row's saved state in each stage, None without a row there
+    st_state = property(lambda self: self.saved.get("TimeStretch"))
+    lim_state = property(lambda self: self.saved.get("Limiter"))
+    res_state = property(lambda self: self.saved.get("Resampler"))
 
     @property
     def shaped(self) -> bool:
-        """Its audio goes through a time-stretch, a limiter or a resampler row."""
-        return self.fmt is not None or self.speed is not None or self.volume is not None
+        """Its audio goes through a chain of stages."""
+        return bool(self.chain)
 
 
 class ContinuousBatcher:
@@ -174,29 +157,28 @@ class ContinuousBatcher:
             self.cstream = codec.open_stream(self.n_slots, max_packet_frames=self.packet) if codec is not None else None
         else:
             raise ValueError(f"codec must be a CodecDecoder or a CodecStream, got {type(codec).__name__}")
-        self._check_format(audio_format)
+        self._chain(audio_format)
         self.audio_format = audio_format
-        self.resampler: Optional[audio.Resampler] = None   # opened when the first request with a format is admitted
-        self.stretcher: Optional[audio.TimeStretch] = None   # opened when the first request with a speed is admitted
-        self.limiter: Optional[audio.Limiter] = None   # opened when the first request with a volume is admitted
+        self.stages: Dict[str, Any] = {}   # stage name -> its object, in chain order; opened by the first request using it
 
-    def _check_format(self, fmt: Optional[AudioFormat]) -> Optional[AudioFormat]:
-        """The rate and encoding a request's resampler row converts to: None for the codec's own 24 kHz float32 without
-        a pitch shift (no resampling)."""
-        if fmt is None:
-            return None
-        audio.check_format(fmt)
-        if self.codec is None:
+    # each stage of `stages`, None until the first request that uses it is admitted
+    stretcher = property(lambda self: self.stages.get("TimeStretch"))
+    limiter = property(lambda self: self.stages.get("Limiter"))
+    resampler = property(lambda self: self.stages.get("Resampler"))
+
+    def _chain(self, fmt: Optional[AudioFormat]) -> Dict[str, tuple]:
+        """The stages a request in `fmt` runs, in order, with their reset arguments (audio.stages)."""
+        chain = dict(audio.stages(fmt))
+        if fmt is not None and self.codec is None:
             raise ValueError("an audio format needs a ContinuousBatcher built with a codec")
-        out = AudioFormat(fmt.sample_rate, fmt.encoding)
-        return None if out == AudioFormat(audio.CODEC_RATE) and fmt.pitch_step == 480 else out
+        return chain
 
-    @staticmethod
-    def _speed(fmt: Optional[AudioFormat]) -> Optional[float]:
-        """The speed a request's time-stretch row runs at: None when its hop is 480 (no stretch)."""
-        if fmt is None or fmt.hop == audio.TimeStretch.HS:
-            return None
-        return fmt.speed
+    def _stage(self, name: str):
+        """The stage `name` (a class of audio, looked up when it is opened, on first use), kept in chain order."""
+        if name not in self.stages:
+            self.stages[name] = getattr(audio, name)(self.eng.device, self.n_slots, self.packet * self.codec.total_upsample)
+            self.stages = {n: self.stages[n] for n in audio.STAGES if n in self.stages}
+        return self.stages[name]
 
     # ------------------------------------------------------------------ API
     def submit(self, inputs_embeds: torch.Tensor, trailing_text: Optional[torch.Tensor] = None, key: Optional[int] = None,
@@ -218,11 +200,7 @@ class ContinuousBatcher:
         request is admitted once it is full or its text is closed (see the module docstring).  `audio_format`: the
         sample rate and encoding of the request's stream() chunks (default: the session's).  Bad parameters raise
         ValueError here, never in a later step()."""
-        src = audio_format if audio_format is not None else self.audio_format
-        fmt, speed = self._check_format(src), self._speed(src)
-        pitched = src is not None and src.pitch_step != 480
-        shape = dict(pitch=src.pitch if pitched else 0.0, in_rate=50 * src.pitch_step if pitched else audio.CODEC_RATE,
-                     volume=src.volume if src is not None and src.volume != 0 else None)
+        chain = self._chain(audio_format if audio_format is not None else self.audio_format)
         H = self.eng.cfg.talker.hidden_size
         L_ref, P = 0, 0
         if overlay is not None:
@@ -274,7 +252,7 @@ class ContinuousBatcher:
         if self.codec is not None:
             horizon = min(horizon, self.codec.max_frames - L_ref)  # a codec row's position may not pass its RoPE table
         r = _Request(rid, inputs_embeds, tr, horizon, sampling, ref_codes, voice, text_open=bool(text_open),
-                     overlay=overlay if K else None, fmt=fmt, speed=speed, **shape)
+                     overlay=overlay if K else None, chain=chain)
         if r.overlay is not None:
             r.trailing = self._fill(r, tr.reshape(-1, H))
         r.n_text = int(r.trailing.reshape(-1, H).shape[0])
@@ -362,11 +340,11 @@ class ContinuousBatcher:
                 self._cancelled.add(rid)
                 return True
         r = self.parked.pop(rid, None)
-        if r is not None:    # its record, its codec bank row and its resampler, time-stretch and limiter states are freed
+        if r is not None:    # its record, its codec bank row and its stages' states are freed
             self.eng.discard(r.record)
             if r.bank is not None:
                 self.codec.bank_release(*r.bank)
-            r.res_state = r.st_state = r.lim_state = None
+            r.saved = {}
             self._cancelled.add(rid)
             return True
         return False
@@ -403,12 +381,7 @@ class ContinuousBatcher:
         r.record = self.eng.park(slot)
         if self.cstream is not None:
             r.bank = self.codec.bank_copy(self.cstream, slot)
-        if r.fmt is not None:
-            r.res_state = self.resampler.save([slot])
-        if r.speed is not None:
-            r.st_state = self.stretcher.save([slot])
-        if r.volume is not None:
-            r.lim_state = self.limiter.save([slot])
+        r.saved = {name: self.stages[name].save([slot]) for name in r.chain}
         r.trailing = r.trailing.reshape(-1, self.eng.cfg.talker.hidden_size)[:0]   # the record holds the text so far
         r.slot = -1
         self.parked[r.rid] = r
@@ -428,15 +401,9 @@ class ContinuousBatcher:
             self.cstream.copy_from(self.codec.bank_stream(r.bank[0]), [r.bank[1]], [slot])
             self.codec.bank_release(*r.bank)   # a later bank_copy into that row is queued behind this copy
             r.bank = None
-        if r.res_state is not None:
-            self.resampler.load([slot], r.res_state)
-            r.res_state = None
-        if r.st_state is not None:
-            self.stretcher.load([slot], r.st_state)
-            r.st_state = None
-        if r.lim_state is not None:
-            self.limiter.load([slot], r.lim_state)
-            r.lim_state = None
+        for name, state in r.saved.items():
+            self.stages[name].load([slot], state)
+        r.saved = {}
         if r.trailing.shape[0] > 0:
             self.eng.append_trailing(slot, r.trailing)
             r.trailing = r.trailing[:0]
@@ -455,7 +422,7 @@ class ContinuousBatcher:
         [ids that finished in the step]) while requests are pending, running or parked, so a request submitted between
         two iterations is admitted at the next one.  A waveform is float32 at the codec's 24 kHz, or in the request's
         audio format (float32, int16 or uint8 at its rate); a request with a format also gets an entry in the step it
-        finishes, holding its resampler's tail."""
+        finishes, holding its stages' tails."""
         if self.cstream is None:
             raise ValueError("stream() needs a ContinuousBatcher built with a codec")
         while self.pending or self.running or self.parked:
@@ -523,18 +490,9 @@ class ContinuousBatcher:
                 for bank in sorted({r.voice.bank[0] for r in banked}):   # one copy per bank, no reference decode
                     rs = [r for r in banked if r.voice.bank[0] == bank]
                     self.cstream.copy_from(self.codec.bank_stream(bank), [r.voice.bank[1] for r in rs], [r.slot for r in rs])
-                for key in dict.fromkeys((r.in_rate, r.fmt) for r in batch if r.fmt is not None):   # one reset per pair
-                    if self.resampler is None:
-                        self.resampler = audio.Resampler(self.eng.device, self.n_slots, self.packet * self.codec.total_upsample)
-                    self.resampler.reset([r.slot for r in batch if (r.in_rate, r.fmt) == key], *key)
-                for key in dict.fromkeys((r.speed, r.pitch) for r in batch if r.speed is not None):   # one per hop
-                    if self.stretcher is None:
-                        self.stretcher = audio.TimeStretch(self.eng.device, self.n_slots, self.packet * self.codec.total_upsample)
-                    self.stretcher.reset([r.slot for r in batch if (r.speed, r.pitch) == key], *key[:1 + (key[1] != 0)])
-                for volume in dict.fromkeys(r.volume for r in batch if r.volume is not None):   # one reset per volume
-                    if self.limiter is None:
-                        self.limiter = audio.Limiter(self.eng.device, self.n_slots, self.packet * self.codec.total_upsample)
-                    self.limiter.reset([r.slot for r in batch if r.volume == volume], volume)
+                for name in audio.STAGES:   # one reset per stage and setting
+                    for args in dict.fromkeys(r.chain[name] for r in batch if name in r.chain):
+                        self._stage(name).reset([r.slot for r in batch if r.chain.get(name) == args], *args)
         if not batch and not self._runnable():
             return {}, []   # every running row is open and waiting for text: launch nothing
         n = min([self.packet] + [r.max_frames - r.emitted for r in self.running.values()])
@@ -560,7 +518,7 @@ class ContinuousBatcher:
 
     def _push_audio(self, new) -> Dict[int, np.ndarray]:
         """One codec step over all slots: slot s takes its new frames codes[s, e0:e0+k] as its count k, idle slots 0.
-        Slots of requests with a format then take their new audio through one resampler launch, and those whose
+        Slots of requests with a chain of stages then take their new audio through it (_push_formats), and those whose
         request finished in this step end their clips there (their tails come even without new frames)."""
         if self.cstream is None:
             return {}
@@ -568,26 +526,6 @@ class ContinuousBatcher:
         ending = [slot for slot, (r, _, _) in new.items() if r.shaped and self.running.get(slot) is not r]
         if m == 0 and not ending:
             return {}
-        if any(r.shaped for r, _, _ in new.values()):
-            return self._push_formats(new, m, ending)
-        start, counts = [0] * self.n_slots, [0] * self.n_slots
-        for slot, (_, e0, k) in new.items():
-            start[slot], counts[slot] = e0, k
-        idx = (torch.tensor(start)[:, None] + torch.arange(m)[None]).clamp_(max=self.max_frames - 1)
-        rows = torch.arange(self.n_slots)[:, None]
-        codes = self.codes[rows.to(self.codes.device), idx.to(self.codes.device)].transpose(1, 2)  # [S][G][m]
-        wav = self.cstream.push(codes, counts)[:, 0].cpu().numpy()
-        up = self.codec.total_upsample
-        return {r.rid: wav[slot, :k * up] for slot, (r, _, k) in new.items() if k > 0}
-
-    def _push_formats(self, new, m: int, ending: List[int]) -> Dict[int, np.ndarray]:
-        """_push_audio of a step in which some request is shaped: the codec push stays on the device, the default
-        slots' audio comes back as before, the others' goes through the chain of stages their requests use, in order:
-        the time-stretch (a speed or pitch), the limiter (a volume), the resampler (a pitch, or a rate or encoding other
-        than 24 kHz float32).  One launch per stage serves every slot that uses it; a request that finished in the step
-        ends its row in each of its stages, and each stage's tail goes on into the next stage's end."""
-        up = self.codec.total_upsample
-        out: Dict[int, np.ndarray] = {}
         wav = None
         if m > 0:
             start, counts = [0] * self.n_slots, [0] * self.n_slots
@@ -597,26 +535,35 @@ class ContinuousBatcher:
             rows = torch.arange(self.n_slots)[:, None]
             codes = self.codes[rows.to(self.codes.device), idx.to(self.codes.device)].transpose(1, 2)  # [S][G][m]
             wav = self.cstream.push(codes, counts)[:, 0]
-            plain = [slot for slot, (r, _, k) in new.items() if not r.shaped and k > 0]
-            if plain:
-                host = wav[plain].cpu().numpy()
-                for i, slot in enumerate(plain):
-                    out[new[slot][0].rid] = host[i, :new[slot][2] * up]
-        stages = [(self.stretcher, lambda r: r.speed is not None), (self.limiter, lambda r: r.volume is not None),
-                  (self.resampler, lambda r: r.fmt is not None)]
-        chain = [(obj, uses) for obj, uses in stages if any(uses(r) for r, _, _ in new.values())]
+        if any(r.shaped for r, _, _ in new.values()):
+            return self._push_formats(new, wav, ending)
+        wav = wav.cpu().numpy()
+        up = self.codec.total_upsample
+        return {r.rid: wav[slot, :k * up] for slot, (r, _, k) in new.items() if k > 0}
+
+    def _push_formats(self, new, wav: Optional[torch.Tensor], ending: List[int]) -> Dict[int, np.ndarray]:
+        """_push_audio of a step in which some request is shaped, `wav` the codec push's audio on the device (None
+        without new frames): the default slots' audio comes back as before, the others' goes through their chains.  One
+        launch per stage serves every slot that uses it; a request that finished in the step ends its row in each of
+        its stages, and each stage's tail goes on into the next stage's end."""
+        up = self.codec.total_upsample
+        out: Dict[int, np.ndarray] = {}
+        plain = [slot for slot, (r, _, k) in new.items() if not r.shaped and k > 0]
+        if plain:
+            host = wav[plain].cpu().numpy()
+            for i, slot in enumerate(plain):
+                out[new[slot][0].rid] = host[i, :new[slot][2] * up]
         x, cnt = wav, {slot: k * up for slot, (r, _, k) in new.items() if r.shaped and k > 0}   # each slot's input
-        for i, (obj, uses) in enumerate(chain):
-            def later(slot, rest=chain[i + 1:]):
-                return any(u(new[slot][0]) for _, u in rest)
-            counts = {slot: c for slot, c in cnt.items() if uses(new[slot][0])}
-            end = [slot for slot in ending if uses(new[slot][0])]
-            if i > 0 and not counts and not end:
+        for name, obj in self.stages.items():
+            counts = {slot: c for slot, c in cnt.items() if name in new[slot][0].chain}
+            end = [slot for slot in ending if name in new[slot][0].chain]
+            if not counts and not end:
                 continue
-            onward = [slot for slot in sorted(set(counts) | set(end)) if later(slot)]
+            last = {slot: next(reversed(new[slot][0].chain)) == name for slot in set(counts) | set(end)}
+            onward = [slot for slot in sorted(last) if not last[slot]]
             got = obj.push_rows(x if counts else None, counts, end, host=not onward)
             for slot, y in got.items():
-                if not later(slot) and (y.shape[0] or slot in ending):   # a stage's delay can hold a short push back
+                if last[slot] and (y.shape[0] or slot in ending):   # a stage's delay can hold a short push back
                     out[new[slot][0].rid] = y if not onward else y.cpu().numpy()
             cnt = {slot: c for slot, c in cnt.items() if slot not in counts}
             if not onward:

@@ -1,13 +1,14 @@
 """Audio formats without a GPU: the resampler's count formulas against a brute-force restatement for every supported
 pair, AudioFormat validation, the G.711 restatement against audioop, and the continuous batcher's format handling
 (default sessions untouched, bad formats refused at submit, a final chunk for a request that ends without new frames,
-park / resume / cancel carrying and dropping the row's state) against fake engines, codec and resampler."""
+park / resume / cancel carrying and dropping the row's state) against fake engines, codec and stages."""
 import numpy as np
 import pytest
 import torch
 
 from qwen3_tts_b200 import audio
 from qwen3_tts_b200.config import SUPPORTED_RATES, AudioFormat, SamplingParams
+from tests.fake_stages import install
 from tests.test_scheduler_cpu import FakeEngine, _mock_sync
 from tests.test_scheduler_park_cpu import H, UP, BankCodec, ParkingEngine
 
@@ -73,47 +74,9 @@ def test_ulaw_restatement_equals_audioop_on_every_int16():
 
 
 # ---------------------------------------------------------------------------------------------- the batcher
-class FakeResampler:
-    """Counts like the real resampler (emitted / total per pair); output sample j of a clip is j (in the encoding's
-    dtype, mod 251), so a row that lost its state would restart at 0.  Records every call."""
-    made = []
-
-    def __init__(self, device, rows, max_in):
-        self.rows, self.max_in, self.log = rows, max_in, []
-        self.state = [None] * rows    # (up, down, encoding, inputs so far)
-        FakeResampler.made.append(self)
-
-    def reset(self, rows, in_rate, fmt):
-        self.log.append(("reset", list(rows), fmt))
-        for r in rows:
-            self.state[r] = (*audio.ratio(in_rate, fmt.sample_rate), fmt.encoding, 0)
-
-    def push_rows(self, x, counts, end=(), host=True):
-        self.log.append(("push", dict(counts), list(end)))
-        out = {}
-        for r in sorted(set(counts) | set(end)):
-            up, down, enc, n = self.state[r]
-            n1 = n + counts.get(r, 0)
-            a, b = audio.emitted(n, up, down), audio.total(n1, up, down) if r in end else audio.emitted(n1, up, down)
-            out[r] = (np.arange(a, b) % 251).astype({"f32": np.float32, "s16": np.int16, "ulaw": np.uint8}[enc])
-            self.state[r] = (up, down, enc, 0 if r in end else n1)
-        return out
-
-    def save(self, rows):
-        self.log.append(("save", list(rows)))
-        return [self.state[r] for r in rows]
-
-    def load(self, rows, state):
-        self.log.append(("load", list(rows)))
-        for r, s in zip(rows, state):
-            self.state[r] = s
-
-
 @pytest.fixture
-def fake_resampler(monkeypatch):
-    FakeResampler.made = []
-    monkeypatch.setattr(audio, "Resampler", FakeResampler)
-    return FakeResampler
+def fakes(monkeypatch):
+    return install(monkeypatch)
 
 
 def _batcher(codec=True, eng=None, **kw):
@@ -138,20 +101,20 @@ def _want(n_frames, fmt):
     return (np.arange(n) % 251).astype({"f32": np.float32, "s16": np.int16, "ulaw": np.uint8}[fmt.encoding])
 
 
-def test_session_without_formats_opens_no_resampler(monkeypatch, fake_resampler):
+def test_session_without_formats_opens_no_resampler(monkeypatch, fakes):
     _mock_sync(monkeypatch)
     for kw in ({}, {"audio_format": AudioFormat(24000)}):
         eng, cb = _batcher(**kw)
         a = cb.submit(torch.zeros(4, H), torch.zeros(2, H), key=1, max_frames=6)
         b = cb.submit(torch.zeros(4, H), torch.zeros(2, H), key=2, max_frames=3, audio_format=AudioFormat(24000, "f32"))
         out = _drain(cb)
-        assert cb.resampler is None and fake_resampler.made == []
+        assert cb.resampler is None and cb.stages == {} and all(f.made == [] for f in fakes.values())
         for rid, n in ((a, 6), (b, 3)):
             assert all(c.dtype == np.float32 and c.shape[0] > 0 for c in out[rid])
             assert np.concatenate(out[rid]).shape == (n * UP,)
 
 
-def test_bad_formats_are_refused_at_submit(monkeypatch, fake_resampler):
+def test_bad_formats_are_refused_at_submit(monkeypatch, fakes):
     _mock_sync(monkeypatch)
     eng, cb = _batcher()
     for bad in ("ulaw", 8000, (8000, "ulaw"), {"sample_rate": 8000}):
@@ -165,7 +128,7 @@ def test_bad_formats_are_refused_at_submit(monkeypatch, fake_resampler):
         plain.submit(torch.zeros(4, H), audio_format=AudioFormat(8000))
 
 
-def test_a_request_ending_without_new_frames_gets_its_tail(monkeypatch, fake_resampler):
+def test_a_request_ending_without_new_frames_gets_its_tail(monkeypatch, fakes):
     _mock_sync(monkeypatch)
     # EOS right after the first packet: the next step has no new frame
     eng, cb = _batcher(eng=FakeEngine(eos_at={1: 4, 2: 4}))
@@ -177,12 +140,12 @@ def test_a_request_ending_without_new_frames_gets_its_tail(monkeypatch, fake_res
     assert a in steps[1][0] and b not in steps[1][0]        # the default request gets no entry, as before
     got = np.concatenate([c[a] for c, _ in steps if a in c])
     assert np.array_equal(got, _want(4, fmt))
-    res = fake_resampler.made[0]
-    assert res.log[-1] == ("push", {}, [0])
+    res = fakes["Resampler"].made[0]
+    assert res.log[-1] == ("push", {}, [0], True)
     assert cb.done[a].shape[0] == 4
 
 
-def test_park_resume_and_cancel_carry_and_drop_the_resampler_state(monkeypatch, fake_resampler):
+def test_park_resume_and_cancel_carry_and_drop_the_resampler_state(monkeypatch, fakes):
     _mock_sync(monkeypatch)
     eng, cb = _batcher()
     fmt = AudioFormat(16000, "s16")
@@ -201,7 +164,7 @@ def test_park_resume_and_cancel_carry_and_drop_the_resampler_state(monkeypatch, 
             assert cb.cancel(c) and rc.res_state is None
             cb.resume(a)
     assert np.array_equal(np.concatenate(out[a]), _want(12, fmt))
-    res = fake_resampler.made[0]
+    res = fakes["Resampler"].made[0]
     assert ("save", [0]) in res.log and ("save", [1]) in res.log and ("load", [0]) in res.log
     assert len([e for e in res.log if e[0] == "load"]) == 1       # the cancelled request's state was never loaded
     assert c not in cb.done

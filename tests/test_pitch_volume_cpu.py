@@ -14,10 +14,10 @@ import torch
 from qwen3_tts_b200 import audio
 from qwen3_tts_b200.config import SUPPORTED_RATES, AudioFormat
 from tests import limiter_ref as LR
-from tests.test_audio_format_cpu import FakeResampler, _batcher, _drain
+from tests.fake_stages import install
+from tests.test_audio_format_cpu import _batcher, _drain
 from tests.test_scheduler_cpu import FakeEngine, _mock_sync
 from tests.test_scheduler_park_cpu import H, UP
-from tests.test_stretch_cpu import FakeStretch
 
 TS = audio.TimeStretch
 LIM = audio.Limiter
@@ -251,67 +251,9 @@ def test_a_full_table_of_filters_in_use_is_refused(monkeypatch):
 
 
 # ------------------------------------------------------------------------------------------------- the batcher
-class PitchStretch(FakeStretch):
-    """FakeStretch whose reset takes a pitch (logged only when given)."""
-
-    def reset(self, rows, speed, *pitch):
-        self.log.append(("reset", list(rows), speed, *pitch))
-        for r in rows:
-            self.state[r] = (TS.hop(speed, *pitch), 0)
-
-
-class PitchResampler(FakeResampler):
-    """FakeResampler that takes a pitched input rate; its resets log the input rate."""
-
-    def reset(self, rows, in_rate, fmt):
-        self.log.append(("reset", list(rows), in_rate, fmt))
-        for r in rows:
-            self.state[r] = (*audio.ratio(in_rate, fmt.sample_rate, pitched=True), fmt.encoding, 0)
-
-
-class FakeLimiter:
-    """Counts like the real limiter (emitted max(0, n - 119), total n); output sample j of a clip is 5000 + j.  Device
-    outputs are float32 tensors.  Records every call."""
-    made = []
-
-    def __init__(self, device, rows, max_in):
-        self.rows, self.max_in, self.log = rows, max_in, []
-        self.state = [None] * rows    # (volume, inputs so far)
-        FakeLimiter.made.append(self)
-
-    def reset(self, rows, volume):
-        self.log.append(("reset", list(rows), volume))
-        for r in rows:
-            self.state[r] = (volume, 0)
-
-    def push_rows(self, x, counts, end=(), host=True):
-        self.log.append(("push", dict(counts), list(end), host))
-        out = {}
-        for r in sorted(set(counts) | set(end)):
-            v, n = self.state[r]
-            n1 = n + counts.get(r, 0)
-            a, b = LIM.emitted(n), n1 if r in end else LIM.emitted(n1)
-            y = (5000 + np.arange(a, b)).astype(np.float32)
-            out[r] = y if host else torch.from_numpy(y)
-            self.state[r] = (v, 0 if r in end else n1)
-        return out
-
-    def save(self, rows):
-        self.log.append(("save", list(rows)))
-        return [self.state[r] for r in rows]
-
-    def load(self, rows, state):
-        self.log.append(("load", list(rows)))
-        for r, s in zip(rows, state):
-            self.state[r] = s
-
-
 @pytest.fixture
 def fakes(monkeypatch):
-    FakeStretch.made, FakeResampler.made, FakeLimiter.made = [], [], []
-    monkeypatch.setattr(audio, "TimeStretch", PitchStretch)
-    monkeypatch.setattr(audio, "Resampler", PitchResampler)
-    monkeypatch.setattr(audio, "Limiter", FakeLimiter)
+    return install(monkeypatch)
 
 
 def _chain(n_frames, fmt):
@@ -335,8 +277,8 @@ def test_sessions_without_pitch_or_volume_open_no_limiter_and_reset_as_before(mo
     eng, cb = _batcher()
     ids = [cb.submit(torch.zeros(4, H), key=i + 1, max_frames=6 + i, audio_format=f) for i, f in enumerate(fmts)]
     out = _drain(cb)
-    assert cb.limiter is None and FakeLimiter.made == []
-    st, res = FakeStretch.made[0], FakeResampler.made[0]
+    assert cb.limiter is None and fakes["Limiter"].made == []
+    st, res = fakes["TimeStretch"].made[0], fakes["Resampler"].made[0]
     assert all(len(e) == 3 for e in st.log if e[0] == "reset")          # reset(rows, speed), as before
     assert all(e[2] == 24000 for e in res.log if e[0] == "reset")       # resampled from 24 kHz, as before
     for rid, f in zip(ids, fmts):
@@ -354,7 +296,7 @@ def test_pitch_and_volume_route_through_stretch_limiter_and_resampler(monkeypatc
     a = cb.submit(torch.zeros(4, H), key=1, max_frames=12, audio_format=fa)
     b = cb.submit(torch.zeros(4, H), key=2, max_frames=12, audio_format=fb)
     out = _drain(cb)
-    st, lim, res = FakeStretch.made[0], FakeLimiter.made[0], FakeResampler.made[0]
+    st, lim, res = (fakes[n].made[0] for n in ("TimeStretch", "Limiter", "Resampler"))
     assert ("reset", [0], 1.1, 3.0) in st.log and ("reset", [1], 1.0, -2.0) in st.log
     assert lim.log[0] == ("reset", [0], -4.0)
     assert ("reset", [0], 50 * fa.pitch_step, AudioFormat(8000, "s16")) in res.log
@@ -390,12 +332,12 @@ def test_volume_alone_and_its_park_resume_and_cancel(monkeypatch, fakes):
             rc = cb.parked[c]
             assert cb.cancel(c) and rc.lim_state is None and rc.res_state is None
             cb.resume(a)
-    assert FakeStretch.made == []
-    lim = FakeLimiter.made[0]
+    assert fakes["TimeStretch"].made == []
+    lim = fakes["Limiter"].made[0]
     assert ("save", [0]) in lim.log and ("save", [1]) in lim.log and ("load", [0]) in lim.log
     assert len([e for e in lim.log if e[0] == "load"]) == 1 and c not in cb.done
     # volume alone at 24 kHz f32 has no resampler row: its chunks are the limiter's, host arrays
-    assert all(0 not in e[1] and 0 not in e[2] for e in FakeResampler.made[0].log if e[0] == "push")
+    assert all(0 not in e[1] and 0 not in e[2] for e in fakes["Resampler"].made[0].log if e[0] == "push")
     assert all(y.dtype == np.float32 and isinstance(y, np.ndarray) for y in out[a])
     assert np.array_equal(np.concatenate(out[a]), _chain(12, fa))
 

@@ -2,7 +2,7 @@
 analysis hop, the output capacity, AudioFormat.speed validation, the reference being a time-stretch (a tone keeps its
 pitch at every speed) and the continuous batcher's speed handling (no stretcher without speeds, a tail for a request
 that ends without new frames, park / resume / cancel carrying and dropping the row's state, speed before a resampler)
-against fake engines, codec, stretcher and resampler."""
+against fake engines, codec and stages."""
 import numpy as np
 import pytest
 import torch
@@ -10,7 +10,8 @@ import torch
 from qwen3_tts_b200 import audio
 from qwen3_tts_b200.config import AudioFormat
 from tests import stretch_ref as S
-from tests.test_audio_format_cpu import FakeResampler, _batcher, _drain
+from tests.fake_stages import install
+from tests.test_audio_format_cpu import _batcher, _drain
 from tests.test_scheduler_cpu import FakeEngine, _mock_sync
 from tests.test_scheduler_park_cpu import H, UP
 
@@ -83,50 +84,9 @@ def test_reference_stretches_a_tone_and_keeps_its_pitch(speed):
 
 
 # ---------------------------------------------------------------------------------------------- the batcher
-class FakeStretch:
-    """Counts like the real time-stretch (emitted / total per hop); output sample j of a clip is 1000 + j, so a row
-    that lost its state would restart at 1000.  Device outputs are float32 tensors.  Records every call."""
-    made = []
-    HS = 480
-    hop = staticmethod(TS.hop)
-
-    def __init__(self, device, rows, max_in):
-        self.rows, self.max_in, self.log = rows, max_in, []
-        self.state = [None] * rows    # (hop, inputs so far)
-        FakeStretch.made.append(self)
-
-    def reset(self, rows, speed):
-        self.log.append(("reset", list(rows), speed))
-        for r in rows:
-            self.state[r] = (TS.hop(speed), 0)
-
-    def push_rows(self, x, counts, end=(), host=True):
-        self.log.append(("push", dict(counts), list(end), host))
-        out = {}
-        for r in sorted(set(counts) | set(end)):
-            ha, n = self.state[r]
-            n1 = n + counts.get(r, 0)
-            a, b = TS.emitted(n, ha), TS.total(n1, ha) if r in end else TS.emitted(n1, ha)
-            y = (1000 + np.arange(a, b)).astype(np.float32)
-            out[r] = y if host else torch.from_numpy(y)
-            self.state[r] = (ha, 0 if r in end else n1)
-        return out
-
-    def save(self, rows):
-        self.log.append(("save", list(rows)))
-        return [self.state[r] for r in rows]
-
-    def load(self, rows, state):
-        self.log.append(("load", list(rows)))
-        for r, s in zip(rows, state):
-            self.state[r] = s
-
-
 @pytest.fixture
 def fakes(monkeypatch):
-    FakeStretch.made, FakeResampler.made = [], []
-    monkeypatch.setattr(audio, "TimeStretch", FakeStretch)
-    monkeypatch.setattr(audio, "Resampler", FakeResampler)
+    return install(monkeypatch)
 
 
 def _want(n_frames, speed):
@@ -139,7 +99,7 @@ def test_no_stretcher_without_speeds(monkeypatch, fakes):
         eng, cb = _batcher(audio_format=fmt)
         a = cb.submit(torch.zeros(4, H), torch.zeros(2, H), key=1, max_frames=6)
         _drain(cb)
-        assert cb.stretcher is None and FakeStretch.made == [] and cb.done[a].shape[0] == 6
+        assert cb.stretcher is None and fakes["TimeStretch"].made == [] and cb.done[a].shape[0] == 6
 
 
 def test_a_request_ending_without_new_frames_gets_its_tail(monkeypatch, fakes):
@@ -152,9 +112,9 @@ def test_a_request_ending_without_new_frames_gets_its_tail(monkeypatch, fakes):
     assert a in steps[1][0] and b not in steps[1][0]
     got = np.concatenate([c[a] for c, _ in steps if a in c])
     assert got.dtype == np.float32 and np.array_equal(got, _want(4, 0.75))
-    st = FakeStretch.made[0]
+    st = fakes["TimeStretch"].made[0]
     assert st.log[0] == ("reset", [0], 0.75) and st.log[-1] == ("push", {}, [0], True)
-    assert FakeResampler.made == []             # 24 kHz f32: no resampler row
+    assert fakes["Resampler"].made == []             # 24 kHz f32: no resampler row
 
 
 def test_park_resume_and_cancel_carry_and_drop_the_stretch_state(monkeypatch, fakes):
@@ -175,7 +135,7 @@ def test_park_resume_and_cancel_carry_and_drop_the_stretch_state(monkeypatch, fa
             assert cb.cancel(c) and rc.st_state is None
             cb.resume(a)
     assert np.array_equal(np.concatenate(out[a]), _want(12, 1.5))
-    st = FakeStretch.made[0]
+    st = fakes["TimeStretch"].made[0]
     assert ("save", [0]) in st.log and ("save", [1]) in st.log and ("load", [0]) in st.log
     assert len([e for e in st.log if e[0] == "load"]) == 1
     assert c not in cb.done
@@ -188,9 +148,9 @@ def test_speed_composes_with_a_resampled_format(monkeypatch, fakes):
     a = cb.submit(torch.zeros(4, H), key=1, max_frames=10, audio_format=fmt)
     b = cb.submit(torch.zeros(4, H), key=2, max_frames=6, audio_format=AudioFormat(16000, "ulaw"))
     out = _drain(cb)
-    st, res = FakeStretch.made[0], FakeResampler.made[0]
+    st, res = fakes["TimeStretch"].made[0], fakes["Resampler"].made[0]
     assert st.log[0] == ("reset", [0], 1.25)
-    assert ("reset", [0], AudioFormat(8000, "s16")) in res.log      # the resampler converts rate and encoding only
+    assert ("reset", [0], 24000, AudioFormat(8000, "s16")) in res.log      # the resampler converts rate and encoding only
     # the stretched samples go into the resampler: its row 0 took exactly the stretch's outputs, and its end came in
     # the step the stretch's tail did
     n_st = TS.total(8 * UP, TS.hop(1.25))

@@ -79,24 +79,15 @@ def main():
             cb = ContinuousBatcher(_Engine(dev), torch.zeros(8), q.SamplingParams(max_new_tokens=2048), n_slots=S,
                                    packet_frames=P, codec=dec)
             cb.codes.copy_(torch.randint(0, ccfg.codebook_size, cb.codes.shape, generator=g).to(cb.codes))
-            pitched = fmt is not None and fmt.pitch_step != 480
-            shape = dict(pitch=fmt.pitch if pitched else 0.0, in_rate=50 * fmt.pitch_step if pitched else 24000,
-                         volume=fmt.volume if fmt is not None and fmt.volume != 0 else None)
-            reqs = [_Request(s, None, None, 2000, fmt=cb._check_format(fmt), speed=cb._speed(fmt), **shape)
-                    for s in range(S)]
+            chain = dict(audio.stages(fmt))
+            reqs = [_Request(s, None, None, 2000, chain=chain) for s in range(S)]
             for s, r in enumerate(reqs):
                 r.slot = s
                 cb.running[s] = r
             cb.cstream.reset()
-            if reqs[0].fmt is not None:
-                cb.resampler = audio.Resampler(dev, S, P * up)
-                cb.resampler.reset(range(S), reqs[0].in_rate, reqs[0].fmt)
-            if reqs[0].speed is not None:
-                cb.stretcher = audio.TimeStretch(dev, S, P * up)
-                cb.stretcher.reset(range(S), reqs[0].speed, reqs[0].pitch)
-            if reqs[0].volume is not None:
-                cb.limiter = audio.Limiter(dev, S, P * up)
-                cb.limiter.reset(range(S), reqs[0].volume)
+            for stage, args in chain.items():
+                cb.stages[stage] = getattr(audio, stage)(dev, S, P * up)
+                cb.stages[stage].reset(range(S), *args)
             times = []
             for it in range(a.warmup + a.steps):
                 new = {s: (r, it * P, P) for s, r in enumerate(reqs)}
@@ -108,13 +99,9 @@ def main():
                     times.append(time.perf_counter() - t0)
             row = {"slots": S, "format": name, "push_audio_ms_mean": 1e3 * sum(times) / len(times),
                    "push_audio_ms_min": 1e3 * min(times)}
-            if fmt is not None:    # one step of the timed stage (its job upload and kernel) of one packet per row
-                r0 = reqs[0]
-                stage = "limit" if r0.volume is not None else "resample" if r0.in_rate != 24000 or r0.speed is None \
-                    else "stretch"
-                res = {"limit": cb.limiter, "resample": cb.resampler, "stretch": cb.stretcher}[stage]
-                fn = getattr(res.lib, {"limit": "q3_limit_step_rows", "resample": "q3_resample_step_rows",
-                                       "stretch": "q3_stretch_step_rows"}[stage])
+            if chain:    # one step of the timed stage (its job upload and kernel) of one packet per row
+                res = cb.stages[next(n for n in ("Limiter", "Resampler", "TimeStretch") if n in chain)]
+                fn = getattr(res.lib, f"q3_{res.PREFIX}_step_rows")
                 x = torch.rand(S, P * up, device=dev) * 2 - 1
                 cnt, end = (C.c_int32 * S)(*[P * up] * S), (C.c_int32 * S)()
                 nout = (C.c_int32 * S)()
@@ -129,11 +116,10 @@ def main():
                     step()
                 e1.record()
                 torch.cuda.synchronize()
-                row[stage + "_step_us"] = 1e3 * e0.elapsed_time(e1) / n
+                row[res.PREFIX + "_step_us"] = 1e3 * e0.elapsed_time(e1) / n
                 row["outputs_per_row"] = int(nout[0])
-                for obj in (cb.resampler, cb.stretcher, cb.limiter):
-                    if obj is not None:
-                        obj.close()
+            for obj in cb.stages.values():
+                obj.close()
             cb.cstream.close()
             results.append(row)
     name, power = _card()
