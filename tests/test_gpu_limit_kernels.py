@@ -3,35 +3,22 @@ against the numpy restatement (tests/limiter_ref.py), bit for bit: whole clips e
 peaks, silence, 0 … 1700 samples across the 256-output tile edges) with rows that have no work beside them; rows
 resumed mid-clip from a history at its deepest read, with their next history half; save / load records."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+from tests import audio_shims
 from tests import limiter_ref as LR
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HIST = 1536
+HIST = audio_shims.LIMIT_HIST
 DEV = "cuda:0"
 
 
 @pytest.fixture(scope="module")
 def lib(tmp_path_factory):
-    from qwen3_tts_b200 import build
-    out = str(tmp_path_factory.mktemp("limit_shim") / "liblimit_shim.so")
-    cmd = [build._nvcc()] + build.NVCC_FLAGS + ["-shared", "-I", build.CSRC,
-                                                 os.path.join(ROOT, "tests", "csrc", "limit_shim.cu"), "-o", out]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, f"shim build failed:\n{r.stdout}\n{r.stderr}"
-    L = C.CDLL(out)
-    vp, i32, i64 = C.c_void_p, C.c_int, C.c_longlong
-    pi, pl, pf = C.POINTER(C.c_int), C.POINTER(C.c_longlong), C.POINTER(C.c_float)
-    L.limit_shim_step.argtypes = [i32, pl, pl, pi, pf, vp, i64, vp, vp, i64]
-    L.limit_shim_move.argtypes = [i32, pi, pl, pi, pf, vp, i32, vp, i32]
-    return L
+    return audio_shims.load(tmp_path_factory, "limit_shim")
 
 
 def _arr(t, xs):

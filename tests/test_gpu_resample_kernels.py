@@ -3,35 +3,22 @@ here, against an fp64 reference: outputs read from the history at its deepest an
 padding past the clip, several filters and encodings in one launch, the s16 clamp and round-half-even ties, the next
 history half (zeros after an end, untouched for an idle row), and save / load records."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+from tests import audio_shims
 from tests.test_gpu_resample import _s16, _ulaw
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HIST = 128
+HIST = audio_shims.RESAMPLE_HIST
 DEV = "cuda:0"
 
 
 @pytest.fixture(scope="module")
 def lib(tmp_path_factory):
-    from qwen3_tts_b200 import build
-    out = str(tmp_path_factory.mktemp("resample_shim") / "libresample_shim.so")
-    cmd = [build._nvcc()] + build.NVCC_FLAGS + ["-shared", "-I", build.CSRC,
-                                                 os.path.join(ROOT, "tests", "csrc", "resample_shim.cu"), "-o", out]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, f"shim build failed:\n{r.stdout}\n{r.stderr}"
-    L = C.CDLL(out)
-    vp, i32, i64 = C.c_void_p, C.c_int, C.c_longlong
-    pi, pl = C.POINTER(C.c_int), C.POINTER(C.c_longlong)
-    L.resample_shim_poly.argtypes = [i32, C.POINTER(vp), pi, pi, pi, i32, pl, pl, pi, vp, i64, vp, vp, i64]
-    L.resample_shim_move.argtypes = [i32, pi, pl, pi, vp, i32, vp, i32]
-    return L
+    return audio_shims.load(tmp_path_factory, "resample_shim")
 
 
 def _arr(t, xs):

@@ -6,36 +6,23 @@ mid-clip from a history at its deepest read, with their next history, tail and f
 offset justified by the fp32 summation bound (the reference follows the kernel after a near-tie); save / load
 records."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+from tests import audio_shims
 from tests import stretch_ref as S
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HIST = 2048
+HIST = audio_shims.STRETCH_HIST
 DEV = "cuda:0"
 HOPS = (240, 360, 479, 481, 600, 960)
 
 
 @pytest.fixture(scope="module")
 def lib(tmp_path_factory):
-    from qwen3_tts_b200 import build
-    out = str(tmp_path_factory.mktemp("stretch_shim") / "libstretch_shim.so")
-    cmd = [build._nvcc()] + build.NVCC_FLAGS + ["-shared", "-I", build.CSRC,
-                                                 os.path.join(ROOT, "tests", "csrc", "stretch_shim.cu"), "-o", out]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, f"shim build failed:\n{r.stdout}\n{r.stderr}"
-    L = C.CDLL(out)
-    vp, i32, i64 = C.c_void_p, C.c_int, C.c_longlong
-    pi, pl = C.POINTER(C.c_int), C.POINTER(C.c_longlong)
-    L.stretch_shim_wsola.argtypes = [i32, pl, pl, pi, vp, vp, i64, vp, vp, vp, vp, i64]
-    L.stretch_shim_move.argtypes = [i32, pl, pl, pi, vp, vp, vp, vp, i32]
-    return L
+    return audio_shims.load(tmp_path_factory, "stretch_shim")
 
 
 def _arr(t, xs):
