@@ -483,6 +483,45 @@ int q3_limit_step_rows(q3_limiter* s, const float* in_dev, int64_t ld, const int
 int q3_limit_save_rows(q3_limiter* s, int32_t n, const int32_t* rows_host, void* dst_dev, void* stream);
 int q3_limit_load_rows(q3_limiter* s, int32_t n, const int32_t* rows_host, const void* src_dev, void* stream);
 
+/* ---------------------------------------------------------------- loudness (streaming BS.1770 normaliser)
+ * A gain towards a target integrated loudness T (LUFS), decided while the audio streams, at the codec's 24 kHz.  The
+ * input x is K-weighted (BS.1770-4 shelf then high-pass, fp32 in transposed direct form II, designed by the caller) over
+ * complete segments s = [2400s, 2400s + 2400) only; z_s is the fp64 sum of a segment's squared K-weighted samples, block
+ * j covers segments max(0, j-3) .. j with ms_j = (z_{j-3} + ... + z_j) / (2400*min(j+1, 4)) and l_j = -0.691 +
+ * 10*log10(ms_j).  When segment s completes: Ja = {j <= s : l_j > -70}; if Ja is empty A_s = A_{s-1}, else
+ * Gr = -0.691 + 10*log10(mean_Ja ms) - 10, J = {j in Ja : l_j > Gr}, I_s = -0.691 + 10*log10(mean_J ms) and
+ * A_s = fp32(10^(clamp(T - I_s, -30, 30)/20)), all in fp64; A_{-1} = A_{-2} = 1.  Output n = 2400k + i:
+ *   y[n] = x[n] * (A_{k-2} + (A_{k-1} - A_{k-2}) * fp32((i+1)/2400)),   fp32 round-to-nearest without contraction,
+ * so a clip of n samples gives n samples with no delay, and an end emits nothing more.  A clip may hold at most
+ * Q3_LOUD_MAX_BLOCKS segments (2400 * Q3_LOUD_MAX_BLOCKS samples).  A clip streamed in pushes of any sizes equals the
+ * clip pushed at once, bit for bit.
+ * open: `rows` rows; a step gives each row at most max_in (1 .. 32768) inputs; each row's output capacity is max_out fp32
+ *   samples, at least max_in.  Device memory of the object is its own.
+ * set_filter: the K-weighting, fp32 host sos[12]: two rows b0 b1 b2 a0 a1 a2 (shelf, then high-pass), a0 = 1.  Required
+ *   before the first step.
+ * reset_rows: the n rows in rows_host start new clips at target targets_host[i] (finite).  Host state only.
+ * step_rows: one launch, one CTA per row with inputs.  Row r takes counts_host[r] (0..max_in) fp32 inputs at
+ *   in_dev + r*ld and, when end_host[r] != 0, ends its clip (it then starts a new one at the same target).  Its new
+ *   outputs go to out_dev + r*max_out, their count (counts_host[r]) to nout_host[r].  A row with count 0 and no end is
+ *   untouched.  A row never reset may take neither inputs nor an end; a row whose clip would pass Q3_LOUD_MAX_BLOCKS
+ *   segments is refused.  Asynchronous on `stream`.
+ * save_rows / load_rows: as q3_resample_save_rows / load_rows, Q3_LOUD_ROW_BYTES per row: a Q3_LOUD_HEADER_BYTES header
+ *   (target fp64, inputs so far int64, A_{k-1} and A_{k-2} fp32, the filter state fp32[4], z_{k-3..k-1} fp64[3]), the
+ *   partial segment's inputs fp32[2400] and the block mean squares fp64[Q3_LOUD_MAX_BLOCKS].  load synchronises.
+ * Bad arguments are rejected before any device work and change nothing. */
+#define Q3_LOUD_MAX_BLOCKS 16384
+#define Q3_LOUD_HEADER_BYTES 64
+#define Q3_LOUD_ROW_BYTES 140736
+typedef struct q3_loudness q3_loudness;
+int q3_loud_open(int32_t rows, int32_t max_in, int32_t max_out, int32_t device, q3_loudness** out);
+void q3_loud_close(q3_loudness* s);
+int q3_loud_set_filter(q3_loudness* s, const float* sos_host);
+int q3_loud_reset_rows(q3_loudness* s, int32_t n, const int32_t* rows_host, const double* targets_host);
+int q3_loud_step_rows(q3_loudness* s, const float* in_dev, int64_t ld, const int32_t* counts_host,
+                      const int32_t* end_host, float* out_dev, int32_t* nout_host, void* stream);
+int q3_loud_save_rows(q3_loudness* s, int32_t n, const int32_t* rows_host, void* dst_dev, void* stream);
+int q3_loud_load_rows(q3_loudness* s, int32_t n, const int32_t* rows_host, const void* src_dev, void* stream);
+
 /* ---------------------------------------------------------------- speaker x-vector (voice cloning)
  * Replaces Qwen3TTSForConditionalGeneration.extract_speaker_embedding (core/models/modeling_qwen3_tts.py:1941-1954):
  * mel_spectrogram (:396-448) + Qwen3TTSSpeakerEncoder.forward (:371-393).  fp32. */

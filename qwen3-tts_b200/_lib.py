@@ -83,7 +83,9 @@ CODEC_SYMBOLS = ["q3_codec_create", "q3_codec_destroy", "q3_codec_load_tensor", 
                  "q3_stretch_open", "q3_stretch_close", "q3_stretch_set_window", "q3_stretch_reset_rows",
                  "q3_stretch_step_rows", "q3_stretch_save_rows", "q3_stretch_load_rows",
                  "q3_limit_open", "q3_limit_close", "q3_limit_reset_rows", "q3_limit_step_rows", "q3_limit_save_rows",
-                 "q3_limit_load_rows"]
+                 "q3_limit_load_rows",
+                 "q3_loud_open", "q3_loud_close", "q3_loud_set_filter", "q3_loud_reset_rows", "q3_loud_step_rows",
+                 "q3_loud_save_rows", "q3_loud_load_rows"]
 
 _lib = None
 
@@ -210,6 +212,14 @@ def load():
         lib.q3_limit_step_rows.argtypes = [vp, vp, i64, C.POINTER(i32), C.POINTER(i32), vp, C.POINTER(i32), vp]
         lib.q3_limit_save_rows.argtypes = [vp, i32, C.POINTER(i32), vp, vp]
         lib.q3_limit_load_rows.argtypes = [vp, i32, C.POINTER(i32), vp, vp]
+        lib.q3_loud_open.argtypes = [i32, i32, i32, i32, C.POINTER(vp)]
+        lib.q3_loud_close.argtypes = [vp]
+        lib.q3_loud_close.restype = None
+        lib.q3_loud_set_filter.argtypes = [vp, C.POINTER(C.c_float)]
+        lib.q3_loud_reset_rows.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(C.c_double)]
+        lib.q3_loud_step_rows.argtypes = [vp, vp, i64, C.POINTER(i32), C.POINTER(i32), vp, C.POINTER(i32), vp]
+        lib.q3_loud_save_rows.argtypes = [vp, i32, C.POINTER(i32), vp, vp]
+        lib.q3_loud_load_rows.argtypes = [vp, i32, C.POINTER(i32), vp, vp]
     _lib = lib
     return lib
 

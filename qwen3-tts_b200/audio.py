@@ -21,9 +21,10 @@ with its state, so load() adds a dropped filter again.
 
 Speaking rate: TimeStretch, a streaming per-row WSOLA time-stretch at 24 kHz (q3_stretch_*, csrc/stretch.cu, DESIGN
 §4.7).  Volume: Limiter, a streaming per-row look-ahead limiter at 24 kHz (q3_limit_*, csrc/limit.cu, DESIGN §4.8).
+Loudness: Loudness, a streaming per-row BS.1770 loudness normaliser at 24 kHz (q3_loud_*, csrc/loud.cu, DESIGN §4.9).
 
-The three are row stages (_RowStage) with one streaming contract, and stages(fmt) is the chain of them, in the order
-time-stretch, limiter, resampler, that turns the codec's audio into a client's AudioFormat.
+The four are row stages (_RowStage) with one streaming contract, and stages(fmt) is the chain of them, in the order
+time-stretch, loudness, limiter, resampler, that turns the codec's audio into a client's AudioFormat.
 """
 import ctypes as C
 from dataclasses import dataclass
@@ -479,14 +480,75 @@ class Limiter(_RowStage):
         self._reset(rows, (C.c_float * len(rows))(*[g] * len(rows)))
 
 
-STAGES = ("TimeStretch", "Limiter", "Resampler")   # the stage classes above, in the order a stream runs them
+class Loudness(_RowStage):
+    """`rows` streaming loudness normaliser rows at the codec's 24 kHz on `device` (q3_loud_*, csrc/loud.cu, DESIGN
+    §4.9): a gain towards a target integrated loudness in LUFS, measured while the audio streams.  The input is K-weighted
+    (k_weighting(), BS.1770-4) over 100 ms segments; when a segment completes, the gated loudness of the clip so far
+    (blocks of the last four segments, the -70 LUFS and -10 LU gates) gives the gain A_s = 10^(clamp(target - I_s, -30,
+    30)/20), and the samples of segment k ramp linearly from A_{k-2} to A_{k-1}.  So the first 100 ms pass at unity gain,
+    silence holds the last gain, and there is no delay: a clip of n samples gives n samples, emitted(n) = n.  A clip may
+    hold at most MAX_BLOCKS segments.  A push gives each row at most `max_in` samples per launch (longer pushes take
+    several launches).  reset(rows, target) starts new clips; push({row: samples}, end=rows) returns {row: float32 numpy
+    array of the row's new output}; push_device keeps them on the device; save(rows) / load(rows, state) move rows'
+    state; oneshot(x, target) normalises a whole clip.  A clip pushed in pieces of any sizes and ended equals oneshot()
+    of the whole clip bit for bit.  A raised gain can clip: the batcher always runs the Limiter after it."""
+
+    SEG = 2400                        # samples per segment (100 ms)
+    MAX_BLOCKS = 16384                # Q3_LOUD_MAX_BLOCKS: segments one clip may hold (27 min 18.4 s)
+    PREFIX, NAME = "loud", "loudness normaliser"
+    ROW_BYTES = 140736                # Q3_LOUD_ROW_BYTES: one row's saved state
+    MAX_IN = 32768                    # the largest max_in the native stage takes
+
+    @staticmethod
+    def k_weighting(fs: int = CODEC_RATE) -> np.ndarray:
+        """The BS.1770-4 K-weighting at `fs` as fp64 second-order sections (2, 6), rows b0 b1 b2 a0 a1 a2: the shelf,
+        then the high-pass, by libebur128's bilinear design (uploaded as fp32)."""
+        def section(f0, q, vh, vb):
+            k = np.tan(np.pi * f0 / fs)
+            a0 = 1 + k / q + k * k
+            a = [1.0, 2 * (k * k - 1) / a0, (1 - k / q + k * k) / a0]
+            if vh is None:
+                return [1.0, -2.0, 1.0] + a
+            return [(vh + vb * k / q + k * k) / a0, 2 * (k * k - vh) / a0, (vh - vb * k / q + k * k) / a0] + a
+        vh = 10 ** (3.999843853973347 / 20)
+        return np.array([section(1681.974450955533, 0.7071752369554196, vh, vh ** 0.4996667741545416),
+                         section(38.13547087602444, 0.5003270373238773, None, None)])
+
+    @staticmethod
+    def emitted(n: int) -> int:
+        """Outputs a row has emitted after n inputs without an end: n."""
+        return n
+
+    @staticmethod
+    def total(n: int) -> int:
+        """Outputs of a whole clip of n inputs: n."""
+        return n
+
+    def __init__(self, device, rows: int, max_in: int):
+        super().__init__(device, rows, max_in)
+        sos = self.k_weighting().astype(np.float32).ravel()
+        _lib.check(self.lib.q3_loud_set_filter(self.h, (C.c_float * 12)(*sos)))
+
+    def _max_out(self) -> int:
+        if not 1 <= self.max_in <= self.MAX_IN:
+            raise ValueError(f"max_in {self.max_in} outside [1, {self.MAX_IN}]")
+        return self.max_in
+
+    def reset(self, rows, target):
+        """Start new clips in `rows` normalised towards `target` LUFS (AudioFormat's loudness range)."""
+        rows = check_rows(rows, self.rows)
+        t = AudioFormat(CODEC_RATE, loudness=target).loudness
+        self._reset(rows, (C.c_double * len(rows))(*[t] * len(rows)))
+
+
+STAGES = ("TimeStretch", "Loudness", "Limiter", "Resampler")   # the stage classes above, in the order a stream runs them
 
 
 def stages(fmt: Optional[AudioFormat]) -> Tuple[Tuple[str, tuple], ...]:
     """The stages the codec's audio runs through to come out in `fmt`, in STAGES order, each as (its class's name in
     this module, the arguments its reset takes after the rows): the time-stretch when the hop is not 480, (speed, pitch)
-    when the pitch step Lp is not 480 and (speed,) (pitch 0) when it is; the limiter (volume,) at a volume other than
-    0 dB; the resampler (50*Lp, AudioFormat(rate, encoding)) when Lp is not 480 or the rate or encoding is not 24 kHz
+    when the pitch step Lp is not 480 and (speed,) (pitch 0) when it is; the loudness normaliser (loudness,) with a
+    loudness target; the limiter (volume,) at a volume other than 0 dB, and always after a loudness target; the resampler (50*Lp, AudioFormat(rate, encoding)) when Lp is not 480 or the rate or encoding is not 24 kHz
     float32.  () for None (the codec's own audio)."""
     if fmt is None:
         return ()
@@ -496,7 +558,9 @@ def stages(fmt: Optional[AudioFormat]) -> Tuple[Tuple[str, tuple], ...]:
     chain = []
     if fmt.hop != 480:
         chain.append(("TimeStretch", (fmt.speed, fmt.pitch) if pitched else (fmt.speed,)))
-    if fmt.volume != 0:
+    if fmt.loudness is not None:
+        chain.append(("Loudness", (fmt.loudness,)))
+    if fmt.volume != 0 or fmt.loudness is not None:
         chain.append(("Limiter", (fmt.volume,)))
     if pitched or out != AudioFormat(CODEC_RATE):
         chain.append(("Resampler", (50 * fmt.pitch_step, out)))

@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libqwen3tts_b200.so")
 SOURCES = ["ar_engine.cu", "codec_engine.cu", "codec_encoder.cu", "speaker_encoder.cu", "conv_f32.cu", "gemm_sm90.cu",
-           "resample.cu", "stretch.cu", "limit.cu"]
+           "resample.cu", "stretch.cu", "limit.cu", "loud.cu"]
 NVCC_FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-cudart", "shared", "--expt-relaxed-constexpr"]
 

@@ -5,7 +5,7 @@ import math
 import numbers
 import operator
 from dataclasses import dataclass, field
-from typing import Tuple
+from typing import Optional, Tuple
 
 
 @dataclass
@@ -197,6 +197,7 @@ ENCODINGS = ("f32", "s16", "ulaw")
 SPEED_RANGE = (0.5, 2.0)
 PITCH_RANGE = (-12.0, 12.0)    # semitones
 VOLUME_RANGE = (-30.0, 12.0)   # dB
+LOUDNESS_RANGE = (-40.0, -10.0)   # LUFS
 
 
 def _real_in(name: str, v, lo: float, hi: float) -> float:
@@ -211,13 +212,16 @@ class AudioFormat:
     "ulaw" 8-bit G.711 mu-law (uint8).  Rates: SUPPORTED_RATES.  `speed`: a real number in SPEED_RANGE, the pace of the
     speech (1.25 is 25 % faster, same pitch; audio.TimeStretch, resolution 1/480).  `pitch`: semitones in PITCH_RANGE
     (time-stretch, then rate conversion from 50*pitch_step Hz; formants move with it).  `volume`: dB in VOLUME_RANGE
-    through audio.Limiter, peaks held at -1 dBFS.  speed / (pitch_step/480) must lie in [0.5, 2] (hop in [240, 960]).
-    Anything else raises ValueError on construction."""
+    through audio.Limiter, peaks held at -1 dBFS.  `loudness`: None, or a target integrated loudness in LUFS in
+    LOUDNESS_RANGE through audio.Loudness (BS.1770 gated loudness measured while the audio streams), always followed by
+    the limiter at `volume`.  speed / (pitch_step/480) must lie in [0.5, 2] (hop in [240, 960]).  Anything else raises
+    ValueError on construction."""
     sample_rate: int
     encoding: str = "f32"
     speed: float = 1.0
     pitch: float = 0.0
     volume: float = 0.0
+    loudness: Optional[float] = None
 
     def __post_init__(self):
         try:
@@ -232,6 +236,8 @@ class AudioFormat:
         object.__setattr__(self, "speed", _real_in("speed", self.speed, *SPEED_RANGE))
         object.__setattr__(self, "pitch", _real_in("pitch", self.pitch, *PITCH_RANGE))
         object.__setattr__(self, "volume", _real_in("volume", self.volume, *VOLUME_RANGE))
+        if self.loudness is not None:
+            object.__setattr__(self, "loudness", _real_in("loudness", self.loudness, *LOUDNESS_RANGE))
         if not 240 <= self.hop <= 960:
             raise ValueError(f"speed {self.speed} at pitch {self.pitch} gives a time-stretch hop of {self.hop}: speed "
                              f"divided by the pitch factor {self.pitch_step}/480 must lie in [0.5, 2]")

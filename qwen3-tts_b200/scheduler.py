@@ -61,9 +61,10 @@ the request is not admitted, takes no slot a park would free, and does not keep 
 admitted and runs as any live request, so it generates what its whole text gives up front (tests/test_gpu_live_clone.py).
 
 Audio formats (`ContinuousBatcher(audio_format=)` for the session, `submit(audio_format=)` per request, an AudioFormat
-of rate, encoding, speed, pitch and volume): a request's audio runs through the chain of stages audio.stages gives its
-format, in order a time-stretch (a speed or pitch), a limiter (a volume) and a resampler (a pitch, or a rate or
-encoding other than 24 kHz float32); a request in the codec's own format has none.  Each stage is one object of
+of rate, encoding, speed, pitch, volume and loudness): a request's audio runs through the chain of stages audio.stages
+gives its format, in order a time-stretch (a speed or pitch), a loudness normaliser (a loudness target), a limiter (a
+volume, or a loudness target) and a resampler (a pitch, or a rate or encoding other than 24 kHz float32); a request in
+the codec's own format has none.  Each stage is one object of
 `n_slots` rows, opened when the first request that uses it is admitted, and a request has a row in each stage of its
 chain, in its slot.  The rows are reset at admission after the codec row's reset, seed or bank copy (they shape the
 generated part only), one reset per stage and setting; saved on the request when it is parked, loaded into its new
@@ -71,10 +72,13 @@ slot when it is resumed, and dropped with it on cancel.  After each codec push o
 that uses it, the samples going from stage to stage on the device; a request that finished in the step ends its row in
 each stage, so each stage's tail goes on into the next stage's end in the same step (even with no new frame), and
 stream() yields its chunk as float32, int16 or uint8.  A request's concatenated chunks equal
-    Resampler.oneshot(Limiter.oneshot(TimeStretch.oneshot(w, speed, pitch), volume), 50*Lp, AudioFormat(rate, encoding))
+    Resampler.oneshot(Limiter.oneshot(Loudness.oneshot(TimeStretch.oneshot(w, speed, pitch), target), volume), 50*Lp,
+                      AudioFormat(rate, encoding))
 bit for bit, w its whole waveform, Lp its pitch step and each stage skipped when its chain has none
-(tests/test_gpu_scheduler_audio_format.py, test_gpu_scheduler_speed.py, test_gpu_scheduler_pitch_volume.py).  A session
-without formats opens no stage and makes the same calls as before.
+(tests/test_gpu_scheduler_audio_format.py, test_gpu_scheduler_speed.py, test_gpu_scheduler_pitch_volume.py,
+test_gpu_scheduler_loudness.py).  A loudness request whose longest possible audio (its horizon's samples, stretched)
+passes Loudness.MAX_BLOCKS segments is refused at submit.  A session without formats opens no stage and makes the
+same calls as before.
 """
 from collections import deque
 from dataclasses import dataclass, field
@@ -113,6 +117,7 @@ class _Request:
     saved: Dict[str, Any] = field(default_factory=dict)     # while parked: {stage name: its row's saved state}
     # while parked: its row's saved state in each stage, None without a row there
     st_state = property(lambda self: self.saved.get("TimeStretch"))
+    loud_state = property(lambda self: self.saved.get("Loudness"))
     lim_state = property(lambda self: self.saved.get("Limiter"))
     res_state = property(lambda self: self.saved.get("Resampler"))
 
@@ -163,6 +168,7 @@ class ContinuousBatcher:
 
     # each stage of `stages`, None until the first request that uses it is admitted
     stretcher = property(lambda self: self.stages.get("TimeStretch"))
+    loudness = property(lambda self: self.stages.get("Loudness"))
     limiter = property(lambda self: self.stages.get("Limiter"))
     resampler = property(lambda self: self.stages.get("Resampler"))
 
@@ -251,6 +257,13 @@ class ContinuousBatcher:
         horizon = min(limit if max_frames is None else max_frames, limit, room)
         if self.codec is not None:
             horizon = min(horizon, self.codec.max_frames - L_ref)  # a codec row's position may not pass its RoPE table
+        if "Loudness" in chain:
+            fmt = audio_format if audio_format is not None else self.audio_format
+            n = audio.TimeStretch.total(horizon * self.codec.total_upsample, fmt.hop)
+            if n > audio.Loudness.MAX_BLOCKS * audio.Loudness.SEG:
+                raise ValueError(f"a loudness target measures at most {audio.Loudness.MAX_BLOCKS} segments of "
+                                 f"{audio.Loudness.SEG} samples, and this request may stream {n} samples: lower "
+                                 f"max_frames")
         r = _Request(rid, inputs_embeds, tr, horizon, sampling, ref_codes, voice, text_open=bool(text_open),
                      overlay=overlay if K else None, chain=chain)
         if r.overlay is not None:

@@ -5,10 +5,12 @@ float32.  With --speed, the same for every row at each of the given speaking rat
 time-stretch runs), and the time-stretch step (CUDA events around q3_stretch_step_rows calls of one packet per row)
 instead of the resampler's.  With --pitch, every row at each of the given pitches (24 kHz float32: the time-stretch
 and the pitched resampler run), timing the pitched resampler step; with --volume, every row at each of the given
-volumes (only the limiter runs), timing the limiter step.  Prints one JSON line, with the card's name and power limit
+volumes (only the limiter runs), timing the limiter step; with --loudness, every row at each of the given loudness
+targets (the loudness normaliser and the limiter run), timing the loudness step.  Prints one JSON line, with the card's name and power limit
 read in the same run.
 
     python tools/format_probe.py [--steps 60] [--warmup 10] [--speed 0.5 1.25 2.0] [--pitch -7 3] [--volume 6 -6]
+                                 [--loudness -16]
 """
 import argparse
 import ctypes as C
@@ -55,6 +57,7 @@ def main():
     ap.add_argument("--speed", type=float, nargs="*", default=None)
     ap.add_argument("--pitch", type=float, nargs="*", default=None)
     ap.add_argument("--volume", type=float, nargs="*", default=None)
+    ap.add_argument("--loudness", type=float, nargs="*", default=None)
     a = ap.parse_args()
     import torch
     import qwen3_tts_b200 as q
@@ -68,10 +71,11 @@ def main():
     dec = CodecDecoder(ccfg, synthetic.random_codec_weights(ccfg, device="cpu", seed=0), device=dev, max_frames=1024)
     P, up = 4, dec.total_upsample
     formats = {"default": None, "8k_ulaw": q.AudioFormat(8000, "ulaw"), "48k_f32": q.AudioFormat(48000, "f32")}
-    if a.speed or a.pitch or a.volume:
+    if a.speed or a.pitch or a.volume or a.loudness:
         formats = {"default": None, **{f"speed_{sp}": q.AudioFormat(24000, speed=sp) for sp in a.speed or ()},
                    **{f"pitch_{p}": q.AudioFormat(24000, pitch=p) for p in a.pitch or ()},
-                   **{f"volume_{v}": q.AudioFormat(24000, volume=v) for v in a.volume or ()}}
+                   **{f"volume_{v}": q.AudioFormat(24000, volume=v) for v in a.volume or ()},
+                   **{f"loudness_{t}": q.AudioFormat(24000, loudness=t) for t in a.loudness or ()}}
     results = []
     g = torch.Generator().manual_seed(0)
     for S in (8, 32):
@@ -100,7 +104,7 @@ def main():
             row = {"slots": S, "format": name, "push_audio_ms_mean": 1e3 * sum(times) / len(times),
                    "push_audio_ms_min": 1e3 * min(times)}
             if chain:    # one step of the timed stage (its job upload and kernel) of one packet per row
-                res = cb.stages[next(n for n in ("Limiter", "Resampler", "TimeStretch") if n in chain)]
+                res = cb.stages[next(n for n in ("Loudness", "Limiter", "Resampler", "TimeStretch") if n in chain)]
                 fn = getattr(res.lib, f"q3_{res.PREFIX}_step_rows")
                 x = torch.rand(S, P * up, device=dev) * 2 - 1
                 cnt, end = (C.c_int32 * S)(*[P * up] * S), (C.c_int32 * S)()
